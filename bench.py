@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — driver contract: `python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload NAME]`.
+"""bench.py — `python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload NAME] [--dump-outputs DIR]`.
 
 Prints ONE JSON line (rank 0).  A "step" = one pass of the hot path over one batch of synthetic images per GPU.
 
@@ -9,12 +9,17 @@ Workloads (BASELINE.json configs):
   zoedepth_nk768    zoedepth_nk @768 (pad + flip TTA, 64 core forwards) + red-cyan anaglyph, batch 32/GPU (configs[3])
   stereo2048        normalise -> stereo SBS (div 2.5, polylines_sharp) -> normal map on 2048x2048, batch 16/GPU
                     (north_star's "2048x2048 stereo warp" HBM-roofline target)
-The default run (depth_beit512) carries the other three as `sub_benchmarks`, so one driver run covers BASELINE's
+The default run (depth_beit512) carries the other three as `sub_benchmarks`, so one run covers BASELINE's
 "depth+stereo 512^2 & 2048^2"; `e2e_funnel` is the same workload through core_generation_funnel with PIL images in and out.
 
 `value` = images/s with inputs resident in HBM; `e2e` = same through the public batched API from pinned HOST buffers,
-H2D and D2H inside the timed region; `roofline` = dominant kernel vs MEASURED_PEAKS.json; `cpu_baseline` = the oracle
+H2D and D2H inside the timed region; `roofline` = dominant kernel vs the peaks of `_peaks()`; `cpu_baseline` = the oracle
 (C restatement of the reference's CPU path) timed on this box's host cores on a bounded sample.
+
+`--dump-outputs DIR` writes what the last timed step returned (the arrays a caller of the timed path receives) as
+DIR/<name>.npy in float32, at most 64 MB (64e6 bytes, file headers included) in all: an output over its share of that is
+reduced to a fixed, seeded sample of its elements.  Inputs and weights are seeded, so two builds run with the same arguments can be compared output for output.
+The benchmark loads the library that `__graft_entry__.build()` left in the tree and writes nothing there.
 """
 from __future__ import annotations
 
@@ -38,11 +43,12 @@ def _peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"], "bf16_tflops_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]), "source": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+    # NVIDIA's data sheet for the H100 SXM at 700 W (dense fp16 / bf16); a power-limited card sustains less
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "H100 SXM data sheet"}
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (read-only queries)."""
 
     def __init__(self, gpu_index):
         self.f = tempfile.NamedTemporaryFile("w+", suffix=".csv", delete=False)
@@ -105,6 +111,7 @@ class Stereo2048:
     B = 16
     dtype = "f64"  # the stereo / normal-map arithmetic type (fp64, truncating to u8); normalise is f32
     fill = "polylines_sharp"
+    output_names = ("depth", "sbs", "normal")
     launches_per_step = 3 + 3 + 1  # normalise (init, minmax, quantise) + stereo (init, minmax, row) + normal map
 
     def __init__(self, dev, rank):
@@ -120,7 +127,7 @@ class Stereo2048:
     def config(self):
         return {"workload": "synthetic 2048x2048 RGB + float32 prediction -> u16 depth -> SBS stereo (divergence 2.5, "
                             "polylines_sharp) -> normal map (Sobel 3)", "batch_per_gpu": self.B, "height": self.H,
-                "width": self.W, "l2_policy": "inputs+outputs per step (1.0 GB) exceed the 126 MB L2"}
+                "width": self.W, "l2_policy": "inputs+outputs per step (1.0 GB) exceed the 50 MB L2"}
 
     def step(self, rgb, pred, time_kernel=False):
         import torch
@@ -157,8 +164,7 @@ class Stereo2048:
         achieved = alg / (kernel_ms * 1e-3) / 1e9
         return {"bound": "hbm", "kernel": "stereo_row_kernel (+ u16 min/max pre-pass)", "achieved": achieved,
                 "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": achieved / peaks["hbm_gbs"],
-                # dram read + write of the row kernel for this batch (profiles/r01_ncu_stereo2048.txt): no re-reads
-                "traffic": 692.5e6 if (self.B == 16 and self.fill == "polylines_sharp") else None, "traffic_unit": "bytes/launch (ncu --set full)",
+                "traffic": None,
                 "peak_source": peaks["source"], "algorithmic_bytes_per_launch": alg, "kernel_ms": kernel_ms,
                 "note": "exact-fp64 polylines is FP64/latency bound, not HBM bound; see DESIGN.md"}
 
@@ -208,6 +214,25 @@ def pick_torch_threads(limit):
             best, best_t = n, dt
     torch.set_num_threads(best)
     return best
+
+
+DUMP_LIMIT_BYTES = 64 * 10 ** 6      # of the files as written, .npy headers included
+NPY_HEADER_BYTES = 4096              # reserved per file; numpy's header for these arrays is 128 bytes
+
+
+def dump_outputs(directory, names, outs, limit_bytes=DUMP_LIMIT_BYTES):
+    """Write `outs` (device tensors or arrays) as <directory>/<name>.npy in float32.  The files together stay within
+    limit_bytes: the limit, less a reserve for the headers, is shared equally, and an output over its share is reduced to
+    the elements at fixed indices drawn from a generator seeded by the output's position (sorted, no repeats), so the same
+    elements are written by every run and every build."""
+    os.makedirs(directory, exist_ok=True)
+    share = (limit_bytes // max(len(outs), 1) - NPY_HEADER_BYTES) // 4
+    for i, o in enumerate(outs):
+        a = np.asarray(o.detach().to("cpu").numpy() if hasattr(o, "detach") else o).astype(np.float32)
+        if a.size > share:
+            idx = np.sort(np.random.default_rng(1234 + i).choice(a.size, size=share, replace=False))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(directory, f"{names[i] if i < len(names) else f'out{i}'}.npy"), a)
 
 
 class GraphedStep:
@@ -354,7 +379,7 @@ def measure(wl, args, world, dev, rank, local_rank, peaks, steps, with_cpu_basel
     import torch
     import torch.distributed as dist
     if hasattr(wl, "measure"):       # a workload with its own step structure (BOOST: one image, patch-parallel, strong scaling)
-        return wl.measure(args, world, dev, rank, local_rank, peaks, steps, with_cpu_baseline, ClockSampler)
+        return wl.measure(args, world, dev, rank, local_rank, peaks, steps, with_cpu_baseline, ClockSampler, dump_outputs)
     graphed = None
     if not args.no_graph:
         graphed = GraphedStep(lambda: wl.step_resident(False))
@@ -379,8 +404,9 @@ def measure(wl, args, world, dev, rank, local_rank, peaks, steps, with_cpu_basel
     sampler = ClockSampler(local_rank) if rank == 0 else None
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
+    outs = None
     for _ in range(steps):
-        full_step(time_kernel=False)
+        outs = full_step(time_kernel=False)
     if gatherer is not None:
         gatherer.drain()
     e1.record()
@@ -393,6 +419,8 @@ def measure(wl, args, world, dev, rank, local_rank, peaks, steps, with_cpu_basel
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
     ms_step = float(t.item()) / steps
+    if rank == 0 and args.dump_outputs and outs is not None:
+        dump_outputs(args.dump_outputs, getattr(wl, "output_names", ()), outs)
 
     # ---- dominant-kernel probe: same kernels, eager, CUDA events around the launches (events cannot be captured) ----
     roofline = None
@@ -468,7 +496,8 @@ SUB_WORKLOADS = {"depth_beit512": ["stereo2048", "dav2_stereo", "zoedepth_nk768"
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--steps", type=int, default=10, help="timed steps of the workload and of each sub-benchmark; --impl reference "
+                    "runs fewer when they would not fit its time budget and reports the number it ran in `steps`")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--workload", default=DEFAULT_WORKLOAD, choices=sorted(WORKLOADS))
@@ -476,7 +505,11 @@ def main():
     ap.add_argument("--no-sub", action="store_true", help="skip the sub-benchmarks (stereo2048, dav2_stereo) of the default run")
     ap.add_argument("--no-funnel", action="store_true", help="skip the core_generation_funnel (PIL in / PIL out) end-to-end measurement")
     ap.add_argument("--no-graph", action="store_true", help="launch every kernel eagerly instead of replaying a CUDA graph")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step of --workload as DIR/<name>.npy (float32, at most 64 MB in all)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
 
     rank = int(os.environ.get("RANK", "0"))
@@ -496,11 +529,8 @@ def main():
         import datetime
         dist.init_process_group("nccl", device_id=dev, timeout=datetime.timedelta(minutes=5))
 
-    import __graft_entry__ as ge
-    if rank == 0:
-        ge.build()
-    if world > 1:
-        dist.barrier()
+    from depthmap_b200 import _lib
+    _lib.load()                            # the library build() left in the tree; a missing one is an error, nothing is compiled here
     peaks = _peaks()
     wl = WORKLOADS[args.workload](dev, rank)
     line = measure(wl, args, world, dev, rank, local_rank, peaks, args.steps, not args.no_cpu_baseline, not args.no_funnel)
@@ -513,7 +543,8 @@ def main():
             torch.cuda.empty_cache()
             try:
                 wl = WORKLOADS[name](dev, rank)
-                sub = measure(wl, args, world, dev, rank, local_rank, peaks, max(2, min(args.steps, 5)), not args.no_cpu_baseline, False)
+                sub_args = argparse.Namespace(**dict(vars(args), dump_outputs=None))
+                sub = measure(wl, sub_args, world, dev, rank, local_rank, peaks, args.steps, not args.no_cpu_baseline, False)
                 sub["workload"] = name
                 subs.append(sub)
             except Exception as e:  # noqa: BLE001

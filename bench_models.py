@@ -65,8 +65,8 @@ class _NetWorkload:
         f = self.fc1_flops / (pr["fc1_ms"] * 1e-3) / 1e12
         share = pr["attn_ms_per_launch"] * pr["attn_launches"] / pr["forward_ms"]
         return {"bound": "tensor", "kernel": self.ATTN_KERNEL, "achieved": a, "peak": peaks["bf16_tflops"], "unit": "TFLOP/s",
-                "frac": a / peaks["bf16_tflops"], "traffic": None, "traffic_note": "see profiles/r02_ncu_attention_fwd4.txt (one ncu --set full capture per kernel)",
-                "peak_source": peaks["source"] + " (cuBLAS bf16 burst)", "algorithmic_flops_per_launch": attn_flops,
+                "frac": a / peaks["bf16_tflops"], "traffic": None,
+                "peak_source": peaks["source"], "algorithmic_flops_per_launch": attn_flops,
                 "kernel_ms": pr["attn_ms_per_launch"], "launches_per_step": pr["attn_launches"],
                 "share_of_step": share, "share_note": "attention launches per forward x kernel time / forward time of the model handle, all CUDA events, this run",
                 "secondary": {"kernel": self.FC1_KERNEL, "achieved": f, "frac": f / peaks["bf16_tflops"], "kernel_ms": pr["fc1_ms"],
@@ -113,10 +113,11 @@ class Dav2Stereo(_NetWorkload):
     B = 64
     dtype = "fp16"  # tensor-core operands fp16, fp32 accumulate / residual stream (the reference's GPU path is .half())
     fill = "polylines_sharp"
+    output_names = ("depth", "sbs", "normal")
     FLOP_PER_IMAGE = 1304.2e9  # SURVEY §8d, cross-checked there against FlopCounterMode on the reference module
     MODEL_TYPE = 14
-    ATTN_KERNEL = "attention_fwd4_kernel<0> (fused softmax(QK^T)V, tcgen05 + TMEM, N = 1370, 16 heads x 64)"
-    FC1_KERNEL = "gemm_tcgen05_2sm_kernel (cta_group::2, 256x256 tile pair; block-0 MLP fc1: M=B*1370, N=4096, K=1024, GELU epilogue)"
+    ATTN_KERNEL = "attention_wgmma_kernel<0> (fused softmax(QK^T)V, wgmma, N = 1370, 16 heads x 64)"
+    FC1_KERNEL = "gemm_wgmma_kernel<128> (128x128 tiles; block-0 MLP fc1: M=B*1370, N=4096, K=1024, GELU epilogue)"
 
     def _state_dict(self):
         from oracle import synth_weights  # synthetic checkpoint-layout weights (data generation, not compute)
@@ -148,7 +149,7 @@ class Dav2Stereo(_NetWorkload):
         return {"workload": "depth_anything_v2 vitl 518x518 -> u16 depth -> SBS stereo (divergence 2.5, polylines_sharp) -> "
                             "normal map (Sobel 3)", "batch_per_gpu": self.B, "height": self.H, "width": self.W,
                 "weights": "seeded synthetic, upstream checkpoint layout",
-                "l2_policy": "activations per step (>10 GB) far exceed the 126 MB L2"}
+                "l2_policy": "activations per step (>10 GB) far exceed the 50 MB L2"}
 
     def step(self, rgb, time_kernel=False):
         import torch
@@ -207,8 +208,9 @@ class DepthBeit512(_NetWorkload):
     dtype = "fp16"
     FLOP_PER_IMAGE = 962.7e9  # SURVEY §8d
     MODEL_TYPE = 1
-    ATTN_KERNEL = "attention_fwd4_kernel<3> (fused softmax(QK^T + rel-pos bias)V, tcgen05 + TMEM, N = 1025, 16 heads x 64; + class-row kernel)"
-    FC1_KERNEL = "gemm_tcgen05_2sm_kernel (cta_group::2, 256x256 tile pair; block-0 MLP fc1: M=B*1025, N=4096, K=1024, GELU epilogue)"
+    output_names = ("depth",)
+    ATTN_KERNEL = "attention_wgmma_kernel<2> (fused softmax(QK^T + rel-pos bias)V, wgmma, N = 1025, 16 heads x 64)"
+    FC1_KERNEL = "gemm_wgmma_kernel<128> (128x128 tiles; block-0 MLP fc1: M=B*1025, N=4096, K=1024, GELU epilogue)"
 
     def _state_dict(self):
         from oracle import synth_weights  # synthetic checkpoint-layout weights (data generation, not compute)
@@ -237,7 +239,7 @@ class DepthBeit512(_NetWorkload):
     def config(self):
         return {"workload": "dpt_beit_large_512 (MiDaS 3.1) 512x512 -> float32 prediction -> u16 depth", "batch_per_gpu": self.B,
                 "height": self.H, "width": self.W, "weights": "seeded synthetic, MiDaS checkpoint layout",
-                "l2_policy": "activations per step (>5 GB) far exceed the 126 MB L2"}
+                "l2_policy": "activations per step (>5 GB) far exceed the 50 MB L2"}
 
     def step(self, rgb, time_kernel=False):
         import torch
@@ -290,8 +292,9 @@ class ZoeAnaglyph(_NetWorkload):
     dtype = "fp16"
     NET_W, NET_H = 384, 512
     FLOP_PER_IMAGE = 2 * 962.7e9 + 2 * 10e9      # SURVEY 8d: two core forwards at 512x512 + the metric head (~1%)
-    ATTN_KERNEL = "attention_fwd4_kernel<3> (fused softmax(QK^T + rel-pos bias)V of the BEiT-L-384 core at a 32x32 window, 64 forwards)"
-    FC1_KERNEL = "gemm_tcgen05_2sm_kernel (block MLP fc1: M=64*1025, N=4096, K=1024, GELU epilogue)"
+    output_names = ("depth", "anaglyph")
+    ATTN_KERNEL = "attention_wgmma_kernel<2> (fused softmax(QK^T + rel-pos bias)V of the BEiT-L-384 core at a 32x32 window, 64 forwards)"
+    FC1_KERNEL = "gemm_wgmma_kernel<128> (block MLP fc1: M=64*1025, N=4096, K=1024, GELU epilogue)"
 
     def _state_dict(self):
         from oracle import beit_dpt, synth_weights
@@ -324,7 +327,7 @@ class ZoeAnaglyph(_NetWorkload):
         return {"workload": "zoedepth_nk (DPT-BEiT-L-384 core + metric head, pad + flip TTA) 768x768 -> u16 depth -> red-cyan anaglyph "
                             "(divergence 2.5, polylines_sharp)", "batch_per_gpu": self.B, "height": self.H, "width": self.W,
                 "net": "384x512 (UI default) -> 512x512 for the padded 884x884 input", "weights": "seeded synthetic, ZoeD_M12_NK checkpoint layout",
-                "l2_policy": "activations per step (>20 GB) far exceed the 126 MB L2"}
+                "l2_policy": "activations per step (>20 GB) far exceed the 50 MB L2"}
 
     def step(self, rgb, time_kernel=False):
         from depthmap_b200.core import normalize_prediction_batch
@@ -410,9 +413,9 @@ class BoostRes101:
     def config(self):
         return {"workload": "BOOST: LeReS res101 double estimation + pix2pix merge net, 2048x2048 -> 2048x2048 fp32 depth", "images_per_step": 1,
                 "height": self.H, "width": self.W, "boost_rmax": self.RMAX, "weights": "seeded synthetic, res101.pth / latest_net_G.pth layouts",
-                "l2_policy": "per-image activations (several GB) far exceed the 126 MB L2"}
+                "l2_policy": "per-image activations (several GB) far exceed the 50 MB L2"}
 
-    def measure(self, args, world, dev, rank, local_rank, peaks, steps, with_cpu_baseline, ClockSampler):
+    def measure(self, args, world, dev, rank, local_rank, peaks, steps, with_cpu_baseline, ClockSampler, dump_outputs):
         import torch
         import torch.distributed as dist
         from PIL import Image
@@ -431,10 +434,13 @@ class BoostRes101:
         sampler = ClockSampler(local_rank) if rank == 0 else None
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
+        out = None
         for _ in range(steps):
-            self.pipe.run(self.rgb, self.RMAX, group=group, precomputed=plan, to_host=False)
+            out = self.pipe.run(self.rgb, self.RMAX, group=group, precomputed=plan, to_host=False)
         e1.record()
         torch.cuda.synchronize()
+        if rank == 0 and getattr(args, "dump_outputs", None):
+            dump_outputs(args.dump_outputs, ("depth",), [out])
         if world > 1:
             dist.barrier()
         clocks = sampler.stop() if sampler else None

@@ -1,5 +1,5 @@
 /*
- * depthmap_b200 — C-ABI of the B200-native depth -> 16-bit depth -> stereo / normal-map hot path.
+ * depthmap_b200 — C-ABI of the H100-native depth -> 16-bit depth -> stereo / normal-map hot path.
  *
  * Every entry point replaces one Python-level operator of thygate/stable-diffusion-webui-depthmap-script
  * (reference @ e4df29bc); the reference has no FFI of its own, so the binding a maintainer adds is the ctypes stub
@@ -125,7 +125,7 @@ int dm_normalmap(const uint16_t *depth, int B, int H, int W, int pre_blur, int s
 enum { DM_EPI_STORE_F16 = 0, DM_EPI_RESID_F32 = 1, DM_EPI_PIXSHUF = 2, DM_EPI_HEAD = 3, DM_EPI_STORE_F32 = 4 };
 enum { DM_ACT_NONE = 0, DM_ACT_GELU = 1, DM_ACT_RELU = 2 };
 
-/* C[M,N] = A[M,K] * W[N,K]^T with a fused epilogue (tcgen05 tensor cores, TMA-fed).  K % 64 == 0, N % 32 == 0. */
+/* C[M,N] = A[M,K] * W[N,K]^T with a fused epilogue (wgmma tensor cores, TMA-fed).  K % 64 == 0, N % 32 == 0. */
 typedef struct dm_gemm_desc {
     int32_t M, N, K;
     int32_t epi, act;        /* DM_EPI_*, DM_ACT_* */
@@ -154,11 +154,9 @@ int dm_conv3x3_f16(const void *act, int B, int H, int W, int Cin, const void *Wt
 int dm_attention_f16(const void *qkv, int B, int N, int H, float scale, const void *bias, int bias_ld, void *out, void *stream);
 /* Same, with the BEiT relative-position bias generated on the fly (dmidas/backbones/beit.py:29-62): rel_table_log2e is
  * fp32 [H, nrd] = the per-head bias table already resized to the gh x gw window, multiplied by log2(e);
- * nrd = (2gh-1)(2gw-1)+3, N = gh*gw+1 tokens (class token first).  No [H,N,N] bias tensor is read by the kernel.
- * rel_rowmax_log2e (fp32 [H, N], the per-query maximum of the bias) was an input of the round-1 kernel; the current kernel computes
- * exact row maxima itself and ignores it: pass NULL (the parameter stays for ABI stability). */
+ * nrd = (2gh-1)(2gw-1)+3, N = gh*gw+1 tokens (class token first).  No [H,N,N] bias tensor is read by the kernel. */
 int dm_attention_relpos_f16(const void *qkv, int B, int gh, int gw, int H, float scale, const float *rel_table_log2e,
-                            const float *rel_rowmax_log2e, int nrd, void *out, void *stream);
+                            int nrd, void *out, void *stream);
 /* uint8 RGB [B,H,W,3] -> (cv2-style bicubic resize to net_h x net_w) -> (x/255 - mean)/std -> fp16 patch matrix
  * [B*(net_h/patch)*(net_w/patch), kpad], K ordered (c, ky, kx); network channel c reads source channel chan_map[c]. */
 int dm_preprocess_patchify(const uint8_t *rgb, int B, int H, int W, int net_h, int net_w, int patch, const float *mean_host,

@@ -151,7 +151,7 @@ def _bind_optional(L):
         L.dm_conv3x3_ex.argtypes = [vp, i32, i32, i32, i32, vp, c.POINTER(GemmDesc), vp]
     if hasattr(L, "dm_attention_f16"):
         L.dm_attention_f16.argtypes = [vp, i32, i32, i32, f32, vp, i32, vp, vp]
-        L.dm_attention_relpos_f16.argtypes = [vp, i32, i32, i32, i32, f32, vp, vp, i32, vp, vp]
+        L.dm_attention_relpos_f16.argtypes = [vp, i32, i32, i32, i32, f32, vp, i32, vp, vp]
     if hasattr(L, "dm_layernorm_f16"):
         L.dm_preprocess_patchify.argtypes = [vp, i32, i32, i32, i32, i32, i32, c.POINTER(c.c_float), c.POINTER(c.c_float),
                                              c.POINTER(c.c_int), vp, i32, vp]
@@ -214,7 +214,7 @@ def check(rc: int, what: str = ""):
 def require_cuda():
     import torch
     if not torch.cuda.is_available():
-        raise RuntimeError("depthmap_b200: no CUDA device visible; the B200 kernels have no CPU fallback")
+        raise RuntimeError("depthmap_b200: no CUDA device visible; the H100 kernels have no CPU fallback")
     return torch.device("cuda", torch.cuda.current_device())
 
 

@@ -1,4 +1,4 @@
-"""BOOST ("Boosting Monocular Depth"): estimateboost and the pix2pix merge network on the sm_100a kernels (SURVEY.md §8a row D9,
+"""BOOST ("Boosting Monocular Depth"): estimateboost and the pix2pix merge network on the sm_90a kernels (SURVEY.md §8a row D9,
 §8e patch-parallel).
 
 reference: src/depthmap_generation.py:774-941 (estimateboost), :944-953 (generatemask), :969-1024 (calculateprocessingres),
@@ -159,7 +159,7 @@ class _NullCtx:
 class UnetMergeEngine:
     """pix2pix `unet_1024` generator (2 -> 1 channels, 10 levels, norm 'none'): down = [LeakyReLU(0.2), Conv 4x4/2], up = [ReLU,
     ConvTranspose 4x4/2] with skip concatenation, tanh at the end (pix2pix/models/networks.py:444-543).  Activations stay fp32 NHWC;
-    every convolution is column building (activation fused into the gather) + the tcgen05 GEMM with fp32 output.  With
+    every convolution is column building (activation fused into the gather) + the wgmma GEMM with fp32 output.  With
     split=True (default: the reference runs this network in fp32) operands are hi + lo fp16 pairs and the GEMM depth is tripled."""
 
     CH = [(2, 64), (64, 128), (128, 256), (256, 512)] + [(512, 512)] * 6      # (in, out) of the down conv at depth d

@@ -1,4 +1,4 @@
-"""The generation funnel on B200 — drop-in for the hot-path part of the reference's ``src/core.py``.
+"""The generation funnel on H100 — drop-in for the hot-path part of the reference's ``src/core.py``.
 
 Kept verbatim from the reference: the generator contract of ``core_generation_funnel`` (src/core.py:83 — alias
 ``run_depthmap``, its historical name): ``(outpath, inputimages, inputdepthmaps, inputnames, inp, ops=None)`` ->

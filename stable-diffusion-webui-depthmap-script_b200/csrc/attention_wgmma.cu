@@ -1,0 +1,273 @@
+// Fused multi-head attention forward for the ViT backbones (head_dim 64, N <= a few thousand tokens, no mask):
+//   O = softmax(scale * Q K^T [+ rel_pos_bias]) V
+// Replaces the materialised attention of the reference (dinov2_layers/attention.py:49-62; dmidas/backbones/beit.py:65-91,
+// which writes a [B,16,N,N] tensor per block and rebuilds the relative-position bias every forward).
+//
+// One CTA per (128-query tile, head, image), three warpgroups:
+//   warpgroup 0    TMA producer (one thread): the Q tile once, then K_j / V_j tiles (128 keys x 64) into a 2-stage ring,
+//                  straight out of the packed qkv activation [B*N, 3C] (no head split / transpose pass)
+//   warpgroups 1-2 consumers, 64 query rows each, everything in registers:
+//                    S  = Q K_j^T   wgmma m64n128k16, both operands K-major in shared memory, fp32 S fragment
+//                    online softmax on the fragment (a query row lives in the four lanes of a quad: two shuffles per
+//                    reduction), exp2 with the scale and log2 e folded in, running (max, sum), O rescaled in registers
+//                    O += P V_j     wgmma m64n64k16 with A = P packed to fp16 in registers (the S fragment IS the A
+//                    fragment layout, tc_common.cuh) and B = V_j used MN-major, so neither P nor V^T ever touches memory
+// While one warpgroup exponentiates, the other one's MMAs keep the tensor cores busy.
+// Bias modes: 0 none (DINOv2) | 1 dense fp16 [H,N,ld] | 2 BEiT relative-position table: the per-head table [nrd]
+// (pre-multiplied by log2 e) and the per-key offset ky*(2gw-1)+kx live in shared memory and the bias of (q, k) is
+// table[base_q - koff_k] — no [H,N,N] tensor is ever read (the reference materialises it per block per forward).
+#include <cuda.h>
+#include <cuda_fp16.h>
+#include <math.h>
+
+#include "common.cuh"
+#include "tc_common.cuh"
+
+namespace dm {
+using namespace tc;
+
+__device__ __forceinline__ float ex2_approx(float x) {
+    float y;
+    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+    return y;
+}
+
+int make_tmap_2d(CUtensorMap *tm, const void *ptr, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows, uint32_t box_cols);
+
+struct AttnParams {
+    int B, N, H;            // images, tokens per image, heads
+    int C;                  // H * 64
+    float scale_log2e;      // softmax scale * log2(e)
+    const __half *bias;     // optional [H, N, bias_ld] additive bias (natural-log domain)
+    int bias_ld;
+    __half *out;            // [B*N, C]
+    const float *rel_table; // optional [H, nrd] * log2(e): BEiT relative-position table
+    int nrd, gh, gw;
+};
+
+constexpr int AT_BQ = 128, AT_BKV = 128, AT_D = 64, AT_STAGES = 2;
+constexpr int AT_THREADS = 384;
+constexpr int AT_Q_BYTES = AT_BQ * AT_D * 2;        // 16 KB
+constexpr int AT_KV_BYTES = AT_BKV * AT_D * 2;      // 16 KB each for K and V
+constexpr int AT_K_OFF = AT_Q_BYTES;
+constexpr int AT_V_OFF = AT_K_OFF + AT_STAGES * AT_KV_BYTES;
+constexpr int AT_BAR_OFF = AT_V_OFF + AT_STAGES * AT_KV_BYTES;
+constexpr int AT_TAB_OFF = AT_BAR_OFF + 64;         // relative-position table + key offsets (mode 2)
+constexpr int AT_SMEM_MAX = 227 * 1024;
+
+template <int BIAS_MODE>
+__global__ void __launch_bounds__(AT_THREADS, 1) attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, AttnParams p) {
+    extern __shared__ __align__(1024) uint8_t smem_raw[];
+    uint8_t *sQ = smem_raw, *sK = smem_raw + AT_K_OFF, *sV = smem_raw + AT_V_OFF;
+    uint64_t *bars = reinterpret_cast<uint64_t *>(smem_raw + AT_BAR_OFF);
+    uint64_t *q_full = bars, *kv_full = bars + 1, *kv_empty = bars + 1 + AT_STAGES;
+    float *s_tab = reinterpret_cast<float *>(smem_raw + AT_TAB_OFF);
+    uint16_t *s_koff = reinterpret_cast<uint16_t *>(s_tab + ((p.nrd + 3) & ~3));
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int q0 = blockIdx.x * AT_BQ, h = blockIdx.y, b = blockIdx.z;
+    const int num_kv = (p.N + AT_BKV - 1) / AT_BKV;
+    const int row_base = b * p.N;
+
+    if (threadIdx.x == 0) {
+        prefetch_tmap(&tmQKV);
+        mbar_init(q_full, 1);
+        for (int s = 0; s < AT_STAGES; ++s) { mbar_init(&kv_full[s], 1); mbar_init(&kv_empty[s], 8); }   // 8 consumer warps
+        fence_barrier_init();
+    }
+    if (BIAS_MODE == 2) {
+        const float *tab = p.rel_table + (size_t)h * p.nrd;
+        for (int i = threadIdx.x; i < p.nrd; i += AT_THREADS) s_tab[i] = __ldg(tab + i);
+        for (int k = threadIdx.x; k < num_kv * AT_BKV; k += AT_THREADS) {
+            const int t = k - 1;
+            s_koff[k] = (k >= 1 && k < p.N) ? (uint16_t)((t / p.gw) * (2 * p.gw - 1) + (t % p.gw)) : (uint16_t)0;
+        }
+    }
+    __syncthreads();
+
+    if (warp < 4) {
+        if (threadIdx.x == 0) {
+            mbar_arrive_expect_tx(q_full, AT_Q_BYTES);
+            tma_load_2d(sQ, &tmQKV, q_full, h * AT_D, row_base + q0);
+            for (int j = 0; j < num_kv; ++j) {
+                const int s = j % AT_STAGES;
+                mbar_wait(&kv_empty[s], ((j / AT_STAGES) & 1) ^ 1);
+                mbar_arrive_expect_tx(&kv_full[s], 2 * AT_KV_BYTES);
+                tma_load_2d(sK + s * AT_KV_BYTES, &tmQKV, &kv_full[s], p.C + h * AT_D, row_base + j * AT_BKV);
+                tma_load_2d(sV + s * AT_KV_BYTES, &tmQKV, &kv_full[s], 2 * p.C + h * AT_D, row_base + j * AT_BKV);
+            }
+        }
+        return;
+    }
+
+    // ===== consumers: warpgroup wg owns query rows [64 wg, 64 wg + 64) of the tile; this thread rows r and r + 8 =====
+    const int wg = (warp >> 2) - 1, t = lane & 3;
+    constexpr float LOG2E = 1.4426950408889634f;
+    int qi[2];
+    bool q_ok[2];
+    const __half *brow[2] = {nullptr, nullptr};
+    int rp_base[2] = {0, 0}, rp_mult[2] = {1, 1};
+    float rp_k0[2] = {0.f, 0.f};
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+        qi[r] = q0 + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * r;
+        q_ok[r] = qi[r] < p.N;
+        const int qq = q_ok[r] ? qi[r] : 0;
+        if (BIAS_MODE == 1) brow[r] = p.bias + ((size_t)h * p.N + qq) * p.bias_ld;
+        if (BIAS_MODE == 2) {
+            // class-token query: the constant class->patch entry; class-token key: see the k == 0 case below
+            // (dmidas/backbones/beit.py:44-62 assembles exactly these three extra entries)
+            if (qq == 0) { rp_base[r] = p.nrd - 3; rp_mult[r] = 0; rp_k0[r] = s_tab[p.nrd - 1]; }
+            else {
+                const int tt = qq - 1, qy = tt / p.gw, qx = tt % p.gw;
+                rp_base[r] = (qy + p.gh - 1) * (2 * p.gw - 1) + (qx + p.gw - 1);
+                rp_k0[r] = s_tab[p.nrd - 2];
+            }
+        }
+    }
+    float o[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[i] = 0.f;
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+    const uint64_t qdesc = make_desc_kmajor_sw128(smem_u32(sQ) + wg * (64 * 128));
+
+    mbar_wait(q_full, 0);
+    for (int j = 0; j < num_kv; ++j) {
+        const int s = j % AT_STAGES;
+        const int kbase = j * AT_BKV;
+        mbar_wait(&kv_full[s], (j / AT_STAGES) & 1);
+        // ---- S = Q K_j^T ---------------------------------------------------------------------------------------------
+        float sc[64];
+        const uint64_t kdesc = make_desc_kmajor_sw128(smem_u32(sK + s * AT_KV_BYTES));
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < AT_D / 16; ++k) wgmma_ss<AT_BKV>(sc, qdesc + (uint64_t)(2 * k), kdesc + (uint64_t)(2 * k), k != 0);
+        wgmma_commit();
+        wgmma_wait<0>();
+        // ---- u = s * scale + bias (log2 domain), keys past the image masked, row maximum ------------------------------
+        float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+        for (int c = 0; c < AT_BKV / 8; ++c) {
+            const int k0 = kbase + 8 * c + 2 * t;
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                float b0 = 0.f, b1 = 0.f;
+                if (BIAS_MODE == 1) {
+                    const float2 bf = __half22float2(__ldg(reinterpret_cast<const __half2 *>(brow[r] + k0)));
+                    b0 = bf.x * LOG2E; b1 = bf.y * LOG2E;
+                } else if (BIAS_MODE == 2) {
+                    const uint32_t kk = *reinterpret_cast<const uint32_t *>(s_koff + k0);
+                    b0 = k0 == 0 ? rp_k0[r] : s_tab[rp_base[r] - rp_mult[r] * (int)(kk & 0xffffu)];
+                    b1 = s_tab[rp_base[r] - rp_mult[r] * (int)(kk >> 16)];
+                }
+                float u0 = fmaf(sc[4 * c + 2 * r], p.scale_log2e, b0), u1 = fmaf(sc[4 * c + 2 * r + 1], p.scale_log2e, b1);
+                u0 = k0 < p.N ? u0 : -INFINITY;
+                u1 = k0 + 1 < p.N ? u1 : -INFINITY;
+                sc[4 * c + 2 * r] = u0; sc[4 * c + 2 * r + 1] = u1;
+                mx[r] = fmaxf(mx[r], fmaxf(u0, u1));
+            }
+        }
+        float alpha[2];
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+            mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+            const float m_new = fmaxf(m_run[r], mx[r]);      // every tile holds at least one valid key: finite
+            alpha[r] = ex2_approx(m_run[r] - m_new);
+            m_run[r] = m_new;
+        }
+        // ---- p = 2^(u - m) -> fp16 A fragments; the row sum adds the ROUNDED values, so the weights of a row sum to one -----
+        uint32_t pa[AT_BKV / 16][4];
+        float ls[2] = {0.f, 0.f};
+#pragma unroll
+        for (int c = 0; c < AT_BKV / 8; ++c) {
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                const float e0 = ex2_approx(sc[4 * c + 2 * r] - m_run[r]), e1 = ex2_approx(sc[4 * c + 2 * r + 1] - m_run[r]);
+                const __half2 h2 = __floats2half2_rn(e0, e1);
+                const float2 pr = __half22float2(h2);
+                ls[r] += pr.x + pr.y;
+                pa[c >> 1][(c & 1) * 2 + r] = *reinterpret_cast<const uint32_t *>(&h2);
+            }
+        }
+#pragma unroll
+        for (int r = 0; r < 2; ++r) l_run[r] = fmaf(l_run[r], alpha[r], ls[r]);
+#pragma unroll
+        for (int c = 0; c < AT_D / 8; ++c) { o[4 * c] *= alpha[0]; o[4 * c + 1] *= alpha[0]; o[4 * c + 2] *= alpha[1]; o[4 * c + 3] *= alpha[1]; }
+        // ---- O += P V_j ------------------------------------------------------------------------------------------------
+        const uint32_t sv = smem_u32(sV + s * AT_KV_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < AT_BKV / 16; ++k) wgmma_rs_n64_bt(o, pa[k], make_desc_mnmajor_sw128(sv + k * 16 * 128));
+        wgmma_commit();
+        wgmma_wait<0>();
+        if (lane == 0) mbar_arrive(&kv_empty[s]);
+    }
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+        float l = l_run[r];
+        l += __shfl_xor_sync(0xffffffffu, l, 1);
+        l += __shfl_xor_sync(0xffffffffu, l, 2);
+        if (!q_ok[r]) continue;
+        const float inv = 1.0f / l;
+        __half *dst = p.out + (size_t)(row_base + qi[r]) * p.C + h * AT_D + 2 * t;
+#pragma unroll
+        for (int c = 0; c < AT_D / 8; ++c)
+            *reinterpret_cast<__half2 *>(dst + 8 * c) = __floats2half2_rn(o[4 * c + 2 * r] * inv, o[4 * c + 2 * r + 1] * inv);
+    }
+}
+
+template <int MODE>
+static int launch_attn(const CUtensorMap &tm, const AttnParams &p, cudaStream_t stream) {
+    const int num_kv = (p.N + AT_BKV - 1) / AT_BKV;
+    const size_t tab = MODE == 2 ? (size_t)((p.nrd + 3) & ~3) * 4 + (size_t)num_kv * AT_BKV * 2 : 0;
+    if (AT_TAB_OFF + tab > (size_t)AT_SMEM_MAX) { set_error("attention: relative-position table (%d entries) does not fit in shared memory", p.nrd); return DM_E_UNSUPPORTED; }
+    static PerDeviceFlag configured;
+    if (!configured.test_and_set())
+        DM_CUDA_CHECK(cudaFuncSetAttribute(attention_wgmma_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, AT_SMEM_MAX));
+    dim3 grid((p.N + AT_BQ - 1) / AT_BQ, p.H, p.B);
+    attention_wgmma_kernel<MODE><<<grid, AT_THREADS, AT_TAB_OFF + tab, stream>>>(tm, p);
+    DM_LAUNCH_CHECK("attention_wgmma_kernel");
+    return DM_OK;
+}
+
+int attention_f16(const __half *qkv, AttnParams p, cudaStream_t stream, const float *rel_table = nullptr, int nrd = 0, int gh = 0, int gw = 0) {
+    if (p.C != p.H * AT_D) { set_error("attention_f16: head_dim must be 64"); return DM_E_UNSUPPORTED; }
+    CUtensorMap tm;
+    int rc = make_tmap_2d(&tm, qkv, (uint64_t)p.B * p.N, (uint64_t)3 * p.C, (uint64_t)3 * p.C, AT_BQ, AT_D);
+    if (rc) return rc;
+    if (p.bias && (p.bias_ld % 8 != 0 || p.bias_ld < ((p.N + AT_BKV - 1) / AT_BKV) * AT_BKV)) {
+        set_error("attention_f16: bias row pitch must be a multiple of 8 and cover whole 128-key tiles (got %d)", p.bias_ld);
+        return DM_E_INVALID;
+    }
+    p.rel_table = rel_table; p.nrd = nrd; p.gh = gh; p.gw = gw;
+    if (rel_table) {
+        if (gh * gw + 1 != p.N || nrd != (2 * gh - 1) * (2 * gw - 1) + 3) { set_error("attention_f16: relative-position mode needs N = gh*gw+1 and nrd = (2gh-1)(2gw-1)+3"); return DM_E_INVALID; }
+        return launch_attn<2>(tm, p, stream);
+    }
+    return p.bias ? launch_attn<1>(tm, p, stream) : launch_attn<0>(tm, p, stream);
+}
+
+}  // namespace dm
+
+extern "C" __attribute__((visibility("default"))) int dm_attention_f16(const void *qkv, int B, int N, int H, float scale, const void *bias, int bias_ld,
+                                                                    void *out, void *stream) {
+    dm::AttnParams p;
+    p.B = B; p.N = N; p.H = H; p.C = H * 64;
+    p.scale_log2e = scale * 1.4426950408889634f;
+    p.bias = (const __half *)bias; p.bias_ld = bias_ld;
+    p.out = (__half *)out;
+    return dm::attention_f16((const __half *)qkv, p, (cudaStream_t)stream);
+}
+
+extern "C" __attribute__((visibility("default"))) int dm_attention_relpos_f16(const void *qkv, int B, int gh, int gw, int H, float scale,
+                                                                           const float *rel_table_log2e, int nrd,
+                                                                           void *out, void *stream) {
+    dm::AttnParams p;
+    p.B = B; p.N = gh * gw + 1; p.H = H; p.C = H * 64;
+    p.scale_log2e = scale * 1.4426950408889634f;
+    p.bias = nullptr; p.bias_ld = 0;
+    p.out = (__half *)out;
+    if (!rel_table_log2e) { dm::set_error("dm_attention_relpos_f16: table is NULL"); return DM_E_INVALID; }
+    return dm::attention_f16((const __half *)qkv, p, (cudaStream_t)stream, rel_table_log2e, nrd, gh, gw);
+}

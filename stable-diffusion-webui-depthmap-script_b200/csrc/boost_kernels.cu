@@ -20,7 +20,7 @@
 
 namespace dm {
 
-constexpr int BOOST_PARTIALS = 592;      // 148 SMs x 4 blocks of partial minima / maxima / sums
+constexpr int BOOST_PARTIALS = 528;      // 132 SMs x 4 blocks of partial minima / maxima / sums
 
 __device__ __forceinline__ void split_store8(const float (&v)[8], __half *hi0, __half *lo, __half *hi1, bool split) {
     uint4 uh, ul;

@@ -1,4 +1,4 @@
-"""Builds libdepthmap_b200.so (the C-ABI of include/depthmap_b200.h) for sm_100a, in-tree.
+"""Builds libdepthmap_b200.so (the C-ABI of include/depthmap_b200.h) for sm_90a, in-tree.
 
     python stable-diffusion-webui-depthmap-script_b200/csrc/build.py [--force] [--verbose]
 
@@ -17,7 +17,7 @@ OUT_DIR = os.path.join(PKG, "_native")
 OBJ_DIR = os.path.join(OUT_DIR, "obj")
 LIB = os.path.join(OUT_DIR, "libdepthmap_b200.so")
 
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden"]
 
 # (source, extra flags)
@@ -27,7 +27,7 @@ UNITS = [
     ("normalmap.cu", ["-fmad=false"]),
     ("stereo.cu", ["-fmad=false"]),
 ]
-for _extra in ("vit_kernels.cu", "gemm_tcgen05.cu", "attention_tcgen05.cu", "zoe_kernels.cu", "leres_kernels.cu", "boost_kernels.cu", "model.cu"):
+for _extra in ("vit_kernels.cu", "gemm_wgmma.cu", "attention_wgmma.cu", "zoe_kernels.cu", "leres_kernels.cu", "boost_kernels.cu", "model.cu"):
     if os.path.exists(os.path.join(HERE, _extra)):
         UNITS.append((_extra, []))
 

@@ -1,0 +1,419 @@
+// Tensor-core GEMM / implicit-GEMM convolution for sm_90a: C[M,N] = A[M,K] * W[N,K]^T with fused epilogues.
+//
+// Used for every Linear layer of the ViT (QKV, proj, fc1, fc2 — reference: timm Block / dinov2_layers/{attention,mlp}.py),
+// the patch embedding, the DPT 1x1 convs, ConvTranspose k=s layers (GEMM + pixel-shuffle store) and, with CONV=true,
+// the 3x3 stride-1 pad-1 convolutions of the DPT decoder (reference: dmidas/blocks.py, depth_anything_v2/util/blocks.py)
+// as implicit GEMM over NHWC activations: the 9 taps are 9 shifted TMA boxes, zero padding = TMA out-of-bounds fill.
+//
+// Structure (one 128 x BN output tile per CTA, three warpgroups):
+//   warpgroup 0   : TMA producer — one thread issues cp.async.bulk.tensor into a STAGES-deep ring of 128B-swizzled smem
+//                   tiles (mbarrier tx); the rest of the warpgroup exits the role branch at once
+//   warpgroups 1-2: consumers — each owns 64 of the 128 rows: wgmma.mma_async m64nBNk16 (fp16 operands from shared memory,
+//                   fp32 accumulators in registers), one commit group per k-block, the previous k-block's ring slot is
+//                   released once its group has retired; then the epilogue on the accumulator fragment: bias / GELU / ReLU /
+//                   LayerScale+residual / pixel-shuffle / fused 1x1 head, 8-byte (fp32) or 4-byte (fp16) accesses in which
+//                   the four lanes of a quad cover one 32- or 16-byte run of a row
+// Tiles of up to 64 columns keep two CTAs resident per SM, so one tile's epilogue overlaps another's main loop.
+#include <cuda.h>
+#include <cuda_fp16.h>
+#include <math.h>
+#include <stdlib.h>
+
+#include "common.cuh"
+#include "tc_common.cuh"
+
+namespace dm {
+using namespace tc;
+
+enum GemmEpi : int {
+    EPI_STORE_F16 = 0,   // C = act(acc + bias) [+ R]           -> fp16 [M, ldc]   (+ optional relu copy C2)
+    EPI_RESID_F32 = 1,   // X += gamma[n] * (acc + bias[n])     -> fp32 in place (LayerScale + residual)
+    EPI_PIXSHUF = 2,     // ConvTranspose k=s: n = (i, j, co) scattered to out[b, s*y+i, s*x+j, co]
+    EPI_HEAD = 3,        // relu(acc + bias) . w2 + b2 -> relu -> fp32 [M]   (conv3x3 -> ReLU -> conv1x1 -> ReLU fused; BN = N)
+    EPI_STORE_F32 = 4,   // C = acc + bias -> fp32 [M, ldc]
+};
+enum GemmAct : int { ACT_NONE = 0, ACT_GELU = 1, ACT_RELU = 2 };
+
+struct GemmParams {
+    int M, N, K;
+    int epi, act;
+    const float *bias;      // [N] or null
+    __half *C; int ldc;     // fp16 output
+    __half *C2;             // optional relu(C) copy (same layout) or null
+    const __half *R; int ldr;  // optional fp16 residual added before the store (EPI_STORE_F16)
+    const __half *R2; int ldr2;  // optional second fp16 residual
+    float *X; int ldx;      // fp32 residual stream (EPI_RESID_F32) / fp32 output (EPI_STORE_F32, EPI_HEAD)
+    const float *gamma;     // [N] LayerScale (EPI_RESID_F32) / w2 (EPI_HEAD)
+    float head_b2;
+    // pixel shuffle
+    int ps_s, ps_cout, ps_h, ps_w;
+    // implicit conv geometry (CONV): activations [B, H, W, Cin]; tile = hbox x wbox pixels
+    int cB, cH, cW, cCin, hbox, wbox, tiles_x, tiles_y;
+};
+
+template <int BN>
+struct GemmCfg {
+    static constexpr int BM = 128, BK = 64;
+    static constexpr int STAGES = 4;
+    static constexpr int A_BYTES = BM * BK * 2, B_BYTES = BN * BK * 2;
+    static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 256 /*barriers*/;   // base is __align__(1024)
+    static constexpr int CTAS_PER_SM = BN <= 64 ? 2 : 1;
+};
+constexpr int GEMM_THREADS = 384;
+
+// exact-erf GELU, one MUFU.  With u = min(|x|, 5.75):
+//     gelu(x) = max(x, 0) - u * 2^(-u Q(u) - 1),      Q(u) = -log2(erfc(u / sqrt 2)) / u
+// Q is smooth and nearly linear on [0, 5.75]; the degree-5 fit below (Lawson-weighted on the GELU error) keeps
+// |gelu - x Phi(x)| < 3.2e-7 in fp32 over all x (tests/test_gelu_formula.py checks the same numbers on
+// the host), i.e. three orders below the fp16 rounding of the stored activation.  Past the clamp u*2^(..) < 3e-8.
+__device__ __forceinline__ float gelu_erf(float x) {
+    const float u = fminf(fabsf(x), 5.75f);
+    float q = -2.992472582263872e-05f;
+    q = fmaf(q, u, 0.0007398786256089807f);
+    q = fmaf(q, u, -0.007977476343512535f);
+    q = fmaf(q, u, 0.05323820561170578f);
+    q = fmaf(q, u, 0.45891568064689636f);
+    q = fmaf(q, u, 1.1511471271514893f);
+    float e;
+    const float t = fmaf(-u, q, -1.f);
+    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(t));
+    return fmaf(-u, e, fmaxf(x, 0.f));
+}
+
+// Epilogue of one consumer thread: its accumulator fragment holds rows r0 = 16 * warp + lane / 4 and r0 + 8 of the
+// warpgroup's 64, and for every 8-column group j the columns 8j + 2 (lane % 4), +1 (tc_common.cuh).
+template <int BN>
+__device__ __forceinline__ void epilogue_fragment(const GemmParams &p, const float (&acc)[BN / 2], const long long (&m)[2], const bool (&row_ok)[2],
+                                                  int n_base, int lane) {
+    const int t = lane & 3;
+    float head_acc[2] = {0.f, 0.f};
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+        const int n = n_base + 8 * j + 2 * t;
+        if (n >= p.N) continue;
+        float2 b2 = make_float2(0.f, 0.f);
+        if (p.bias) b2 = __ldg(reinterpret_cast<const float2 *>(p.bias + n));
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            if (!row_ok[r]) continue;
+            float v0 = acc[4 * j + 2 * r] + b2.x, v1 = acc[4 * j + 2 * r + 1] + b2.y;
+            if (p.epi == EPI_RESID_F32) {
+                float2 *xp = reinterpret_cast<float2 *>(p.X + m[r] * p.ldx + n);
+                const float2 g2 = __ldg(reinterpret_cast<const float2 *>(p.gamma + n));
+                float2 x = *xp;
+                x.x = fmaf(g2.x, v0, x.x); x.y = fmaf(g2.y, v1, x.y);
+                *xp = x;
+                continue;
+            }
+            if (p.epi == EPI_STORE_F32) {
+                *reinterpret_cast<float2 *>(p.X + m[r] * p.ldx + n) = make_float2(v0, v1);
+                continue;
+            }
+            if (p.act == ACT_GELU) { v0 = gelu_erf(v0); v1 = gelu_erf(v1); }
+            else if (p.act == ACT_RELU) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+            if (p.epi == EPI_HEAD) {
+                const float2 w2 = __ldg(reinterpret_cast<const float2 *>(p.gamma + n));
+                head_acc[r] = fmaf(v1, w2.y, fmaf(v0, w2.x, head_acc[r]));
+                continue;
+            }
+            if (p.R) { const float2 f = __half22float2(__ldg(reinterpret_cast<const __half2 *>(p.R + m[r] * p.ldr + n))); v0 += f.x; v1 += f.y; }
+            if (p.R2) { const float2 f = __half22float2(__ldg(reinterpret_cast<const __half2 *>(p.R2 + m[r] * p.ldr2 + n))); v0 += f.x; v1 += f.y; }
+            const __half2 h2 = __floats2half2_rn(v0, v1);
+            if (p.epi == EPI_PIXSHUF) {
+                const int s = p.ps_s, ij = n / p.ps_cout, co = n % p.ps_cout;
+                const int i = ij / s, jx = ij % s;
+                const long long bb = m[r] / ((long long)p.ps_h * p.ps_w);
+                const int rem = (int)(m[r] % ((long long)p.ps_h * p.ps_w));
+                const int y = rem / p.ps_w, x = rem % p.ps_w;
+                *reinterpret_cast<__half2 *>(p.C + (((bb * (p.ps_h * s) + (y * s + i)) * (long long)(p.ps_w * s)) + (x * s + jx)) * p.ps_cout + co) = h2;
+            } else {
+                *reinterpret_cast<__half2 *>(p.C + m[r] * p.ldc + n) = h2;
+                if (p.C2) *reinterpret_cast<__half2 *>(p.C2 + m[r] * p.ldc + n) = __hmax2(h2, __float2half2_rn(0.f));
+            }
+        }
+    }
+    if (p.epi == EPI_HEAD) {
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            float s = head_acc[r];
+            s += __shfl_xor_sync(0xffffffffu, s, 1);
+            s += __shfl_xor_sync(0xffffffffu, s, 2);
+            if (t == 0 && row_ok[r]) p.X[m[r]] = fmaxf(s + p.head_b2, 0.f);
+        }
+    }
+}
+
+template <int BN, bool CONV>
+__global__ void __launch_bounds__(GEMM_THREADS, GemmCfg<BN>::CTAS_PER_SM) gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA,
+                                                                                          const __grid_constant__ CUtensorMap tmB, GemmParams p) {
+    using Cfg = GemmCfg<BN>;
+    extern __shared__ __align__(1024) uint8_t smem_raw[];
+    uint8_t *smem = smem_raw;
+    uint64_t *full = reinterpret_cast<uint64_t *>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
+    uint64_t *empty = full + Cfg::STAGES;
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int m_blk = blockIdx.x, n_blk = blockIdx.y;
+    const int num_kb = CONV ? 9 * (p.cCin / Cfg::BK) : p.K / Cfg::BK;
+
+    if (threadIdx.x == 0) {
+        prefetch_tmap(&tmA);
+        prefetch_tmap(&tmB);
+        for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }   // 8 consumer warps
+        fence_barrier_init();
+    }
+    __syncthreads();
+
+    // conv tile coordinates
+    int cb = 0, cy0 = 0, cx0 = 0;
+    if (CONV) {
+        const int tiles_per_img = p.tiles_x * p.tiles_y;
+        cb = m_blk / tiles_per_img;
+        const int t = m_blk % tiles_per_img;
+        cy0 = (t / p.tiles_x) * p.hbox;
+        cx0 = (t % p.tiles_x) * p.wbox;
+    }
+
+    if (warp < 4) {
+        if (threadIdx.x == 0) {
+            int stage = 0, phase = 0;
+            for (int kb = 0; kb < num_kb; ++kb) {
+                mbar_wait(&empty[stage], phase ^ 1);
+                uint8_t *sa = smem + stage * Cfg::STAGE_BYTES, *sb = sa + Cfg::A_BYTES;
+                mbar_arrive_expect_tx(&full[stage], Cfg::STAGE_BYTES);
+                if (CONV) {
+                    const int cblks = p.cCin / Cfg::BK;
+                    const int tap = kb / cblks, cblk = kb % cblks;
+                    const int dy = tap / 3 - 1, dx = tap % 3 - 1;
+                    tma_load_4d(sa, &tmA, &full[stage], cblk * Cfg::BK, cx0 + dx, cy0 + dy, cb);
+                } else {
+                    tma_load_2d(sa, &tmA, &full[stage], kb * Cfg::BK, m_blk * Cfg::BM);
+                }
+                tma_load_2d(sb, &tmB, &full[stage], kb * Cfg::BK, n_blk * BN);
+                if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
+            }
+        }
+        return;
+    }
+
+    // ===== consumers: warpgroup wg owns rows [64 wg, 64 wg + 64) of the tile =====
+    const int wg = (warp >> 2) - 1;
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    int stage = 0, phase = 0, prev = 0;
+    for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full[stage], phase);
+        const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES) + wg * (64 * 128), sb = smem_u32(smem + stage * Cfg::STAGE_BYTES) + Cfg::A_BYTES;
+        const uint64_t adesc = make_desc_kmajor_sw128(sa), bdesc = make_desc_kmajor_sw128(sb);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < Cfg::BK / 16; ++k) wgmma_ss<BN>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (kb | k) != 0);
+        wgmma_commit();
+        if (kb > 0) {                       // the previous k-block's MMAs have retired: hand its slot back to the producer
+            wgmma_wait<1>();
+            if (lane == 0) mbar_arrive(&empty[prev]);
+        }
+        prev = stage;
+        if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+
+    long long m[2];
+    bool row_ok[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+        const int row = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * r;
+        if (CONV) {
+            const int y = cy0 + row / p.wbox, x = cx0 + row % p.wbox;
+            row_ok[r] = (y < p.cH) && (x < p.cW);
+            m[r] = ((long long)cb * p.cH + y) * p.cW + x;
+        } else {
+            m[r] = (long long)m_blk * Cfg::BM + row;
+            row_ok[r] = m[r] < p.M;
+        }
+    }
+    epilogue_fragment<BN>(p, acc, m, row_ok, n_blk * BN, lane);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// host side
+// ---------------------------------------------------------------------------------------------------------------------
+typedef CUresult (*PFN_encodeTiled)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
+                                    const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+static PFN_encodeTiled get_encode() {
+    static PFN_encodeTiled fn = nullptr;
+    if (!fn) {
+        void *p = nullptr;
+        cudaDriverEntryPointQueryResult qres;
+        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) != cudaSuccess || !p) return nullptr;
+        fn = (PFN_encodeTiled)p;
+    }
+    return fn;
+}
+
+// 2-D fp16 row-major [rows, cols] with row pitch ld (elements); box = box_rows x 64 cols, 128B swizzle
+int make_tmap_2d(CUtensorMap *tm, const void *ptr, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows, uint32_t box_cols) {
+    PFN_encodeTiled enc = get_encode();
+    if (!enc) { set_error("cuTensorMapEncodeTiled unavailable"); return DM_E_CUDA; }
+    cuuint64_t dims[2] = {cols, rows};
+    cuuint64_t strides[1] = {ld * 2};
+    cuuint32_t box[2] = {box_cols, box_rows};
+    cuuint32_t es[2] = {1, 1};
+    CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void *>(ptr), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(2d) failed: %d (rows=%llu cols=%llu ld=%llu)", (int)r, (unsigned long long)rows, (unsigned long long)cols, (unsigned long long)ld); return DM_E_CUDA; }
+    return DM_OK;
+}
+
+// 4-D fp16 NHWC [B, H, W, C]; box = [1, hbox, wbox, 64]
+int make_tmap_nhwc(CUtensorMap *tm, const void *ptr, uint64_t B, uint64_t H, uint64_t W, uint64_t C, uint32_t hbox, uint32_t wbox) {
+    PFN_encodeTiled enc = get_encode();
+    if (!enc) { set_error("cuTensorMapEncodeTiled unavailable"); return DM_E_CUDA; }
+    cuuint64_t dims[4] = {C, W, H, B};
+    cuuint64_t strides[3] = {C * 2, W * C * 2, H * W * C * 2};
+    cuuint32_t box[4] = {64, wbox, hbox, 1};
+    cuuint32_t es[4] = {1, 1, 1, 1};
+    CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void *>(ptr), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(4d) failed: %d", (int)r); return DM_E_CUDA; }
+    return DM_OK;
+}
+
+template <int BN, bool CONV>
+static int launch_gemm(const CUtensorMap &tmA, const CUtensorMap &tmB, const GemmParams &p, int m_tiles, cudaStream_t stream) {
+    using Cfg = GemmCfg<BN>;
+    static PerDeviceFlag configured;
+    if (!configured.test_and_set())
+        DM_CUDA_CHECK(cudaFuncSetAttribute(gemm_wgmma_kernel<BN, CONV>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    dim3 grid(m_tiles, (p.N + BN - 1) / BN);      // m fastest: the CTAs running together share one weight panel in L2
+    gemm_wgmma_kernel<BN, CONV><<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, p);
+    DM_LAUNCH_CHECK("gemm_wgmma_kernel");
+    return DM_OK;
+}
+
+// The epilogue reads and writes column PAIRS: 8-byte accesses to the fp32 operands (bias, gamma, X), 4-byte ones to the fp16
+// operands (C, C2, R, R2).  Their pitches must therefore be even and their base addresses aligned accordingly.
+static int check_epilogue_operands(const GemmParams &p, const char *who) {
+    auto misaligned = [](const void *q, size_t a) { return q && (reinterpret_cast<uintptr_t>(q) % a) != 0; };
+    const bool f32_rows = p.epi == EPI_RESID_F32 || p.epi == EPI_STORE_F32;
+    const bool f16_rows = p.epi == EPI_STORE_F16 || p.epi == EPI_PIXSHUF;
+    if ((f32_rows && (!p.X || p.ldx % 2)) || (p.epi == EPI_HEAD && !p.X)) { set_error("%s: fp32 output missing or its pitch is odd (ldx=%d)", who, p.ldx); return DM_E_INVALID; }
+    if (f16_rows && (!p.C || (p.epi == EPI_STORE_F16 && p.ldc % 2))) { set_error("%s: fp16 output missing or its pitch is odd (ldc=%d)", who, p.ldc); return DM_E_INVALID; }
+    if (f16_rows && ((p.R && p.ldr % 2) || (p.R2 && p.ldr2 % 2))) { set_error("%s: residual pitches must be even (ldr=%d ldr2=%d)", who, p.ldr, p.ldr2); return DM_E_INVALID; }
+    if (p.epi == EPI_PIXSHUF && (p.ps_s < 1 || p.ps_cout < 2 || p.ps_cout % 2 || p.N != p.ps_s * p.ps_s * p.ps_cout)) {
+        set_error("%s: pixel shuffle needs an even channel count and N = s*s*cout (s=%d cout=%d N=%d)", who, p.ps_s, p.ps_cout, p.N);
+        return DM_E_INVALID;
+    }
+    if ((p.epi == EPI_RESID_F32 || p.epi == EPI_HEAD) && !p.gamma) { set_error("%s: gamma is NULL", who); return DM_E_INVALID; }
+    if (misaligned(p.bias, 8) || misaligned(p.gamma, 8) || (f32_rows && misaligned(p.X, 8))) { set_error("%s: fp32 operands must be 8-byte aligned", who); return DM_E_INVALID; }
+    if (f16_rows && (misaligned(p.C, 4) || misaligned(p.C2, 4) || misaligned(p.R, 4) || misaligned(p.R2, 4))) { set_error("%s: fp16 operands must be 4-byte aligned", who); return DM_E_INVALID; }
+    return DM_OK;
+}
+
+// the fused head keeps a whole output row in one tile (BN = N = 32)
+static int pick_bn(const GemmParams &p) { return p.epi == EPI_HEAD ? 32 : (p.N % 128 == 0 ? 128 : (p.N % 64 == 0 ? 64 : 32)); }
+
+// Plain GEMM: A fp16 [M, K] (pitch lda), W fp16 [N, K] (pitch ldw)
+int gemm_f16(const __half *A, int lda, const __half *W, int ldw, GemmParams p, cudaStream_t stream) {
+    if (p.K % 64 != 0 || p.N % 32 != 0) { set_error("gemm_f16: K must be a multiple of 64 and N of 32 (K=%d N=%d)", p.K, p.N); return DM_E_INVALID; }
+    if (p.epi == EPI_HEAD && p.N != 32) { set_error("gemm_f16: the fused head needs N = 32 (N=%d)", p.N); return DM_E_UNSUPPORTED; }
+    if (int rc0 = check_epilogue_operands(p, "gemm_f16")) return rc0;
+    if ((lda % 8) || (ldw % 8)) { set_error("gemm_f16: row pitches must be multiples of 8 elements"); return DM_E_INVALID; }
+    const int m_tiles = (p.M + 127) / 128;
+    const int bn = pick_bn(p);
+    CUtensorMap tmA, tmB;
+    int rc = make_tmap_2d(&tmA, A, (uint64_t)p.M, (uint64_t)p.K, (uint64_t)lda, 128, 64);
+    if (rc) return rc;
+    rc = make_tmap_2d(&tmB, W, (uint64_t)p.N, (uint64_t)p.K, (uint64_t)ldw, (uint32_t)bn, 64);
+    if (rc) return rc;
+    switch (bn) {
+        case 128: return launch_gemm<128, false>(tmA, tmB, p, m_tiles, stream);
+        case 64: return launch_gemm<64, false>(tmA, tmB, p, m_tiles, stream);
+        case 32: return launch_gemm<32, false>(tmA, tmB, p, m_tiles, stream);
+    }
+    set_error("gemm_f16: unsupported N tile %d", bn);
+    return DM_E_UNSUPPORTED;
+}
+
+// 3x3 stride-1 pad-1 convolution, NHWC fp16 activations [B,H,W,Cin], weights fp16 [Cout, 9*Cin] ordered (ky, kx, cin)
+int conv3x3_f16(const __half *act, int B, int H, int W, int Cin, const __half *Wt, GemmParams p, cudaStream_t stream) {
+    if (Cin % 64 != 0 || p.N % 32 != 0) { set_error("conv3x3_f16: Cin must be a multiple of 64 and Cout of 32"); return DM_E_INVALID; }
+    if (p.epi == EPI_HEAD && p.N != 32) { set_error("conv3x3_f16: the fused head needs Cout = 32 (Cout=%d)", p.N); return DM_E_UNSUPPORTED; }
+    if (int rc0 = check_epilogue_operands(p, "conv3x3_f16")) return rc0;
+    // tile = hbox x wbox pixels = 128 rows; choose the wbox in {128,64,32,16,8} with the least padding waste
+    int best_w = 128; double best_eff = -1;
+    for (int wb = 128; wb >= 8; wb >>= 1) {
+        const int hb = 128 / wb;
+        const double eff = (double)(W * H) / ((double)((W + wb - 1) / wb * wb) * ((H + hb - 1) / hb * hb));
+        if (eff > best_eff + 1e-9) { best_eff = eff; best_w = wb; }
+    }
+    p.wbox = best_w; p.hbox = 128 / best_w;
+    p.tiles_x = (W + p.wbox - 1) / p.wbox; p.tiles_y = (H + p.hbox - 1) / p.hbox;
+    p.cB = B; p.cH = H; p.cW = W; p.cCin = Cin;
+    p.M = B * H * W; p.K = 9 * Cin;
+    const int m_tiles = B * p.tiles_x * p.tiles_y;
+    const int bn = pick_bn(p);
+    CUtensorMap tmA, tmB;
+    int rc = make_tmap_nhwc(&tmA, act, B, H, W, Cin, p.hbox, p.wbox);
+    if (rc) return rc;
+    rc = make_tmap_2d(&tmB, Wt, (uint64_t)p.N, (uint64_t)p.K, (uint64_t)p.K, (uint32_t)bn, 64);
+    if (rc) return rc;
+    switch (bn) {
+        case 128: return launch_gemm<128, true>(tmA, tmB, p, m_tiles, stream);
+        case 64: return launch_gemm<64, true>(tmA, tmB, p, m_tiles, stream);
+        case 32: return launch_gemm<32, true>(tmA, tmB, p, m_tiles, stream);
+    }
+    set_error("conv3x3_f16: unsupported N tile %d", bn);
+    return DM_E_UNSUPPORTED;
+}
+
+}  // namespace dm
+
+// ---- C-ABI test / building-block entry points ---------------------------------------------------------------------
+extern "C" __attribute__((visibility("default"))) int dm_gemm_f16(const void *A, int lda, const void *W, int ldw, const float *bias, void *C,
+                                                               int ldc, int M, int N, int K, int act, int out_f32, void *stream) {
+    using namespace dm;
+    GemmParams p;
+    memset(&p, 0, sizeof(p));
+    p.M = M; p.N = N; p.K = K; p.act = act; p.bias = bias;
+    if (out_f32) { p.epi = EPI_STORE_F32; p.X = (float *)C; p.ldx = ldc; }
+    else { p.epi = EPI_STORE_F16; p.C = (__half *)C; p.ldc = ldc; }
+    return gemm_f16((const __half *)A, lda, (const __half *)W, ldw, p, (cudaStream_t)stream);
+}
+
+extern "C" __attribute__((visibility("default"))) int dm_conv3x3_f16(const void *act, int B, int H, int W, int Cin, const void *Wt, const float *bias,
+                                                                  void *out, int Cout, int relu, void *stream) {
+    using namespace dm;
+    GemmParams p;
+    memset(&p, 0, sizeof(p));
+    p.N = Cout; p.act = relu ? ACT_RELU : ACT_NONE; p.bias = bias; p.epi = EPI_STORE_F16; p.C = (__half *)out; p.ldc = Cout;
+    return conv3x3_f16((const __half *)act, B, H, W, Cin, (const __half *)Wt, p, (cudaStream_t)stream);
+}
+
+static void desc_to_params(const dm_gemm_desc *d, dm::GemmParams &p) {
+    memset(&p, 0, sizeof(p));
+    p.M = d->M; p.N = d->N; p.K = d->K; p.epi = d->epi; p.act = d->act; p.bias = d->bias;
+    p.C = (__half *)d->C; p.ldc = d->ldc; p.C2 = (__half *)d->C2;
+    p.R = (const __half *)d->R; p.ldr = d->ldr; p.R2 = (const __half *)d->R2; p.ldr2 = d->ldr2;
+    p.X = d->X; p.ldx = d->ldx; p.gamma = d->gamma; p.head_b2 = d->head_b2;
+    p.ps_s = d->ps_s; p.ps_cout = d->ps_cout; p.ps_h = d->ps_h; p.ps_w = d->ps_w;
+}
+
+extern "C" __attribute__((visibility("default"))) int dm_gemm_ex(const void *A, int lda, const void *W, int ldw, const dm_gemm_desc *d, void *stream) {
+    if (!A || !W || !d) { dm::set_error("dm_gemm_ex: null argument"); return DM_E_INVALID; }
+    dm::GemmParams p;
+    desc_to_params(d, p);
+    return dm::gemm_f16((const __half *)A, lda, (const __half *)W, ldw, p, (cudaStream_t)stream);
+}
+
+extern "C" __attribute__((visibility("default"))) int dm_conv3x3_ex(const void *act, int B, int H, int W, int Cin, const void *Wt, const dm_gemm_desc *d, void *stream) {
+    if (!act || !Wt || !d) { dm::set_error("dm_conv3x3_ex: null argument"); return DM_E_INVALID; }
+    dm::GemmParams p;
+    desc_to_params(d, p);
+    return dm::conv3x3_f16((const __half *)act, B, H, W, Cin, (const __half *)Wt, p, (cudaStream_t)stream);
+}
+

@@ -1,6 +1,6 @@
 // D8 — LeReS (ResNeXt-101 32x8d + FTB / FFM / AO decoder): the pieces that are not GEMMs or 3x3 stride-1 convolutions.
 // Replaces parts of estimateleres / scale_torch (src/depthmap_generation.py:406-440), lib/Resnext_torch.py:196-220 and
-// lib/network_auxi.py:95-215.  Everything else of the network runs on the tcgen05 GEMM / implicit-GEMM conv: 1x1 convs are GEMMs
+// lib/network_auxi.py:95-215.  Everything else of the network runs on the wgmma GEMM / implicit-GEMM conv: 1x1 convs are GEMMs
 // on NHWC activations, the 32-group 3x3 convs run as dense implicit GEMMs with block-diagonal filters (zero blocks between the
 // groups keep the tensor core busy with exact zeros: 0.49 TFLOP-equivalent per 448^2 image instead of 0.29, but no new MMA shape),
 // BatchNorm (inference statistics) is folded into the filters and biases at load time.

@@ -495,13 +495,13 @@ static int run_forward(dm_model *m, const uint8_t *rgb, int B, int H, int W, int
         const Block &k = m->blocks[i];
         DM_TRY(dm_layernorm_f16((float *)Bf("x"), rows, C, k.ln1_w, k.ln1_b, 1e-6f, Bf("h"), 1, 0, st));
         DM_TRY(gemm(m, Bf("h"), C, k.qkv_w, C, (int)rows, 3 * C, C, st, DM_EPI_STORE_F16, DM_ACT_NONE, k.qkv_b, Bf("qkv"), 3 * C));
-        if (beit) DM_TRY(dm_attention_relpos_f16(Bf("qkv"), B, gh, gw, heads, scale, m->rel_tab[i], nullptr, m->nrd, Bf("att"), st));
+        if (beit) DM_TRY(dm_attention_relpos_f16(Bf("qkv"), B, gh, gw, heads, scale, m->rel_tab[i], m->nrd, Bf("att"), st));
         else DM_TRY(dm_attention_f16(Bf("qkv"), B, N, heads, scale, nullptr, 0, Bf("att"), st));
         DM_TRY(gemm(m, Bf("att"), C, k.proj_w, C, (int)rows, C, C, st, DM_EPI_RESID_F32, DM_ACT_NONE, k.proj_b, nullptr, 0, (float *)Bf("x"), C, k.ls1));
         DM_TRY(dm_layernorm_f16((float *)Bf("x"), rows, C, k.ln2_w, k.ln2_b, 1e-6f, Bf("h"), 1, 0, st));
         DM_TRY(gemm(m, Bf("h"), C, k.fc1_w, C, (int)rows, 4 * C, C, st, DM_EPI_STORE_F16, DM_ACT_GELU, k.fc1_b, Bf("mlp"), 4 * C));
         DM_TRY(gemm(m, Bf("mlp"), 4 * C, k.fc2_w, 4 * C, (int)rows, C, 4 * C, st, DM_EPI_RESID_F32, DM_ACT_NONE, k.fc2_b, nullptr, 0, (float *)Bf("x"), C, k.ls2));
-        m->launches += 3 + (beit && gw % 16 == 0 ? 1 : 0);
+        m->launches += 3;
         if (fi < 4 && i == c.layers[fi]) {
             const std::string f = "feat" + std::to_string(fi);
             if (midas) {  // forward hook on the raw block output + ProjectReadout: GELU(Linear(cat(tokens, cls)))

@@ -263,7 +263,7 @@ extern "C" __attribute__((visibility("default"))) int dm_normalize_u16(const flo
     int64_t work = vec_ok ? n / 4 : n;
     int bx = (int)((work + 256 * 4 - 1) / (256 * 4));
     if (bx < 1) bx = 1;
-    if (bx > 148 * 8) bx = 148 * 8;
+    if (bx > 132 * 8) bx = 132 * 8;
     dim3 grid(bx, B);
     minmax_f32_kernel<<<grid, 256, 0, stream>>>(pred, n, ws, vec_ok);
     DM_LAUNCH_CHECK("minmax_f32_kernel");
@@ -296,7 +296,7 @@ extern "C" __attribute__((visibility("default"))) int dm_normalize_u16_outliers(
     int64_t work = vec_ok ? n / 4 : n;
     int bx = (int)((work + 256 * 4 - 1) / (256 * 4));
     if (bx < 1) bx = 1;
-    if (bx > 148 * 8) bx = 148 * 8;
+    if (bx > 132 * 8) bx = 132 * 8;
     dim3 grid(bx, B);
     minmax_f32_kernel<<<grid, 256, 0, stream>>>(pred, n, ws, vec_ok);
     DM_LAUNCH_CHECK("minmax_f32_kernel");
@@ -304,7 +304,7 @@ extern "C" __attribute__((visibility("default"))) int dm_normalize_u16_outliers(
     DM_LAUNCH_CHECK("select_init_kernel");
     int sx = (int)((n + 256 * 16 - 1) / (256 * 16));
     if (sx < 1) sx = 1;
-    if (sx > 148 * 4) sx = 148 * 4;
+    if (sx > 132 * 4) sx = 132 * 4;
     for (int pass = 0; pass < 4; ++pass) {
         select_hist_kernel<<<dim3(sx, B), 256, 0, stream>>>(pred, n, invert ? 1 : 0, pass, st);
         DM_LAUNCH_CHECK("select_hist_kernel");
@@ -375,7 +375,7 @@ __global__ void __launch_bounds__(256) video_scale_f64_kernel(const float *__res
 
 static int video_grid(int64_t n) {
     int64_t b = (n + 256 * 8 - 1) / (256 * 8);
-    return (int)(b < 1 ? 1 : (b > 148 * 8 ? 148 * 8 : b));
+    return (int)(b < 1 ? 1 : (b > 132 * 8 ? 132 * 8 : b));
 }
 
 }  // namespace dm
@@ -430,7 +430,7 @@ DM_EXPORT int dm_video_select_hist(const float *x, long long n, int pass, void *
     using namespace dm;
     if (n > 0) {
         int sx = (int)((n + 256 * 16 - 1) / (256 * 16));
-        sx = sx < 1 ? 1 : (sx > 148 * 4 ? 148 * 4 : sx);
+        sx = sx < 1 ? 1 : (sx > 132 * 4 ? 132 * 4 : sx);
         select_hist_kernel<<<dim3(sx, 1), 256, 0, (cudaStream_t)stream_>>>(x, n, 0, pass, (SelectState *)workspace);
         DM_LAUNCH_CHECK("select_hist_kernel");
     }

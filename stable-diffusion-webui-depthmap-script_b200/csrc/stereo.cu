@@ -294,7 +294,7 @@ __device__ void polylines_eye(const RowSmem &sm, const NdSrc &nds, int W, double
                 s = lo;
             }
             // Source columns of vertices s and s+1.  Written as plain clamps of the column index on purpose: with
-            // CUDA 12.9 ptxas for sm_100a, `s = min(s, n-2)` followed by a test `s == n-2` is fused into a VIMNMX with a
+            // CUDA 12.9 ptxas (seen on a Blackwell target; not re-examined on sm_90a), `s = min(s, n-2)` followed by a test `s == n-2` is fused into a VIMNMX with a
             // predicate output whose sense is wrong on the hardware (observed: the equality came out true for every
             // s < n-2), so no equality test may follow a min/max on the same operands here.
             int col_l = SHARP ? ((s - 1) >> 1) : (s - 1);   // vertex 0 (opening sentinel) -> -1 -> column 0
@@ -613,7 +613,7 @@ extern "C" __attribute__((visibility("default"))) int dm_stereo(const uint8_t *r
         minmax_u16_init_kernel<<<(B + 255) / 256, 256, 0, stream>>>(ws, B);
         DM_LAUNCH_CHECK("minmax_u16_init_kernel");
         int bx = (int)((n / 8 + 255) / 256);
-        bx = bx < 1 ? 1 : (bx > 148 * 4 ? 148 * 4 : bx);
+        bx = bx < 1 ? 1 : (bx > 132 * 4 ? 132 * 4 : bx);
         minmax_u16_kernel<<<dim3(bx, B), 256, 0, stream>>>((const uint16_t *)depth, n, ws);
         DM_LAUNCH_CHECK("minmax_u16_kernel");
     }

@@ -1,7 +1,7 @@
 // D7 — ZoeDepth-NK: everything around the DPT-BEiT core that the reference's DepthModel / ZoeDepthNK adds
 // (dzoedepth/models/depth_model.py:57-152, zoedepth_nk/zoedepth_nk_v1.py:159-243, layers/attractor.py:127-208,
 // layers/dist_layers.py:29-121, layers/patch_transformer.py:29-92, base_models/midas.py:175-186).
-// The 1x1 convolutions of the head run on the tcgen05 GEMM (NHWC activations = row-major [pixels, channels]); the
+// The 1x1 convolutions of the head run on the wgmma GEMM (NHWC activations = row-major [pixels, channels]); the
 // kernels here are the bandwidth-side pieces, fp32 math:
 //   zoe_preprocess_patchify  ToTensor -> reflect pad -> (flip) -> bilinear align_corners=True to the net size -> (x-.5)/.5
 //                            -> fp16 patch matrix; forward 2b is image b, forward 2b+1 its horizontal flip (TTA)

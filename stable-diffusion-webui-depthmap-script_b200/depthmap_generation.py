@@ -1,10 +1,10 @@
-"""Depth estimation on B200 — drop-in for the hot-path part of the reference's ``src/depthmap_generation.py``.
+"""Depth estimation on H100 — drop-in for the hot-path part of the reference's ``src/depthmap_generation.py``.
 
 ``ModelHolder`` keeps the reference's public methods and attributes (src/depthmap_generation.py:40-403):
 ``update_settings``, ``ensure_models``, ``load_models``, ``get_default_net_size``, ``offload``, ``reload``,
 ``unload_models``, ``get_raw_prediction(input, net_width, net_height) -> (float32 [H,W], invert)``, plus the additive
 ``get_raw_prediction_batch`` (uint8 CUDA batch in, float32 CUDA batch out, no host sync) used by the batched funnel and
-the bench.  The network forward is a sequence of C-ABI calls (tcgen05 GEMM / implicit-GEMM conv / fused attention /
+the bench.  The network forward is a sequence of C-ABI calls (wgmma GEMM / implicit-GEMM conv / fused attention /
 LayerNorm / resize kernels, include/depthmap_b200.h); PyTorch only owns device memory and the stream.
 
 Implemented model types: 1, 2 (MiDaS 3.1 DPT-BEiT-L 512 / 384), 3 (MiDaS 3.0 DPT-Large 384), 9 (ZoeDepth-NK) and 12, 13, 14
@@ -110,8 +110,8 @@ class _Ops:
                                            bias_ld, out.data_ptr(), _lib.stream_ptr()), "dm_attention_f16")
         self.launches += 1
 
-    def attention_relpos(self, qkv, B, gh, gw, H, scale, table, rowmax, nrd, out):
-        _lib.check(self.L.dm_attention_relpos_f16(qkv.data_ptr(), B, gh, gw, H, float(scale), table.data_ptr(), rowmax.data_ptr(), nrd,
+    def attention_relpos(self, qkv, B, gh, gw, H, scale, table, nrd, out):
+        _lib.check(self.L.dm_attention_relpos_f16(qkv.data_ptr(), B, gh, gw, H, float(scale), table.data_ptr(), nrd,
                                                   out.data_ptr(), _lib.stream_ptr()), "dm_attention_relpos_f16")
         self.launches += 1
 
@@ -164,7 +164,7 @@ def _pad_vec(b, n):
 
 
 class DepthAnythingV2Engine:
-    """Depth-Anything-V2 (DINOv2 ViT + DPT head) forward on the sm_100a kernels.
+    """Depth-Anything-V2 (DINOv2 ViT + DPT head) forward on the sm_90a kernels.
 
     Mirrors DepthAnythingV2.forward / DPTHead.forward / DINOv2.get_intermediate_layers of the reference
     (ddepth_anything_v2/depth_anything_v2/dpt.py:117-184, dinov2.py:297-321) plus image2tensor (dpt.py:196-221) and the
@@ -488,7 +488,7 @@ def _gen_relative_position_index(wh, ww):
 
 
 class DptBeitEngine(DepthAnythingV2Engine):
-    """MiDaS 3.1 DPT-BEiT (dpt_beit_large_512 / _384) on the sm_100a kernels.
+    """MiDaS 3.1 DPT-BEiT (dpt_beit_large_512 / _384) on the sm_90a kernels.
 
     Mirrors the reference's overriding forwards (dmidas/backbones/beit.py:18-129), the reassemble stage
     (dmidas/backbones/utils.py:28-39,83-124,144-249), DPT / DPTDepthModel (dmidas/dpt_depth.py:110-166) and estimatemidas
@@ -567,7 +567,6 @@ class DptBeitEngine(DepthAnythingV2Engine):
             old_h = old_w = 2 * win - 1
             new_h, new_w = 2 * gh - 1, 2 * gw - 1
             out = []
-            idx = _gen_relative_position_index(gh, gw).to(self.device)       # [N, N]
             nrd_new = new_h * new_w + 3
             heads = self.cfg['heads']
             for t in self._tables:
@@ -575,28 +574,21 @@ class DptBeitEngine(DepthAnythingV2Engine):
                 src = np.ascontiguousarray(t.cpu().numpy(), dtype=np.float32)
                 dst = np.empty((heads, nrd_new), dtype=np.float32)
                 _lib.check(self.ops.L.dm_beit_rel_table(src.ctypes.data, win, heads, gh, gw, dst.ctypes.data), "dm_beit_rel_table")
-                tab = torch.from_numpy(dst).to(self.device)
-                # per (head, query) maximum of the bias over all keys: the round-1 kernel's row-max upper bound
-                rowmax = torch.stack([tab[hh][idx].max(dim=1).values for hh in range(tab.shape[0])]).contiguous()
-                out.append((tab, rowmax))
+                out.append(torch.from_numpy(dst).to(self.device))
             self._bias_cache = {key: (out, new_h * new_w + 3)}  # keep one resolution resident (drops dense tables too)
         return self._bias_cache[key]
 
     @staticmethod
     def table_fits_on_chip(gh, gw):
-        """The table attention modes keep one head's bias table (twice, reversed, for 16-aligned grids) and the per-key
-        offsets in the 60.75 KB of shared memory the kernel has left (csrc/attention_tcgen05.cu, A4_TAB_MAX)."""
+        """The table attention mode keeps one head's bias table and the per-key offsets in the shared memory the kernel
+        has left beside its Q / K / V tiles (csrc/attention_wgmma.cu: AT_SMEM_MAX - AT_TAB_OFF)."""
         nrd, N = (2 * gh - 1) * (2 * gw - 1) + 3, gh * gw + 1
-        if gw % 16 == 0:
-            nrd_pad = ((nrd + 16) & ~31) + 16                 # csrc/attention_tcgen05.cu: attn4_nrd_pad
-            need = 8 * nrd_pad + 2 * (((N + 126) // 128) * 8 + 8) + 16
-        else:
-            need = 4 * ((nrd + 3) & ~3) + 2 * ((N + 127) // 128) * 128 + 16
-        return need <= 227 * 1024 - 170240
+        need = 4 * ((nrd + 3) & ~3) + 2 * ((N + 127) // 128) * 128
+        return need <= 227 * 1024 - (5 * 16384 + 64)
 
     def dense_bias(self, gh, gw):
-        """Fallback for windows whose table does not fit on chip (e.g. a 3:2 image on dpt_beit_large_512: net 768x512,
-        nrd = 5988): the gather half of _get_rel_pos_bias (beit.py:52-62) done once per resolution into a dense fp16
+        """Fallback for windows whose table does not fit on chip (from about 96 x 96 patches, nrd = 36484, upwards; a 3:2
+        image on dpt_beit_large_512, net 768x512, nrd = 5988, fits): the gather half of _get_rel_pos_bias (beit.py:52-62) done once per resolution into a dense fp16
         [heads, N, ld] tensor per block (ld = N rounded up to whole 128-key tiles), added inside the attention kernel."""
         import torch
         key = ('dense', gh, gw)
@@ -606,7 +598,7 @@ class DptBeitEngine(DepthAnythingV2Engine):
             N = gh * gw + 1
             ld = _ru(N, 128)
             out = []
-            for tab, _ in tabs:
+            for tab in tabs:
                 d = torch.zeros(tab.shape[0], N, ld, dtype=torch.float16, device=self.device)
                 d[:, :, :N] = (tab / 1.4426950408889634)[:, idx.view(-1)].view(-1, N, N).to(torch.float16)
                 out.append(d)
@@ -619,7 +611,7 @@ class DptBeitEngine(DepthAnythingV2Engine):
             dense, ld = self.dense_bias(gh, gw)
             self.ops.attention(b['qkv'], B, N, heads, (C // heads) ** -0.5, b['att'], bias=dense[i], bias_ld=ld)
             return
-        self.ops.attention_relpos(b['qkv'], B, gh, gw, heads, (C // heads) ** -0.5, tabs[i][0], tabs[i][1], nrd, b['att'])
+        self.ops.attention_relpos(b['qkv'], B, gh, gw, heads, (C // heads) ** -0.5, tabs[i], nrd, b['att'])
 
     def emit_feature(self, b, fi, B, N, C):
         """forward hook on the raw block output + ProjectReadout: GELU(Linear(cat(tokens, cls)))."""
@@ -630,7 +622,7 @@ class DptBeitEngine(DepthAnythingV2Engine):
 
 
 class DptVitEngine(DptBeitEngine):
-    """MiDaS 3.0 dpt_large_384 (model type 3) on the sm_100a kernels, op-level path: timm's vit_large_patch16_384 driven by
+    """MiDaS 3.0 dpt_large_384 (model type 3) on the sm_90a kernels, op-level path: timm's vit_large_patch16_384 driven by
     the reference's forward_flex (dmidas/backbones/vit.py:12-79,107-118) — absolute position embedding resized bilinearly to
     the current grid, plain (un-biased) attention, no LayerScale — with the hooks, ProjectReadout, reassemble stage and DPT
     decoder it shares with the BEiT models (dmidas/dpt_depth.py:31-166)."""
@@ -678,7 +670,7 @@ class DptVitEngine(DptBeitEngine):
 
 
 class LeresEngine:
-    """LeReS / res101 (model type 0) on the sm_100a kernels: estimateleres (src/depthmap_generation.py:406-440) around
+    """LeReS / res101 (model type 0) on the sm_90a kernels: estimateleres (src/depthmap_generation.py:406-440) around
     RelDepthModel('resnext101') (lib/multi_depth_model_woauxi.py:6-32, lib/Resnext_torch.py:60-220, lib/network_auxi.py:15-215).
     NHWC fp16 activations, fp32 accumulation.  1x1 convolutions are GEMMs, 3x3 ones the implicit-GEMM conv; the 32-group 3x3
     convolutions use block-diagonal dense filters (exact: the extra products are zeros), the three stride-2 ones go through the
@@ -1070,7 +1062,7 @@ ZOE_CONFIG = dict(n_bins=64, emb=128, min_temp=0.0212, max_temp=50.0, router_dim
 
 
 class ZoeDepthNKEngine(DptBeitEngine):
-    """ZoeDepth-NK (model types 7-9 share this head family; 9 = zoedepth_nk) on the sm_100a kernels: DepthModel.infer_pil
+    """ZoeDepth-NK (model types 7-9 share this head family; 9 = zoedepth_nk) on the sm_90a kernels: DepthModel.infer_pil
     (pad + flip test-time augmentation, dzoedepth/models/depth_model.py:57-152), PrepForMidas (base_models/midas.py:175-186),
     the DPT-BEiT-L-384 core with MidasCore's hooks (midas.py:258-319) and the metric head of ZoeDepthNK.forward
     (zoedepth_nk/zoedepth_nk_v1.py:159-243).  Image b and its horizontal flip run as forwards 2b / 2b+1 of ONE batch; the
@@ -1343,7 +1335,7 @@ class ModelHolder:
         if tiling_mode:
             raise NotImplementedError("tiling_mode (circular conv padding) is not implemented in depthmap_b200 yet")
         if getattr(self, "no_half", False):
-            # reference: `no_half` keeps the network in fp32 (src/depthmap_generation.py:268-275).  The B200 path feeds the tensor
+            # reference: `no_half` keeps the network in fp32 (src/depthmap_generation.py:268-275).  The H100 path feeds the tensor
             # cores fp16 operands (fp32 accumulation, fp32 residual stream) and has no fp32-operand variant: say so instead of
             # silently ignoring the setting
             raise NotImplementedError("no_half (fp32 network) is not implemented in depthmap_b200: the tensor-core path uses fp16 operands "

@@ -1,4 +1,4 @@
-"""Normal maps on B200 — drop-in for the reference's ``src/normalmap_generation.py``.
+"""Normal maps on H100 — drop-in for the reference's ``src/normalmap_generation.py``.
 
 ``create_normalmap`` keeps the reference signature and return type (PIL RGB, 8-bit); ``create_normalmap_batch`` is the
 additive batched device face.  Compute = ``dm_normalmap`` (csrc/normalmap.cu).

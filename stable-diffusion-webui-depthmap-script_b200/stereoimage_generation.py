@@ -1,4 +1,4 @@
-"""Stereo pair generation on B200 — drop-in for the reference's ``src/stereoimage_generation.py``.
+"""Stereo pair generation on H100 — drop-in for the reference's ``src/stereoimage_generation.py``.
 
 ``create_stereoimages`` keeps the reference signature, argument meaning, return type (list of PIL RGB images) and
 error behaviour (src/stereoimage_generation.py:13-74); the per-row warp + gap-fill + packing runs in the

@@ -1,4 +1,4 @@
-"""Video mode's cross-frame depth normalisation on B200 — drop-in for ``process_predicitons`` of the reference's
+"""Video mode's cross-frame depth normalisation on H100 — drop-in for ``process_predicitons`` of the reference's
 ``src/video_mode.py:103-128`` (the misspelt name is the reference's), SURVEY.md §8(f) rank 1.
 
 ``process_predicitons(predictions, smoothening)`` keeps the reference's contract: a list of float32 [H,W] raw predictions in,

@@ -55,7 +55,14 @@ def main():
         if name != "flat":
             for ci, (pb, sb, qb, inv) in enumerate(NORMAL_CASES):
                 out[f"normal_{name}_{ci}"] = np.asarray(refn.create_normalmap(dep, pb, sb, qb, inv))
-    np.savez_compressed(os.path.join(HERE, "stereo_normal_golden.npz"), **out)
+    # split over four files of less than 1 MB each, largest arrays dealt first to the emptiest file
+    parts, sizes = [{} for _ in range(4)], [0] * 4
+    for k in sorted(out, key=lambda k: -np.asarray(out[k]).nbytes):
+        i = sizes.index(min(sizes))
+        parts[i][k] = out[k]
+        sizes[i] += np.asarray(out[k]).nbytes
+    for i, part in enumerate(parts):
+        np.savez_compressed(os.path.join(HERE, f"stereo_normal_golden_{i}.npz"), **part)
     print("wrote", len(out), "arrays")
 
     # funnel normalisation (src/core.py:189-211 + convert_to_i16) — executed through the reference's own functions

@@ -6,7 +6,7 @@ fp16 weights, fp16 activations, fp16 residual stream).  `reference_fp16_error` e
 on the GPU box (the oracle is pinned to the reference module, so this is the reference's own GPU arithmetic up to kernel
 selection) and the bar for the product is:  max error <= max(1e-3, 1.25 x the reference-policy max error on the same input)
 (1.5 x for the tiny ZoeDepth test networks, whose near-argmax bin selection turns rounding noise into isolated outlier pixels);  mean error < max(4e-4, 1.5 x the
-reference-policy mean error).  Both numbers are printed by every test; profiles/r02_precision.txt keeps the table."""
+reference-policy mean error).  Both numbers are printed by every test."""
 import numpy as np
 
 TOL_NORTH_STAR = 1e-3

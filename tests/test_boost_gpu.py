@@ -1,4 +1,4 @@
-"""GPU: BOOST (SURVEY §8a row D9) — the merge U-Net and estimateboost on the sm_100a kernels against the oracle (oracle/pix2pix.py,
+"""GPU: BOOST (SURVEY §8a row D9) — the merge U-Net and estimateboost on the sm_90a kernels against the oracle (oracle/pix2pix.py,
 oracle/boost.py, oracle/leres.py; all three pinned to the reference in tests/test_oracle_pin.py).  The reference runs both networks
 in fp32 when boost is on (src/depthmap_generation.py:268-275), so there is no fp16 yardstick: the merge network uses split-operand
 (fp32-class) GEMMs and is held to 1e-4; the end-to-end result carries the fp16-operand LeReS forwards and is reported against

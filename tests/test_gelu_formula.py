@@ -1,4 +1,4 @@
-"""Host check of the single-MUFU GELU used by the GEMM epilogue (csrc/gemm_tcgen05.cu: gelu_erf2): the same fp32
+"""Host check of the single-MUFU GELU used by the GEMM epilogue (csrc/gemm_wgmma.cu: gelu_erf): the same fp32
 arithmetic, step by step in numpy, against x * Phi(x) in float64 (torch.nn.GELU() of the reference networks is the erf form:
 dmidas/backbones/beit.py Mlp, ddepth_anything_v2/dinov2_layers/mlp.py)."""
 import numpy as np

@@ -1,4 +1,4 @@
-"""GPU: tcgen05 GEMM / implicit-GEMM conv building blocks vs a plain PyTorch fp32 reference of the same op."""
+"""GPU: wgmma GEMM / implicit-GEMM conv building blocks vs a plain PyTorch fp32 reference of the same op."""
 import numpy as np
 import pytest
 
@@ -54,3 +54,21 @@ def test_conv3x3_f16(cuda_device, B, H, W, Cin, Cout):
     ref = torch.relu(torch.nn.functional.conv2d(x.float().permute(0, 3, 1, 2), w.float(), bias, padding=1)).permute(0, 2, 3, 1)
     err = (out.float() - ref).abs().max().item()
     assert err < 1e-2 * max(1.0, ref.abs().max().item()), err
+
+
+def test_gemm_rejects_operands_the_epilogue_cannot_address(cuda_device):
+    """The epilogue stores column pairs: an odd output pitch or an output that is not aligned to a pair is DM_E_INVALID,
+    not a misaligned access inside the kernel."""
+    import torch
+    L, lib = _lib()
+    M, N, K = 128, 64, 64
+    A = torch.zeros(M, K, dtype=torch.float16, device=cuda_device)
+    W = torch.zeros(N, K, dtype=torch.float16, device=cuda_device)
+    C16 = torch.zeros(M * (N + 2) + 2, dtype=torch.float16, device=cuda_device)
+    C32 = torch.zeros(M * (N + 2) + 2, dtype=torch.float32, device=cuda_device)
+    for out, out_f32 in ((C16, 0), (C32, 1)):
+        esz = out.element_size()
+        assert lib.dm_gemm_f16(A.data_ptr(), K, W.data_ptr(), K, None, out.data_ptr(), N + 2, M, N, K, 0, out_f32, L.stream_ptr()) == L.DM_OK
+        assert lib.dm_gemm_f16(A.data_ptr(), K, W.data_ptr(), K, None, out.data_ptr(), N + 1, M, N, K, 0, out_f32, L.stream_ptr()) == L.DM_E_INVALID
+        assert lib.dm_gemm_f16(A.data_ptr(), K, W.data_ptr(), K, None, out.data_ptr() + esz, N + 2, M, N, K, 0, out_f32, L.stream_ptr()) == L.DM_E_INVALID
+    torch.cuda.synchronize()

@@ -16,7 +16,11 @@ MODES = ['left-right', 'red-cyan-anaglyph', 'top-bottom', 'cyan-red-reverseanagl
 
 @pytest.fixture(scope="module")
 def gold():
-    return np.load(os.path.join(G, "stereo_normal_golden.npz"))
+    out = {}                                   # the vectors are split over files of less than 1 MB each
+    for f in sorted(os.listdir(G)):
+        if f.startswith("stereo_normal_golden_") and f.endswith(".npz"):
+            out.update(np.load(os.path.join(G, f)))
+    return out
 
 
 @pytest.mark.parametrize("name", ["smooth", "noise", "black", "flat"])

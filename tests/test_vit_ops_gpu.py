@@ -129,15 +129,15 @@ def test_im2col_s2_matches_conv(cuda_device):
 
 @pytest.mark.parametrize("B,gh,gw,H", [(1, 4, 4, 1), (2, 8, 6, 2), (2, 32, 32, 16), (1, 24, 24, 3), (1, 16, 16, 2), (2, 24, 16, 3),
                                         (1, 20, 32, 2), (1, 9, 48, 1)])
-@pytest.mark.parametrize("generic", [False, True])
-def test_attention_relpos_table(cuda_device, B, gh, gw, H, generic, monkeypatch):
-    """BEiT relative-position bias generated inside the kernel vs the dense [H,N,N] gather of the reference.  Grids whose
-    width is a multiple of 16 take the class-token-shifted tiling (contiguous table reads, SIMT class row) unless
-    DEPTHMAP_B200_ATTN_GENERIC=1; both table modes are checked on every grid."""
+@pytest.mark.parametrize("mode", ["table", "dense"])
+def test_attention_relpos_table(cuda_device, B, gh, gw, H, mode):
+    """BEiT relative-position bias vs the dense [H,N,N] gather of the reference, on every grid through both ways the engine
+    has of applying it: "table" = generated inside the kernel from the per-head table in shared memory
+    (dm_attention_relpos_f16), "dense" = the fp16 [H, N, ld] bias the engine builds for windows whose table does not fit
+    on chip (dm_attention_f16 with a bias, as DptBeitEngine.dense_bias lays it out)."""
     import torch
     from oracle.beit_dpt import gen_relative_position_index
     L, lib = _lib()
-    monkeypatch.setenv("DEPTHMAP_B200_ATTN_GENERIC", "1" if generic else "0")
     N, C = gh * gw + 1, H * 64
     nrd = (2 * gh - 1) * (2 * gw - 1) + 3
     g = torch.Generator(device="cpu").manual_seed(gh * 100 + gw)
@@ -147,9 +147,14 @@ def test_attention_relpos_table(cuda_device, B, gh, gw, H, generic, monkeypatch)
     bias = table[idx.view(-1)].view(N, N, H).permute(2, 0, 1)
     tab_k = (table.t().contiguous() * 1.4426950408889634).float().contiguous()
     out = torch.full((B * N, C), float("nan"), dtype=torch.float16, device=cuda_device)
-    rowmax = (bias.max(dim=2).values * 1.4426950408889634).float().contiguous()
-    L.check(lib.dm_attention_relpos_f16(qkv.data_ptr(), B, gh, gw, H, 0.125, tab_k.data_ptr(), rowmax.data_ptr(), nrd, out.data_ptr(),
-                                        L.stream_ptr()))
+    if mode == "table":
+        L.check(lib.dm_attention_relpos_f16(qkv.data_ptr(), B, gh, gw, H, 0.125, tab_k.data_ptr(), nrd, out.data_ptr(), L.stream_ptr()))
+    else:
+        ld = (N + 127) // 128 * 128
+        dense = torch.zeros(H, N, ld, dtype=torch.float16, device=cuda_device)
+        dense[:, :, :N] = (tab_k / 1.4426950408889634)[:, idx.view(-1)].view(H, N, N).to(torch.float16)
+        L.check(lib.dm_attention_f16(qkv.data_ptr(), B, N, H, 0.125, dense.data_ptr(), ld, out.data_ptr(), L.stream_ptr()))
+        bias = dense[:, :, :N].float()                 # the reference adds the bias the kernel was given (rounded to fp16)
     torch.cuda.synchronize()
     q, k, v = qkv.float().view(B, N, 3, H, 64).permute(2, 0, 3, 1, 4)
     s = (q * 0.125) @ k.transpose(-1, -2) + bias.unsqueeze(0)
@@ -161,8 +166,8 @@ def test_attention_relpos_table(cuda_device, B, gh, gw, H, generic, monkeypatch)
 
 @pytest.mark.parametrize("N", [1025, 700])
 def test_attention_rising_scores_force_rescale(cuda_device, N):
-    """Keys grow along the sequence so the running row max jumps by far more than 2^8 from tile to tile: exercises the
-    lazy-rescale path (tile redone against the raised max, accumulated output and row sum scaled down)."""
+    """Keys grow along the sequence so the running row max rises by a large factor from tile to tile: exercises the
+    online-softmax rescale (accumulated output and row sum scaled down by 2^(old max - new max) before each tile is added)."""
     import torch
     L, lib = _lib()
     B, H = 1, 2

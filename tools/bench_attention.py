@@ -1,5 +1,4 @@
 """Tool: times the fused attention kernel alone on the two bench shapes (CUDA events, 20 launches after 3 warm-ups).
-DEPTHMAP_B200_ATTN_PTMEM=0 / DEPTHMAP_B200_ATTN_TOKEN=0 select the measured variants of the kernel for A/B timing (read once per process).
 usage: python tools/bench_attention.py [beit|dav2|both]"""
 import os
 import sys
@@ -37,10 +36,9 @@ def main():
         nrd = (2 * gh - 1) * (2 * gw - 1) + 3
         qkv = torch.randn(B * N, 3 * C, generator=g).half().to(dev)
         tab = (torch.randn(H, nrd, generator=g) * 2).float().to(dev).contiguous()
-        rowmax = tab.max(dim=1, keepdim=True).values.expand(H, N).contiguous()
         out = torch.empty(B * N, C, dtype=torch.float16, device=dev)
         run("beit512 B=32 N=1025 relpos", lambda: L.check(lib.dm_attention_relpos_f16(
-            qkv.data_ptr(), B, gh, gw, H, 0.125, tab.data_ptr(), rowmax.data_ptr(), nrd, out.data_ptr(), L.stream_ptr())),
+            qkv.data_ptr(), B, gh, gw, H, 0.125, tab.data_ptr(), nrd, out.data_ptr(), L.stream_ptr())),
             4.0 * B * H * N * N * 64)
     if which in ("dav2", "both"):
         B, N = 32, 1370

@@ -1,4 +1,4 @@
-"""Micro-benchmark of the tcgen05 GEMM: isolates main loop vs epilogue cost.  Prints TFLOP/s per configuration."""
+"""Micro-benchmark of the wgmma GEMM: isolates main loop vs epilogue cost.  Prints TFLOP/s per configuration."""
 import ctypes, os, sys
 sys.path.insert(0, os.getcwd())
 import torch
@@ -36,8 +36,6 @@ def run(M, N, K, mode, iters=10):
     ms = e0.elapsed_time(e1) / iters
     print(f"M={M} N={N} K={K} {mode:6s} {ms:8.3f} ms {2.0*M*N*K/ms/1e9:8.1f} TFLOP/s", flush=True)
 
-tag = 'NO_PERSIST' if os.environ.get('DEPTHMAP_B200_NO_PERSIST') == '1' else 'persist'
-print('==', tag)
 for (M, N, K) in [(32800, 4096, 1024), (32800, 1024, 4096), (32800, 3072, 1024), (32800, 1024, 1024)]:
     for mode in ['plain', 'bias', 'gelu', 'resid', 'f32']:
         run(M, N, K, mode)

@@ -1,4 +1,4 @@
-"""Tool: two properties of the fp16 tcgen05 GEMM that decide how the split-operand (fp32-class) mode must be built
+"""Tool: two properties of the fp16 wgmma GEMM that decide how the split-operand (fp32-class) mode must be built
 (csrc/boost_kernels.cu, depthmap_b200/boost.py): (1) are fp16 SUBNORMAL operands honoured or flushed; (2) how does the error of
 the tensor core's own fp32 accumulation grow with the GEMM depth K (rounding grows like sqrt(K), alignment-truncation like K).
 usage: python tools/probe_tensor_core.py"""
