@@ -157,10 +157,20 @@ int dm_attention_f16(const void *qkv, int B, int N, int H, float scale, const vo
  * nrd = (2gh-1)(2gw-1)+3, N = gh*gw+1 tokens (class token first).  No [H,N,N] bias tensor is read by the kernel. */
 int dm_attention_relpos_f16(const void *qkv, int B, int gh, int gw, int H, float scale, const float *rel_table_log2e,
                             int nrd, void *out, void *stream);
+/* Any window: per 128-key tile the kernel stages only the table rows the tile pair spans, read from L2 (the table is at most
+ * ~160 KB per head at 100 x 100). */
 /* uint8 RGB [B,H,W,3] -> (cv2-style bicubic resize to net_h x net_w) -> (x/255 - mean)/std -> fp16 patch matrix
  * [B*(net_h/patch)*(net_w/patch), kpad], K ordered (c, ky, kx); network channel c reads source channel chan_map[c]. */
 int dm_preprocess_patchify(const uint8_t *rgb, int B, int H, int W, int net_h, int net_w, int patch, const float *mean_host,
                            const float *std_host, const int *chan_map_host, void *out, int kpad, void *stream);
+/* The same for B crops of one planar fp32 image [3, Hi, Wi] (values used as they are, no /255), all resized to net_h x net_w:
+ * rects_dev: DEVICE int32 [B][4] = x0, y0, w, h inside the image (validated by the caller), 16-byte aligned (DM_E_INVALID
+ * otherwise).  BOOST's estimatemidasBoost
+ * (src/depthmap_generation.py:1180-1203): cv2 INTER_CUBIC resize of the float crop (a copy when the sizes match), then
+ * (x - mean) / std, then network channel c reads plane chan_map[c]. */
+int dm_preprocess_patchify_f32_crops(const float *img, int Hi, int Wi, const int *rects_dev, int B, int net_h, int net_w, int patch,
+                                     const float *mean_host, const float *std_host, const int *chan_map_host, void *out, int kpad,
+                                     void *stream);
 /* X[b,0,:] = cls + pos[0]; X[b,1+p,:] = pe[b*Np+p,:] + pos[1+p]  (pos may be NULL); X fp32 [B, Np+1, C] */
 int dm_assemble_tokens(const void *pe, const float *cls, const float *pos, float *X, int B, int Np, int C, void *stream);
 /* LayerNorm over the last dim of fp32 x [rows, C] -> fp16; drop_first != 0 skips token 0 of every image (tokens_per_img) */
@@ -305,6 +315,9 @@ int dm_boost_minmax(const float *x, long long n, float *partial /*[partials][2]*
 int dm_boost_merge_input(const float *outer, const float *inner, long long n, const float *p_outer, const float *p_inner, float *out /*[n,2]*/,
                          void *stream);
 int dm_boost_post(const float *t, long long n, const float *partial, int normalise, float *out, void *stream);
+/* out = (x - min) / (max - min) with min / max folded from dm_boost_minmax's partials (estimatemidasBoost, :1212-1220); a spread of
+ * at most float64 eps writes zeros and sets *degenerate (device int) to 1 */
+int dm_boost_minmax_normalise(const float *x, long long n, const float *partial, float *out, int *degenerate, void *stream);
 int dm_boost_fit_sums(const float *x, const float *y, long long n, double *partial /*[partials][4]*/, void *stream);
 int dm_boost_blend(const float *mapped /*[S,S]*/, int S, const double *fit_partial, const float *profile, int n_profile, float *updated, int pitch,
                    int x1, int y1, int w, int h, void *stream);

@@ -70,7 +70,8 @@ EXPORTS = [
     "dm_normalize_u16_workspace_bytes", "dm_normalize_u16", "dm_normalize_u16_outliers_workspace_bytes", "dm_normalize_u16_outliers",
     "dm_stereo_workspace_bytes", "dm_stereo", "dm_stereo_pack", "dm_depth_to_nd64", "dm_convert_to_i16_f64",
     "dm_normalmap_workspace_bytes", "dm_normalmap",
-    "dm_gemm_ex", "dm_conv3x3_ex", "dm_gemm_f16", "dm_conv3x3_f16", "dm_attention_f16", "dm_attention_relpos_f16", "dm_preprocess_patchify",
+    "dm_gemm_ex", "dm_conv3x3_ex", "dm_gemm_f16", "dm_conv3x3_f16", "dm_attention_f16", "dm_attention_relpos_f16",
+    "dm_preprocess_patchify", "dm_preprocess_patchify_f32_crops",
     "dm_assemble_tokens", "dm_layernorm_f16", "dm_resize_bilinear_nhwc_f16", "dm_resize_f32", "dm_im2col_s2_f16", "dm_concat_readout_f16",
     "dm_zoe_preprocess_patchify", "dm_layernorm_post_f16", "dm_attention_small_f16", "dm_cast_f32_f16", "dm_zoe_select_softplus",
     "dm_resize_add_nhwc_f16", "dm_zoe_attractor", "dm_zoe_clb_final", "dm_zoe_tta_combine",
@@ -80,7 +81,7 @@ EXPORTS = [
     "dm_leres_stem_im2col", "dm_maxpool3x3s2_nhwc_f16", "dm_subsample2_nhwc_f16", "dm_add_f16", "dm_resize_f32_ld",
     "dm_boost_partials", "dm_unet_first_cols", "dm_unet_down_cols", "dm_unet_up_cols", "dm_unet_interleave", "dm_unet_final", "dm_unet_first", "dm_unet_last", "dm_sum_chunks_f32", "dm_boost_minmax",
     "dm_boost_merge_input", "dm_boost_post", "dm_boost_fit_sums", "dm_boost_blend", "dm_boost_resize_cubic", "dm_boost_u8_to_planar",
-    "dm_leres_stem_im2col_f32", "dm_leres_stem_im2col_f32_batch",
+    "dm_leres_stem_im2col_f32", "dm_leres_stem_im2col_f32_batch", "dm_boost_minmax_normalise",
 ]
 
 
@@ -155,6 +156,8 @@ def _bind_optional(L):
     if hasattr(L, "dm_layernorm_f16"):
         L.dm_preprocess_patchify.argtypes = [vp, i32, i32, i32, i32, i32, i32, c.POINTER(c.c_float), c.POINTER(c.c_float),
                                              c.POINTER(c.c_int), vp, i32, vp]
+        L.dm_preprocess_patchify_f32_crops.argtypes = [vp, i32, i32, vp, i32, i32, i32, i32, c.POINTER(c.c_float), c.POINTER(c.c_float),
+                                                       c.POINTER(c.c_int), vp, i32, vp]
         L.dm_assemble_tokens.argtypes = [vp, vp, vp, vp, i32, i32, i32, vp]
         L.dm_layernorm_f16.argtypes = [vp, c.c_longlong, i32, vp, vp, f32, vp, i32, i32, vp]
         L.dm_resize_bilinear_nhwc_f16.argtypes = [vp, i32, i32, i32, i32, vp, i32, i32, vp]
@@ -181,6 +184,7 @@ def _bind_optional(L):
         L.dm_boost_merge_input.argtypes = [vp, vp, ll, vp, vp, vp, vp]
         L.dm_boost_post.argtypes = [vp, ll, vp, i32, vp, vp]
         L.dm_boost_fit_sums.argtypes = [vp, vp, ll, vp, vp]
+        L.dm_boost_minmax_normalise.argtypes = [vp, ll, vp, vp, vp, vp]
         L.dm_boost_blend.argtypes = [vp, i32, vp, vp, i32, vp, i32, i32, i32, i32, i32, vp]
         L.dm_boost_resize_cubic.argtypes = [vp, i32, ll, i32, i32, vp, i32, ll, i32, i32, i32, vp]
         L.dm_boost_u8_to_planar.argtypes = [vp, i32, i32, vp, vp]

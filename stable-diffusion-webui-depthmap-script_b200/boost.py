@@ -8,7 +8,9 @@ pix2pix/models/networks.py:444-543 (UnetGenerator 'unet_1024', norm 'none'), pix
 Split of work.  The CONTROL PLANE stays on the host exactly as in the reference, because its results are integers that must not
 move: the R_x resolution search and the patch selection look only at the RGB image (Sobel gradients, thresholds, an integral
 image) and run through the same cv2 calls.  Every PIXEL of the depth result is produced on the GPU: the float image and its two
-cubic resizes, the LeReS forwards on crops (csrc/boost_kernels.cu: leres_stem_im2col_f32), the cubic resizes to and from the
+cubic resizes, the base-network forwards on crops (LeReS, model type 0: csrc/boost_kernels.cu leres_stem_im2col_f32; the MiDaS DPT
+models 1-3 through estimatemidasBoost, :1180-1220: csrc/vit_kernels.cu preprocess_patchify_f32_crops, then the per-call min-max
+normalisation at crop size), the cubic resizes to and from the
 1024^2 merge resolution, the merge U-Net (split-operand fp32-class GEMMs), min-max normalisations, the degree-1 least-squares fit
 (fp64 sums) and the Gaussian-mask blend; one device->host copy at the end.
 
@@ -363,17 +365,23 @@ class UnetMergeEngine:
 # ---------------------------------------------------------------------------------------------------------------------
 # data plane
 # ---------------------------------------------------------------------------------------------------------------------
+BASE_NETWORKS = (0, 1, 2, 3)      # LeReS res101; DPT-BEiT-L 512, DPT-BEiT-L 384, DPT-Large 384 (singleestimate, :1053-1066)
+
+
 class BoostPipeline:
     """estimateboost for one image on one GPU (or one rank of a patch-parallel group)."""
 
     def __init__(self, depth_engine, merge_engine, device, model_type=0):
         import torch
-        if model_type != 0:
-            raise NotImplementedError("boost is built for the reference's default base network, LeReS res101 (model type 0)")
+        if model_type not in BASE_NETWORKS:
+            raise NotImplementedError(f"boost is built for the base networks LeReS res101 (model type 0) and the MiDaS DPT models (1, 2, 3), "
+                                      f"not model type {model_type}")
         self.depth, self.merge, self.device, self.model_type = depth_engine, merge_engine, device, model_type
+        self.midas = model_type != 0      # estimatemidasBoost: crop-size min-max normalisation of every estimate
         self.L = _lib.load()
         self.P = int(self.L.dm_boost_partials())
         self.profile = torch.from_numpy(mask_profile()).to(device)
+        self._degenerate = torch.zeros(1, dtype=torch.int32, device=device)
         self.launches = 0
 
     # -- small device helpers ---------------------------------------------------------------------------------------
@@ -413,9 +421,23 @@ class BoostPipeline:
         self.launches += 1
         return out
 
+    def _normalise_estimate(self, est):
+        """estimatemidasBoost's tail (:1212-1220): (p - min) / (max - min) of the crop-size prediction; a constant prediction is
+        flagged on the device and reported by run() (the reference returns a scalar there and its next cv2.resize fails)"""
+        import torch
+        out = torch.empty_like(est)
+        p = self._minmax(est)
+        _lib.check(self.L.dm_boost_minmax_normalise(est.data_ptr(), est.numel(), p.data_ptr(), out.data_ptr(), self._degenerate.data_ptr(),
+                                                    _lib.stream_ptr()), "dm_boost_minmax_normalise")
+        self.launches += 1
+        return out
+
     def _estimate_1024(self, planar, rect, msize):
-        """singleestimate on a crop (LeReS at msize x msize, cubic back to the crop size) followed by the cubic resize to 1024^2"""
+        """singleestimate on a crop (LeReS at msize x msize or the DPT at its upper-bound net size, cubic back to the crop size;
+        min-max normalised for the DPT) followed by the cubic resize to 1024^2"""
         est = self.depth.forward_batch(None, msize, msize, planar=(planar, rect))[0]
+        if self.midas:
+            est = self._normalise_estimate(est)
         return self._cubic(est.data_ptr(), rect[2], rect[3], rect[2], PIX2PIX_SIZE, PIX2PIX_SIZE)
 
     def double_estimate(self, planar, rect, size1, size2):
@@ -424,7 +446,7 @@ class BoostPipeline:
         high = self._estimate_1024(planar, rect, size2)
         return self._post(self._merge(low, high), True)
 
-    PATCH_BATCH = 8      # crops per LeReS forward in the patch loop (activation memory of the 896 net: ~1.5 GB per crop)
+    PATCH_BATCH = 8      # crops per base-network forward in the patch loop (LeReS 896 net: ~1.5 GB per crop; BEiT-L 1024 net: ~1 GB)
 
     def fitted_patches(self, work_img, base, rects, rf):
         """fitted_patch for a list of patches with the base network BATCHED over the crops (all patches use the same two net sizes);
@@ -441,7 +463,10 @@ class BoostPipeline:
                 x, y, w, h = rect
                 ests = []
                 for net, src in ((rf, low[k]), (2 * rf, high[k])):      # cubic back to the crop's size (estimateleres), then to 1024^2 (doubleestimate)
-                    at_crop = self._cubic(src.data_ptr(), net, net, net, h, w)
+                    if self.midas:                                     # the DPT engines return the crop-size map; estimatemidasBoost normalises it
+                        at_crop = self._normalise_estimate(src)
+                    else:
+                        at_crop = self._cubic(src.data_ptr(), net, net, net, h, w)
                     ests.append(self._cubic(at_crop.data_ptr(), w, h, w, PIX2PIX_SIZE, PIX2PIX_SIZE))
                 est = self._post(self._merge(ests[0], ests[1]), True)
                 yield self.fitted_patch(work_img, base, rect, rf, est=est)
@@ -475,6 +500,7 @@ class BoostPipeline:
         import torch
         rgb_u8 = np.array(rgb_u8, dtype=np.uint8, order='C', copy=True)      # PIL hands out read-only buffers
         H, W = rgb_u8.shape[:2]
+        self._degenerate.zero_()
         if precomputed is None:
             swapped = cv2.cvtColor(rgb_u8, cv2.COLOR_BGR2RGB) / 255.0        # the image the reference's control plane sees (:381)
             p = plan(swapped, self.model_type, whole_size_threshold)
@@ -510,4 +536,6 @@ class BoostPipeline:
             for i, rect in enumerate(rects):                                # the blend is order dependent: every rank replays it in order
                 self.blend(updated, all_m[i].view(PIX2PIX_SIZE, PIX2PIX_SIZE), all_s[i], rect)
         out = self._cubic(updated.data_ptr(), ww, wh, ww, H, W)
+        if self.midas and int(self._degenerate.item()):
+            raise ValueError("boost: the base network returned a constant depth map for a crop (estimatemidasBoost cannot normalise it)")
         return out.cpu().numpy() if to_host else out

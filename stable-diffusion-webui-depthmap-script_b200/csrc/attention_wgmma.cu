@@ -13,9 +13,12 @@
 //                    O += P V_j     wgmma m64n64k16 with A = P packed to fp16 in registers (the S fragment IS the A
 //                    fragment layout, tc_common.cuh) and B = V_j used MN-major, so neither P nor V^T ever touches memory
 // While one warpgroup exponentiates, the other one's MMAs keep the tensor cores busy.
-// Bias modes: 0 none (DINOv2) | 1 dense fp16 [H,N,ld] | 2 BEiT relative-position table: the per-head table [nrd]
-// (pre-multiplied by log2 e) and the per-key offset ky*(2gw-1)+kx live in shared memory and the bias of (q, k) is
-// table[base_q - koff_k] — no [H,N,N] tensor is ever read (the reference materialises it per block per forward).
+// Bias modes: 0 none (DINOv2) | 1 dense fp16 [H,N,ld] | 2 BEiT relative-position table [H, nrd] (pre-multiplied by log2 e),
+// any window: the bias of (q, k) is table[base_q - koff_k] with base_q = (qy+gh-1)(2gw-1) + qx+gw-1 and koff_k = ky(2gw-1) + kx,
+// so no [H,N,N] tensor is ever read (the reference materialises it per block per forward).  A 128-query x 128-key tile pair
+// needs only the table rows dy = qy - ky it spans, (query rows spanned + key rows spanned - 1) x (2gw - 1) contiguous entries
+// (995 floats at 100 x 100).  Warps 1-3 of the producer warpgroup copy that sub-window out of the L2-resident table, with the
+// key offsets rebased onto it (32-bit), into the same 2-stage ring as K / V and arrive on the stage's full barrier.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <math.h>
@@ -43,6 +46,7 @@ struct AttnParams {
     __half *out;            // [B*N, C]
     const float *rel_table; // optional [H, nrd] * log2(e): BEiT relative-position table
     int nrd, gh, gw;
+    int sub_stride;         // mode 2: floats per stage of the streamed sub-window (the last one holds the class-query entry)
 };
 
 constexpr int AT_BQ = 128, AT_BKV = 128, AT_D = 64, AT_STAGES = 2;
@@ -52,8 +56,16 @@ constexpr int AT_KV_BYTES = AT_BKV * AT_D * 2;      // 16 KB each for K and V
 constexpr int AT_K_OFF = AT_Q_BYTES;
 constexpr int AT_V_OFF = AT_K_OFF + AT_STAGES * AT_KV_BYTES;
 constexpr int AT_BAR_OFF = AT_V_OFF + AT_STAGES * AT_KV_BYTES;
-constexpr int AT_TAB_OFF = AT_BAR_OFF + 64;         // relative-position table + key offsets (mode 2)
+constexpr int AT_TAB_OFF = AT_BAR_OFF + 64;         // mode 2: table sub-windows + key offsets, per stage
 constexpr int AT_SMEM_MAX = 227 * 1024;
+constexpr int AT_STAGERS = 96;                      // mode 2: producer warps 1-3 stage the table sub-windows
+
+// mode 2: largest sub-window of a tile pair (+1 for the class-query entry), rounded to 16 bytes.  128 consecutive patch
+// tokens cover at most 127 / gw + 2 grid rows, so a pair spans at most 2 * that - 1 offsets dy.
+static inline int relpos_sub_stride(int gh, int gw) {
+    const int span = gh < (AT_BQ - 1) / gw + 2 ? gh : (AT_BQ - 1) / gw + 2;
+    return ((2 * span - 1) * (2 * gw - 1) + 1 + 3) & ~3;
+}
 
 template <int BIAS_MODE>
 __global__ void __launch_bounds__(AT_THREADS, 1) attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, AttnParams p) {
@@ -61,8 +73,8 @@ __global__ void __launch_bounds__(AT_THREADS, 1) attention_wgmma_kernel(const __
     uint8_t *sQ = smem_raw, *sK = smem_raw + AT_K_OFF, *sV = smem_raw + AT_V_OFF;
     uint64_t *bars = reinterpret_cast<uint64_t *>(smem_raw + AT_BAR_OFF);
     uint64_t *q_full = bars, *kv_full = bars + 1, *kv_empty = bars + 1 + AT_STAGES;
-    float *s_tab = reinterpret_cast<float *>(smem_raw + AT_TAB_OFF);
-    uint16_t *s_koff = reinterpret_cast<uint16_t *>(s_tab + ((p.nrd + 3) & ~3));
+    float *s_tab = reinterpret_cast<float *>(smem_raw + AT_TAB_OFF);                 // mode 2: [stage][sub_stride]
+    int *s_koff = reinterpret_cast<int *>(s_tab + AT_STAGES * p.sub_stride);         // mode 2: [stage][128] after the sub-windows
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int q0 = blockIdx.x * AT_BQ, h = blockIdx.y, b = blockIdx.z;
@@ -72,16 +84,11 @@ __global__ void __launch_bounds__(AT_THREADS, 1) attention_wgmma_kernel(const __
     if (threadIdx.x == 0) {
         prefetch_tmap(&tmQKV);
         mbar_init(q_full, 1);
-        for (int s = 0; s < AT_STAGES; ++s) { mbar_init(&kv_full[s], 1); mbar_init(&kv_empty[s], 8); }   // 8 consumer warps
-        fence_barrier_init();
-    }
-    if (BIAS_MODE == 2) {
-        const float *tab = p.rel_table + (size_t)h * p.nrd;
-        for (int i = threadIdx.x; i < p.nrd; i += AT_THREADS) s_tab[i] = __ldg(tab + i);
-        for (int k = threadIdx.x; k < num_kv * AT_BKV; k += AT_THREADS) {
-            const int t = k - 1;
-            s_koff[k] = (k >= 1 && k < p.N) ? (uint16_t)((t / p.gw) * (2 * p.gw - 1) + (t % p.gw)) : (uint16_t)0;
+        for (int s = 0; s < AT_STAGES; ++s) {
+            mbar_init(&kv_full[s], BIAS_MODE == 2 ? 1 + AT_STAGERS : 1);      // mode 2: + the table stagers
+            mbar_init(&kv_empty[s], 8);                                       // 8 consumer warps
         }
+        fence_barrier_init();
     }
     __syncthreads();
 
@@ -95,6 +102,30 @@ __global__ void __launch_bounds__(AT_THREADS, 1) attention_wgmma_kernel(const __
                 mbar_arrive_expect_tx(&kv_full[s], 2 * AT_KV_BYTES);
                 tma_load_2d(sK + s * AT_KV_BYTES, &tmQKV, &kv_full[s], p.C + h * AT_D, row_base + j * AT_BKV);
                 tma_load_2d(sV + s * AT_KV_BYTES, &tmQKV, &kv_full[s], 2 * p.C + h * AT_D, row_base + j * AT_BKV);
+            }
+        } else if (BIAS_MODE == 2 && warp >= 1) {
+            // Every query / key tile holds at least one patch token (N >= 2); class and padding positions take the offsets of the
+            // nearest patch token of their tile, so every index the consumers form stays inside the sub-window (the values they
+            // read there are replaced or masked).
+            const int st = threadIdx.x - 32, rw = 2 * p.gw - 1;
+            const float *tab = p.rel_table + (size_t)h * p.nrd;
+            const int qy_min = (max(q0, 1) - 1) / p.gw, qy_max = (min(q0 + AT_BQ, p.N) - 2) / p.gw;
+            for (int j = 0; j < num_kv; ++j) {
+                const int s = j % AT_STAGES, kbase = j * AT_BKV;
+                const int k_lo = max(kbase, 1), k_hi = min(kbase + AT_BKV, p.N) - 1;
+                const int ky_min = (k_lo - 1) / p.gw, ky_max = (k_hi - 1) / p.gw;
+                const int lo = (qy_min - ky_max + p.gh - 1) * rw;                 // first table entry of the pair
+                const int cnt = (qy_max - qy_min + ky_max - ky_min + 1) * rw;
+                float *sub = s_tab + s * p.sub_stride;
+                int *kof = s_koff + s * AT_BKV;
+                mbar_wait(&kv_empty[s], ((j / AT_STAGES) & 1) ^ 1);
+                for (int i = st; i < cnt; i += AT_STAGERS) sub[i] = __ldg(tab + lo + i);
+                if (st == 0) sub[p.sub_stride - 1] = __ldg(tab + p.nrd - 3);      // class query -> patch key
+                for (int k = st; k < AT_BKV; k += AT_STAGERS) {
+                    const int t = min(max(kbase + k, k_lo), k_hi) - 1;
+                    kof[k] = (t / p.gw) * rw + (t % p.gw) + lo;
+                }
+                mbar_arrive(&kv_full[s]);
             }
         }
         return;
@@ -116,12 +147,15 @@ __global__ void __launch_bounds__(AT_THREADS, 1) attention_wgmma_kernel(const __
         if (BIAS_MODE == 1) brow[r] = p.bias + ((size_t)h * p.N + qq) * p.bias_ld;
         if (BIAS_MODE == 2) {
             // class-token query: the constant class->patch entry; class-token key: see the k == 0 case below
-            // (dmidas/backbones/beit.py:44-62 assembles exactly these three extra entries)
-            if (qq == 0) { rp_base[r] = p.nrd - 3; rp_mult[r] = 0; rp_k0[r] = s_tab[p.nrd - 1]; }
+            // (dmidas/backbones/beit.py:44-62 assembles exactly these three extra entries).  The key offsets are rebased onto
+            // each tile pair's sub-window, so the query base stays the full-table one; the class->patch entry sits in the
+            // sub-window's last slot.
+            const float *tab = p.rel_table + (size_t)h * p.nrd;
+            if (qq == 0) { rp_base[r] = p.sub_stride - 1; rp_mult[r] = 0; rp_k0[r] = __ldg(tab + p.nrd - 1); }
             else {
                 const int tt = qq - 1, qy = tt / p.gw, qx = tt % p.gw;
                 rp_base[r] = (qy + p.gh - 1) * (2 * p.gw - 1) + (qx + p.gw - 1);
-                rp_k0[r] = s_tab[p.nrd - 2];
+                rp_k0[r] = __ldg(tab + p.nrd - 2);
             }
         }
     }
@@ -138,6 +172,8 @@ __global__ void __launch_bounds__(AT_THREADS, 1) attention_wgmma_kernel(const __
         mbar_wait(&kv_full[s], (j / AT_STAGES) & 1);
         // ---- S = Q K_j^T ---------------------------------------------------------------------------------------------
         float sc[64];
+        const float *sub = s_tab + s * p.sub_stride;          // mode 2: this tile pair's table rows and rebased key offsets
+        const int *kof = s_koff + s * AT_BKV;
         const uint64_t kdesc = make_desc_kmajor_sw128(smem_u32(sK + s * AT_KV_BYTES));
         wgmma_fence();
 #pragma unroll
@@ -156,9 +192,9 @@ __global__ void __launch_bounds__(AT_THREADS, 1) attention_wgmma_kernel(const __
                     const float2 bf = __half22float2(__ldg(reinterpret_cast<const __half2 *>(brow[r] + k0)));
                     b0 = bf.x * LOG2E; b1 = bf.y * LOG2E;
                 } else if (BIAS_MODE == 2) {
-                    const uint32_t kk = *reinterpret_cast<const uint32_t *>(s_koff + k0);
-                    b0 = k0 == 0 ? rp_k0[r] : s_tab[rp_base[r] - rp_mult[r] * (int)(kk & 0xffffu)];
-                    b1 = s_tab[rp_base[r] - rp_mult[r] * (int)(kk >> 16)];
+                    const int2 kk = *reinterpret_cast<const int2 *>(kof + 8 * c + 2 * t);
+                    b0 = k0 == 0 ? rp_k0[r] : sub[rp_base[r] - rp_mult[r] * kk.x];
+                    b1 = sub[rp_base[r] - rp_mult[r] * kk.y];
                 }
                 float u0 = fmaf(sc[4 * c + 2 * r], p.scale_log2e, b0), u1 = fmaf(sc[4 * c + 2 * r + 1], p.scale_log2e, b1);
                 u0 = k0 < p.N ? u0 : -INFINITY;
@@ -219,9 +255,8 @@ __global__ void __launch_bounds__(AT_THREADS, 1) attention_wgmma_kernel(const __
 
 template <int MODE>
 static int launch_attn(const CUtensorMap &tm, const AttnParams &p, cudaStream_t stream) {
-    const int num_kv = (p.N + AT_BKV - 1) / AT_BKV;
-    const size_t tab = MODE == 2 ? (size_t)((p.nrd + 3) & ~3) * 4 + (size_t)num_kv * AT_BKV * 2 : 0;
-    if (AT_TAB_OFF + tab > (size_t)AT_SMEM_MAX) { set_error("attention: relative-position table (%d entries) does not fit in shared memory", p.nrd); return DM_E_UNSUPPORTED; }
+    const size_t tab = MODE == 2 ? (size_t)AT_STAGES * ((size_t)p.sub_stride * 4 + AT_BKV * 4) : 0;
+    if (AT_TAB_OFF + tab > (size_t)AT_SMEM_MAX) { set_error("attention: relative-position window %d x %d too wide for the table sub-windows", p.gh, p.gw); return DM_E_UNSUPPORTED; }
     static PerDeviceFlag configured;
     if (!configured.test_and_set())
         DM_CUDA_CHECK(cudaFuncSetAttribute(attention_wgmma_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, AT_SMEM_MAX));
@@ -240,9 +275,13 @@ int attention_f16(const __half *qkv, AttnParams p, cudaStream_t stream, const fl
         set_error("attention_f16: bias row pitch must be a multiple of 8 and cover whole 128-key tiles (got %d)", p.bias_ld);
         return DM_E_INVALID;
     }
-    p.rel_table = rel_table; p.nrd = nrd; p.gh = gh; p.gw = gw;
+    p.rel_table = rel_table; p.nrd = nrd; p.gh = gh; p.gw = gw; p.sub_stride = 0;
     if (rel_table) {
-        if (gh * gw + 1 != p.N || nrd != (2 * gh - 1) * (2 * gw - 1) + 3) { set_error("attention_f16: relative-position mode needs N = gh*gw+1 and nrd = (2gh-1)(2gw-1)+3"); return DM_E_INVALID; }
+        if (gh < 1 || gw < 1 || (long long)gh * gw + 1 != p.N || (long long)nrd != (long long)(2 * gh - 1) * (2 * gw - 1) + 3) {
+            set_error("attention_f16: relative-position mode needs N = gh*gw+1 and nrd = (2gh-1)(2gw-1)+3");
+            return DM_E_INVALID;
+        }
+        p.sub_stride = relpos_sub_stride(gh, gw);
         return launch_attn<2>(tm, p, stream);
     }
     return p.bias ? launch_attn<1>(tm, p, stream) : launch_attn<0>(tm, p, stream);

@@ -13,6 +13,8 @@
 //   the base crop on the merged patch (fp64 sums) and the blend: cubic resize of the fitted patch, Gaussian mask evaluated as the
 //   outer product of a bilinearly resampled 1-D profile, updated = updated (1 - m) + merged m.
 //   leres_stem_im2col_f32: the LeReS stem for a crop of a planar fp32 image (BOOST hands estimateleres float crops)
+//   minmax_normalise     estimatemidasBoost's per-call (x - min) / (max - min) of the crop-size prediction, with a device flag for the
+//                        constant prediction the reference cannot continue from (src/depthmap_generation.py:1212-1220)
 #include <cuda_fp16.h>
 #include <math.h>
 
@@ -283,6 +285,20 @@ __global__ void __launch_bounds__(256) boost_post_kernel(const float *__restrict
     if (i >= n) return;
     const float m = (t[i] + 1.f) / 2.f;
     out[i] = normalise ? (m - lo) / (hi - lo) : m;
+}
+
+// estimatemidasBoost's tail: (x - min) / (max - min) in fp32; a spread of at most float64 eps writes zeros and sets *degenerate (the
+// reference returns a scalar 0 there, which the following cv2.resize rejects)
+__global__ void __launch_bounds__(256) boost_minmax_normalise_kernel(const float *__restrict__ x, long long n, const float *__restrict__ partial,
+                                                                     float *__restrict__ out, int *__restrict__ degenerate) {
+    float lo, hi;
+    fold_minmax(partial, lo, hi);
+    const float span = hi - lo;
+    const bool flat = !((double)span > 2.220446049250313e-16);
+    if (flat && blockIdx.x == 0 && threadIdx.x == 0) *degenerate = 1;
+    const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
+    if (i >= n) return;
+    out[i] = flat ? 0.f : (x[i] - lo) / span;
 }
 
 // np.polyfit(mapped, base, 1): sums in fp64; partial[b] = {sum x, sum y, sum xx, sum xy}
@@ -568,6 +584,14 @@ DM_EXPORT int dm_boost_post(const float *t, long long n, const float *partial, i
     if (!t || !out || (normalise && !partial)) { set_error("dm_boost_post: null argument"); return DM_E_INVALID; }
     boost_post_kernel<<<GRID(n), 256, 0, (cudaStream_t)stream_>>>(t, n, partial, normalise, out);
     DM_LAUNCH_CHECK("boost_post_kernel");
+    return DM_OK;
+}
+
+DM_EXPORT int dm_boost_minmax_normalise(const float *x, long long n, const float *partial, float *out, int *degenerate, void *stream_) {
+    using namespace dm;
+    if (!x || !partial || !out || !degenerate || n <= 0) { set_error("dm_boost_minmax_normalise: bad arguments"); return DM_E_INVALID; }
+    boost_minmax_normalise_kernel<<<GRID(n), 256, 0, (cudaStream_t)stream_>>>(x, n, partial, out, degenerate);
+    DM_LAUNCH_CHECK("boost_minmax_normalise_kernel");
     return DM_OK;
 }
 

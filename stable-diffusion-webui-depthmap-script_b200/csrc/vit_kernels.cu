@@ -2,6 +2,8 @@
 //   preprocess_patchify  uint8 image -> [cv2-style bicubic resize] -> normalise -> fp16 patch matrix (im2col of the
 //                        patch-embedding conv; reference: depth_anything_v2/dpt.py:196-221 + util/transform.py,
 //                        dmidas/transforms.py:48-231, dinov2_layers/patch_embed.py:76, dmidas/backbones/beit.py:18-26)
+//   preprocess_patchify_f32_crops  the same for B crops of one planar fp32 image (BOOST's estimatemidasBoost,
+//                        src/depthmap_generation.py:1180-1203: cubic resize of the float crop, ImageNet mean / std)
 //   assemble_tokens      [cls | patch tokens] + positional embedding -> fp32 residual stream (dinov2.py:212-216)
 //   layernorm_f16        fp32 residual stream -> LayerNorm -> fp16 GEMM operand (eps 1e-6), optional "drop cls" remap
 //   resize_bilinear_nhwc fp16 NHWC bilinear, align_corners=True (util/blocks.py:143, dmidas/blocks.py:433)
@@ -37,6 +39,64 @@ __device__ __forceinline__ void cubic_coeffs(float x, float *c) {
     c[3] = 1.f - c[0] - c[1] - c[2];
 }
 
+// Pixel sources of the patchify kernels: load(y, x, v) reads the three channels of source pixel (y, x) as floats.
+struct U8Source {               // one image of a uint8 [B, H, W, 3] batch
+    const uint8_t *img;
+    int H, W;
+    __device__ __forceinline__ void load(int y, int x, float (&v)[3]) const {
+        const uint8_t *px = img + ((long long)y * W + x) * 3;
+        v[0] = px[0]; v[1] = px[1]; v[2] = px[2];
+    }
+};
+struct F32CropSource {          // a (x0, y0, w, h) crop of a planar fp32 [3, Hi, Wi] image
+    const float *img;
+    long long plane;
+    int pitch, H, W;
+    __device__ __forceinline__ void load(int y, int x, float (&v)[3]) const {
+        const float *px = img + (long long)y * pitch + x;
+        v[0] = px[0]; v[1] = px[plane]; v[2] = px[2 * plane];
+    }
+};
+
+// network pixel (y, x) of an nh x nw input: the source pixel when the sizes match, otherwise cv2.resize(..., INTER_CUBIC):
+// separable, A = -0.75, replicated borders, float coefficients
+template <class Src>
+__device__ __forceinline__ void cubic_sample(const Src &src, int nh, int nw, int y, int x, float (&v)[3]) {
+    if (nh == src.H && nw == src.W) { src.load(y, x, v); return; }
+    const float sx = (float)src.W / (float)nw, sy = (float)src.H / (float)nh;
+    float fx = ((float)x + 0.5f) * sx - 0.5f, fy = ((float)y + 0.5f) * sy - 0.5f;
+    const int ix = (int)floorf(fx), iy = (int)floorf(fy);
+    fx -= (float)ix; fy -= (float)iy;
+    float cx[4], cy[4];
+    cubic_coeffs(fx, cx);
+    cubic_coeffs(fy, cy);
+    v[0] = v[1] = v[2] = 0.f;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const int yy = min(max(iy - 1 + j, 0), src.H - 1);
+        float r[3] = {0.f, 0.f, 0.f};
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const int xx = min(max(ix - 1 + i, 0), src.W - 1);
+            float px[3];
+            src.load(yy, xx, px);
+            r[0] = fmaf(cx[i], px[0], r[0]); r[1] = fmaf(cx[i], px[1], r[1]); r[2] = fmaf(cx[i], px[2], r[2]);
+        }
+        v[0] = fmaf(cy[j], r[0], v[0]); v[1] = fmaf(cy[j], r[1], v[1]); v[2] = fmaf(cy[j], r[2], v[2]);
+    }
+}
+
+// normalise network pixel (y, x) of image b and store it into its patch row, K ordered (c, ky, kx)
+__device__ __forceinline__ void store_patch_pixel(const PreParams &p, int b, int y, int x, const float (&v)[3], float value_scale) {
+    const int py = y / p.patch, ky = y % p.patch, pxi = x / p.patch, kx = x % p.patch;
+    __half *row = p.out + ((long long)(b * p.gh + py) * p.gw + pxi) * p.kpad;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        const float val = (v[p.chan_map[c]] * value_scale - p.mean[c]) * p.inv_std[c];
+        row[(c * p.patch + ky) * p.patch + kx] = __float2half_rn(val);
+    }
+}
+
 __global__ void __launch_bounds__(256) preprocess_patchify_kernel(PreParams p) {
     // one thread per (network pixel, channel triple): thread -> (b, y, x) of the network input
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -45,41 +105,26 @@ __global__ void __launch_bounds__(256) preprocess_patchify_kernel(PreParams p) {
     const int x = (int)(idx % p.nw);
     const int y = (int)((idx / p.nw) % p.nh);
     const int b = (int)(idx / ((long long)p.nw * p.nh));
-    const uint8_t *img = p.rgb + (long long)b * p.H * p.W * 3;
+    const U8Source src{p.rgb + (long long)b * p.H * p.W * 3, p.H, p.W};
     float v[3];
-    if (p.nh == p.H && p.nw == p.W) {
-        const uint8_t *px = img + ((long long)y * p.W + x) * 3;
-        v[0] = px[0]; v[1] = px[1]; v[2] = px[2];
-    } else {
-        // cv2.resize(..., INTER_CUBIC) on the /255 image: separable, A = -0.75, replicated borders, float coefficients
-        const float sx = (float)p.W / (float)p.nw, sy = (float)p.H / (float)p.nh;
-        float fx = ((float)x + 0.5f) * sx - 0.5f, fy = ((float)y + 0.5f) * sy - 0.5f;
-        const int ix = (int)floorf(fx), iy = (int)floorf(fy);
-        fx -= (float)ix; fy -= (float)iy;
-        float cx[4], cy[4];
-        cubic_coeffs(fx, cx);
-        cubic_coeffs(fy, cy);
-        v[0] = v[1] = v[2] = 0.f;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            const int yy = min(max(iy - 1 + j, 0), p.H - 1);
-            float r[3] = {0.f, 0.f, 0.f};
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const int xx = min(max(ix - 1 + i, 0), p.W - 1);
-                const uint8_t *px = img + ((long long)yy * p.W + xx) * 3;
-                r[0] = fmaf(cx[i], (float)px[0], r[0]); r[1] = fmaf(cx[i], (float)px[1], r[1]); r[2] = fmaf(cx[i], (float)px[2], r[2]);
-            }
-            v[0] = fmaf(cy[j], r[0], v[0]); v[1] = fmaf(cy[j], r[1], v[1]); v[2] = fmaf(cy[j], r[2], v[2]);
-        }
-    }
-    const int py = y / p.patch, ky = y % p.patch, pxi = x / p.patch, kx = x % p.patch;
-    __half *row = p.out + ((long long)(b * p.gh + py) * p.gw + pxi) * p.kpad;
-#pragma unroll
-    for (int c = 0; c < 3; ++c) {
-        const float val = (v[p.chan_map[c]] * (1.0f / 255.0f) - p.mean[c]) * p.inv_std[c];
-        row[(c * p.patch + ky) * p.patch + kx] = __float2half_rn(val);
-    }
+    cubic_sample(src, p.nh, p.nw, y, x, v);
+    store_patch_pixel(p, b, y, x, v, 1.0f / 255.0f);
+}
+
+// BOOST crops: p.rgb unused; image b is the crop rects[b] = (x0, y0, w, h) of the planar fp32 image, values used as they are
+__global__ void __launch_bounds__(256) preprocess_patchify_f32_crops_kernel(PreParams p, const float *__restrict__ img, int Hi, int Wi,
+                                                                            const int *__restrict__ rects) {
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const long long total = (long long)p.B * p.nh * p.nw;
+    if (idx >= total) return;
+    const int x = (int)(idx % p.nw);
+    const int y = (int)((idx / p.nw) % p.nh);
+    const int b = (int)(idx / ((long long)p.nw * p.nh));
+    const int4 r = __ldg(reinterpret_cast<const int4 *>(rects) + b);
+    const F32CropSource src{img + (long long)r.y * Wi + r.x, (long long)Hi * Wi, Wi, r.w, r.z};
+    float v[3];
+    cubic_sample(src, p.nh, p.nw, y, x, v);
+    store_patch_pixel(p, b, y, x, v, 1.0f);
 }
 
 __global__ void zero_pad_cols_kernel(__half *out, long long rows, int kused, int kpad) {
@@ -285,13 +330,10 @@ __global__ void __launch_bounds__(256) concat_readout_kernel(const float *__rest
 
 #define DM_EXPORT extern "C" __attribute__((visibility("default")))
 
-DM_EXPORT int dm_preprocess_patchify(const uint8_t *rgb, int B, int H, int W, int net_h, int net_w, int patch, const float *mean_host,
-                                     const float *std_host, const int *chan_map_host, void *out, int kpad, void *stream_) {
+static int patchify_setup(dm::PreParams &p, int B, int net_h, int net_w, int patch, const float *mean_host, const float *std_host,
+                          const int *chan_map_host, void *out, int kpad, cudaStream_t stream) {
     using namespace dm;
-    if (!rgb || !out || net_h % patch || net_w % patch || kpad < 3 * patch * patch) { set_error("dm_preprocess_patchify: bad arguments"); return DM_E_INVALID; }
-    cudaStream_t stream = (cudaStream_t)stream_;
-    PreParams p;
-    p.rgb = rgb; p.B = B; p.H = H; p.W = W; p.nh = net_h; p.nw = net_w; p.patch = patch; p.gh = net_h / patch; p.gw = net_w / patch;
+    p.B = B; p.nh = net_h; p.nw = net_w; p.patch = patch; p.gh = net_h / patch; p.gw = net_w / patch;
     p.kpad = kpad; p.out = (__half *)out;
     for (int c = 0; c < 3; ++c) { p.mean[c] = mean_host[c]; p.inv_std[c] = 1.0f / std_host[c]; p.chan_map[c] = chan_map_host[c]; }
     const long long rows = (long long)B * p.gh * p.gw;
@@ -301,9 +343,40 @@ DM_EXPORT int dm_preprocess_patchify(const uint8_t *rgb, int B, int H, int W, in
         zero_pad_cols_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>((__half *)out, rows, kused, kpad);
         DM_LAUNCH_CHECK("zero_pad_cols_kernel");
     }
+    return DM_OK;
+}
+
+DM_EXPORT int dm_preprocess_patchify(const uint8_t *rgb, int B, int H, int W, int net_h, int net_w, int patch, const float *mean_host,
+                                     const float *std_host, const int *chan_map_host, void *out, int kpad, void *stream_) {
+    using namespace dm;
+    if (!rgb || !out || net_h % patch || net_w % patch || kpad < 3 * patch * patch) { set_error("dm_preprocess_patchify: bad arguments"); return DM_E_INVALID; }
+    cudaStream_t stream = (cudaStream_t)stream_;
+    PreParams p;
+    p.rgb = rgb; p.H = H; p.W = W;
+    const int rc = patchify_setup(p, B, net_h, net_w, patch, mean_host, std_host, chan_map_host, out, kpad, stream);
+    if (rc) return rc;
     const long long total = (long long)B * net_h * net_w;
     preprocess_patchify_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(p);
     DM_LAUNCH_CHECK("preprocess_patchify_kernel");
+    return DM_OK;
+}
+
+DM_EXPORT int dm_preprocess_patchify_f32_crops(const float *img, int Hi, int Wi, const int *rects_dev, int B, int net_h, int net_w, int patch,
+                                               const float *mean_host, const float *std_host, const int *chan_map_host, void *out, int kpad,
+                                               void *stream_) {
+    using namespace dm;
+    if (!img || !rects_dev || !out || B <= 0 || Hi <= 0 || Wi <= 0 || net_h % patch || net_w % patch || kpad < 3 * patch * patch) {
+        set_error("dm_preprocess_patchify_f32_crops: bad arguments"); return DM_E_INVALID;
+    }
+    if (reinterpret_cast<uintptr_t>(rects_dev) % 16) { set_error("dm_preprocess_patchify_f32_crops: rects must be 16-byte aligned (read as int4)"); return DM_E_INVALID; }
+    cudaStream_t stream = (cudaStream_t)stream_;
+    PreParams p;
+    p.rgb = nullptr; p.H = Hi; p.W = Wi;
+    const int rc = patchify_setup(p, B, net_h, net_w, patch, mean_host, std_host, chan_map_host, out, kpad, stream);
+    if (rc) return rc;
+    const long long total = (long long)B * net_h * net_w;
+    preprocess_patchify_f32_crops_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(p, img, Hi, Wi, rects_dev);
+    DM_LAUNCH_CHECK("preprocess_patchify_f32_crops_kernel");
     return DM_OK;
 }
 

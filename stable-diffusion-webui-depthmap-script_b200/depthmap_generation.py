@@ -430,8 +430,9 @@ class DepthAnythingV2Engine:
             ops.gemm(b[f'u{li}'], Fp, w[f'rf{rf}_out_w'], Fp, B * s[0] * s[1], Fp, Fp, bias=w[f'rf{rf}_out_b'], C=b['v'][step + 1], ldc=Fp)
             ops.resize_nhwc(b['v'][step + 1], B, s[0], s[1], Fp, b['path'][step + 1], t[0], t[1])
 
-    def run_head(self, b, B, H, W, nh, nw, out_hw=None):
-        """output_conv (dpt.py:139-150 / dpt_depth.py:150-158) + the final resize to the image size."""
+    def run_head(self, b, B, H, W, nh, nw, out_hw=None, resize=True):
+        """output_conv (dpt.py:139-150 / dpt_depth.py:150-158) + the final resize to the image size.  resize=False returns the
+        net-size prediction [B, nh, nw] itself (a pooled buffer, valid until the next forward at this shape)."""
         import torch
         ops, w = self.ops, self.w
         Fp = self.Fp
@@ -442,6 +443,8 @@ class DepthAnythingV2Engine:
         # conv3x3 -> ReLU -> conv1x1 -> ReLU (+ the outer F.relu, idempotent) fused into one epilogue
         ops.conv3x3(b['oc1u'], B, nh, nw, self.F2p, w['oc2_w'], 32, epi=E.EPI_HEAD, act=A.ACT_RELU, bias=w['oc2_b'], X=b['d'], gamma=w['oc3_w'],
                     head_b2=self.oc3_b)
+        if not resize:
+            return b['d']
         oh, ow = out_hw if out_hw is not None else (H, W)
         out = torch.empty(B, oh, ow, dtype=torch.float32, device=self.device)
         ops.resize_f32(b['d'], B, nh, nw, out, oh, ow, self.FINAL_RESIZE_MODE)
@@ -470,21 +473,17 @@ def midas_net_size(width, height, net_w, net_h, multiple_of=32):
     return _constrain_to_multiple_of(sw * width, multiple_of), _constrain_to_multiple_of(sh * height, multiple_of)
 
 
-def _gen_relative_position_index(wh, ww):
-    """timm 0.9 gen_relative_position_index (restated): cls rows / cols use the three extra table entries."""
-    import torch
-    nrd = (2 * wh - 1) * (2 * ww - 1) + 3
-    coords = torch.stack(torch.meshgrid([torch.arange(wh), torch.arange(ww)], indexing='ij')).flatten(1)
-    rel = (coords[:, :, None] - coords[:, None, :]).permute(1, 2, 0).contiguous()
-    rel[:, :, 0] += wh - 1
-    rel[:, :, 1] += ww - 1
-    rel[:, :, 0] *= 2 * ww - 1
-    idx = torch.zeros((wh * ww + 1,) * 2, dtype=rel.dtype)
-    idx[1:, 1:] = rel.sum(-1)
-    idx[0, 0:] = nrd - 3
-    idx[0:, 0] = nrd - 2
-    idx[0, 0] = nrd - 1
-    return idx
+def midas_boost_net_size(width, height, msize, multiple_of=32):
+    """Resize(msize, msize, keep_aspect_ratio, 'upper_bound', multiple of 32) of estimatemidasBoost (src/depthmap_generation.py:1183-1192,
+    dmidas/transforms.py:94-160): the largest net inside msize x msize with the crop's aspect; a side that rounds past msize is
+    floored instead."""
+    sh, sw = msize / height, msize / width
+    if sw < sh:
+        sh = sw
+    else:
+        sw = sh
+    return (_constrain_to_multiple_of(sw * width, multiple_of, max_val=msize),
+            _constrain_to_multiple_of(sh * height, multiple_of, max_val=msize))
 
 
 class DptBeitEngine(DepthAnythingV2Engine):
@@ -493,8 +492,13 @@ class DptBeitEngine(DepthAnythingV2Engine):
     Mirrors the reference's overriding forwards (dmidas/backbones/beit.py:18-129), the reassemble stage
     (dmidas/backbones/utils.py:28-39,83-124,144-249), DPT / DPTDepthModel (dmidas/dpt_depth.py:110-166) and estimatemidas
     (src/depthmap_generation.py:455-499).  The relative-position bias, which the reference rebuilds (bilinear table
-    resize + gather) in every block of every forward, is expanded once per resolution into a [heads, N, N] fp16 table
-    per block and added inside the fused attention kernel."""
+    resize + gather) in every block of every forward, is resized once per resolution into a per-head fp32 table per block;
+    the fused attention kernel gathers from it (csrc/attention_wgmma.cu), so no [heads, N, N] tensor exists.
+
+    BOOST (estimatemidasBoost, src/depthmap_generation.py:1180-1220) calls forward_batch(None, msize, msize, planar=(img, rect))
+    and forward_crops(img, rects, msize) on float crops of a planar fp32 image: upper-bound net size (midas_boost_net_size),
+    ImageNet mean / std, the channel order of the crop unchanged (network channel c = plane 2 - c of the RGB image), and a cv2
+    INTER_CUBIC resize of the prediction back to the crop."""
 
     PATCH = 16
     MEAN = (0.5, 0.5, 0.5)
@@ -555,6 +559,8 @@ class DptBeitEngine(DepthAnythingV2Engine):
         self._tables = [f32(sd[p + f'blocks.{i}.attn.relative_position_bias_table']) for i in range(cfg['depth'])]
         self._bias_cache = {}
 
+    TABLE_RESOLUTIONS = 4      # resized tables kept resident: BOOST alternates between its whole-image and patch windows
+
     def rel_tables(self, gh, gw):
         """Table half of _get_rel_pos_bias (dmidas/backbones/beit.py:29-50): per block, the [nrd, heads] table resized
         (bilinear) to the current window, laid out [heads, nrd] in fp32 and multiplied by log2(e).  Once per resolution.
@@ -575,43 +581,62 @@ class DptBeitEngine(DepthAnythingV2Engine):
                 dst = np.empty((heads, nrd_new), dtype=np.float32)
                 _lib.check(self.ops.L.dm_beit_rel_table(src.ctypes.data, win, heads, gh, gw, dst.ctypes.data), "dm_beit_rel_table")
                 out.append(torch.from_numpy(dst).to(self.device))
-            self._bias_cache = {key: (out, new_h * new_w + 3)}  # keep one resolution resident (drops dense tables too)
-        return self._bias_cache[key]
-
-    @staticmethod
-    def table_fits_on_chip(gh, gw):
-        """The table attention mode keeps one head's bias table and the per-key offsets in the shared memory the kernel
-        has left beside its Q / K / V tiles (csrc/attention_wgmma.cu: AT_SMEM_MAX - AT_TAB_OFF)."""
-        nrd, N = (2 * gh - 1) * (2 * gw - 1) + 3, gh * gw + 1
-        need = 4 * ((nrd + 3) & ~3) + 2 * ((N + 127) // 128) * 128
-        return need <= 227 * 1024 - (5 * 16384 + 64)
-
-    def dense_bias(self, gh, gw):
-        """Fallback for windows whose table does not fit on chip (from about 96 x 96 patches, nrd = 36484, upwards; a 3:2
-        image on dpt_beit_large_512, net 768x512, nrd = 5988, fits): the gather half of _get_rel_pos_bias (beit.py:52-62) done once per resolution into a dense fp16
-        [heads, N, ld] tensor per block (ld = N rounded up to whole 128-key tiles), added inside the attention kernel."""
-        import torch
-        key = ('dense', gh, gw)
-        if key not in self._bias_cache:
-            tabs, nrd = self.rel_tables(gh, gw)
-            idx = _gen_relative_position_index(gh, gw).to(self.device)
-            N = gh * gw + 1
-            ld = _ru(N, 128)
-            out = []
-            for tab in tabs:
-                d = torch.zeros(tab.shape[0], N, ld, dtype=torch.float16, device=self.device)
-                d[:, :, :N] = (tab / 1.4426950408889634)[:, idx.view(-1)].view(-1, N, N).to(torch.float16)
-                out.append(d)
-            self._bias_cache[key] = (out, ld)
+            while len(self._bias_cache) >= self.TABLE_RESOLUTIONS:
+                self._bias_cache.pop(next(iter(self._bias_cache)))
+            self._bias_cache[key] = (out, new_h * new_w + 3)
         return self._bias_cache[key]
 
     def attention(self, i, b, B, N, heads, C, gh, gw):
         tabs, nrd = self.rel_tables(gh, gw)
-        if not self.table_fits_on_chip(gh, gw):
-            dense, ld = self.dense_bias(gh, gw)
-            self.ops.attention(b['qkv'], B, N, heads, (C // heads) ** -0.5, b['att'], bias=dense[i], bias_ld=ld)
-            return
         self.ops.attention_relpos(b['qkv'], B, gh, gw, heads, (C // heads) ** -0.5, tabs[i], nrd, b['att'])
+
+    # ---- BOOST: estimatemidasBoost on float crops ---------------------------------------------------------------------
+    BOOST_MEAN = (0.485, 0.456, 0.406)
+    BOOST_STD = (0.229, 0.224, 0.225)
+
+    def forward_batch(self, rgb, net_w, net_h=None, out_hw=None, planar=None):
+        """rgb: uint8 CUDA [B,H,W,3] -> float32 CUDA [B,H,W] (estimatemidas).  planar = (fp32 CUDA [3,Hi,Wi] image, (x0, y0, w, h))
+        instead of `rgb`: estimatemidasBoost's network and resize on that crop with msize = net_w -> [1, h, w] (not normalised)."""
+        if planar is None:
+            return super().forward_batch(rgb, net_w, net_h, out_hw)
+        img, rect = planar
+        return self.forward_crops(img, [rect], net_w)[0].unsqueeze(0)
+
+    def forward_crops(self, planar, rects, msize):
+        """B crops (x0, y0, w, h) of one planar fp32 image [3, Hi, Wi] -> [fp32 CUDA [h, w]] in the order of `rects`: each crop at its
+        upper-bound net size for msize, then cv2-cubic back to the crop.  Crops clipped at the image border are not square, so the
+        crops are grouped by net shape, one batched forward per shape."""
+        import torch
+        L, st = self.ops.L, _lib.stream_ptr
+        hi, wi = int(planar.shape[1]), int(planar.shape[2])
+        if planar.dtype != torch.float32 or planar.dim() != 3 or planar.shape[0] != 3 or not planar.is_contiguous():
+            raise ValueError("planar must be a contiguous float32 tensor [3, H, W]")
+        groups = {}
+        for k, (x0, y0, w, h) in enumerate(rects):
+            if x0 < 0 or y0 < 0 or w <= 0 or h <= 0 or x0 + w > wi or y0 + h > hi:
+                raise ValueError(f"crop {(x0, y0, w, h)} outside the {wi}x{hi} image")
+            nw, nh = midas_boost_net_size(w, h, msize)
+            if nw <= 0 or nh <= 0:
+                raise ValueError(f"crop {w}x{h} is too elongated for a net of at most {msize} px")
+            groups.setdefault((nh, nw), []).append(k)
+        m, sd, cm = (ctypes.c_float * 3)(*self.BOOST_MEAN), (ctypes.c_float * 3)(*self.BOOST_STD), (ctypes.c_int * 3)(*self.CHAN_MAP)
+        out = [None] * len(rects)
+        for (nh, nw), ks in groups.items():
+            B = len(ks)
+            r = torch.tensor([[int(v) for v in rects[k]] for k in ks], dtype=torch.int32).to(self.device)
+            b = self._buffers(B, nh, nw)
+            _lib.check(L.dm_preprocess_patchify_f32_crops(planar.data_ptr(), hi, wi, r.data_ptr(), B, nh, nw, self.PATCH, m, sd, cm,
+                                                           b['patches'].data_ptr(), self.kpad, st()), "dm_preprocess_patchify_f32_crops")
+            self.ops.launches += 1
+            self.run_network(b, B, nh, nw)
+            d = self.run_head(b, B, nh, nw, nh, nw, resize=False)
+            for i, k in enumerate(ks):
+                w, h = int(rects[k][2]), int(rects[k][3])
+                o = torch.empty(h, w, dtype=torch.float32, device=self.device)
+                _lib.check(L.dm_boost_resize_cubic(d[i].data_ptr(), nw, 0, nh, nw, o.data_ptr(), w, 0, h, w, 1, st()), "dm_boost_resize_cubic")
+                self.ops.launches += 1
+                out[k] = o
+        return out
 
     def emit_feature(self, b, fi, B, N, C):
         """forward hook on the raw block output + ProjectReadout: GELU(Linear(cat(tokens, cls)))."""
@@ -1329,9 +1354,10 @@ class ModelHolder:
         """Ensure that the depth model is loaded (reference: src/depthmap_generation.py:76-301)."""
         import torch
         _lib.require_cuda()
-        if boost and model_type != 0:
-            raise NotImplementedError("BOOST is built for the reference's default base network only, LeReS res101 (model type 0); "
-                                      "the other base networks (estimatemidasBoost etc.) are not implemented in depthmap_b200")
+        from .boost import BASE_NETWORKS
+        if boost and model_type not in BASE_NETWORKS:
+            raise NotImplementedError(f"BOOST is implemented in depthmap_b200 for the base networks LeReS res101 (model type 0), "
+                                      f"DPT-BEiT-L 512 / 384 (1, 2) and DPT-Large 384 (3), not for model type {model_type}")
         if tiling_mode:
             raise NotImplementedError("tiling_mode (circular conv padding) is not implemented in depthmap_b200 yet")
         if getattr(self, "no_half", False):
@@ -1361,7 +1387,8 @@ class ModelHolder:
                 sd = torch.load(model_path, map_location='cpu')
                 if "optimizer" in sd:       # dmidas/base_model.py:13: training checkpoints wrap the weights
                     sd = sd["model"]
-            model = NativeDepthModel(sd, model_type, torch.device(device))
+            # BOOST feeds float crops through the op-level engine (estimatemidasBoost); plain forwards use the model-level handle
+            model = DptBeitEngine(sd, name, torch.device(device)) if boost else NativeDepthModel(sd, model_type, torch.device(device))
         elif model_type == 0:  # res101 (LeReS)
             if self.weights_provider is not None:
                 sd = self.weights_provider(model_type)
@@ -1373,16 +1400,6 @@ class ModelHolder:
                 if "depth_model" in sd:      # src/depthmap_generation.py:113-116: strip_prefix_if_present(checkpoint['depth_model'], "module.")
                     sd = {(k[len("module."):] if k.startswith("module.") else k): v for k, v in sd["depth_model"].items()}
             model = LeresEngine(sd, torch.device(device))
-            if boost:      # reference :284-299: the pix2pix merge network ('latest_net_G.pth', netG = unet_1024, norm none)
-                from .boost import BoostPipeline, UnetMergeEngine
-                if self.weights_provider is not None:
-                    psd = self.weights_provider("pix2pix")
-                else:
-                    p2p_path = "./models/pix2pix/latest_net_G.pth"
-                    if not os.path.exists(p2p_path):
-                        raise FileNotFoundError(f"{p2p_path} not found (depthmap_b200 does not download checkpoints)")
-                    psd = torch.load(p2p_path, map_location='cpu')
-                self.pix2pix_model = BoostPipeline(model, UnetMergeEngine(psd, torch.device(device)), torch.device(device), model_type)
         elif model_type == 3:  # dpt_large_384 (MiDaS 3.0)
             if self.weights_provider is not None:
                 sd = self.weights_provider(model_type)
@@ -1393,7 +1410,7 @@ class ModelHolder:
                 sd = torch.load(model_path, map_location='cpu')
                 if "optimizer" in sd:
                     sd = sd["model"]
-            model = NativeDepthModel(sd, model_type, torch.device(device))
+            model = DptVitEngine(sd, 'vitl16_384', torch.device(device)) if boost else NativeDepthModel(sd, model_type, torch.device(device))
         elif model_type == 9:  # zoedepth_nk (src/depthmap_generation.py:221-226: ZoeD_M12_NK.pt)
             if self.weights_provider is not None:
                 sd = self.weights_provider(model_type)
@@ -1408,6 +1425,16 @@ class ModelHolder:
         else:
             raise NotImplementedError(f"model_type {model_type} is not implemented in depthmap_b200 yet "
                                       f"(implemented: 0 = LeReS res101; 1, 2 = DPT-BEiT-L 512/384; 3 = DPT-Large 384; 9 = ZoeDepth-NK; 12, 13, 14 = Depth-Anything-V2 S/B/L)")
+        if boost:      # reference :284-299: the pix2pix merge network ('latest_net_G.pth', netG = unet_1024, norm none)
+            from .boost import BoostPipeline, UnetMergeEngine
+            if self.weights_provider is not None:
+                psd = self.weights_provider("pix2pix")
+            else:
+                p2p_path = "./models/pix2pix/latest_net_G.pth"
+                if not os.path.exists(p2p_path):
+                    raise FileNotFoundError(f"{p2p_path} not found (depthmap_b200 does not download checkpoints)")
+                psd = torch.load(p2p_path, map_location='cpu')
+            self.pix2pix_model = BoostPipeline(model, UnetMergeEngine(psd, torch.device(device)), torch.device(device), model_type)
         self.depth_model = model
         self.depth_model_type = model_type
         self.resize_mode = "minimal"

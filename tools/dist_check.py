@@ -1,7 +1,8 @@
 """torchrun tool: the N-rank sharded + gathered result equals the 1-rank result BIT FOR BIT (SURVEY.md §4 / §8e).
 Every rank builds the same model (seeded synthetic weights), takes its contiguous slice of the same batch, runs
 depth -> u16 -> stereo -> normal map, all-gathers the finished tensors over NCCL and compares with the whole batch computed
-locally.   python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 tools/dist_check.py"""
+locally.   python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 tools/dist_check.py [--boost-model-type T]
+--boost-model-type: the BOOST base network, 0 = LeReS res101 (default), 1 = DPT-BEiT-L 512, 2 = DPT-BEiT-L 384, 3 = DPT-Large 384."""
 import os
 import sys
 
@@ -47,16 +48,21 @@ def main():
     boost_note = ""
     if os.environ.get("DIST_CHECK_BOOST", "1") != "0":
         from depthmap_b200.boost import BoostPipeline, UnetMergeEngine
-        from depthmap_b200.depthmap_generation import LeresEngine
-        pipe = BoostPipeline(LeresEngine(synth_weights.make_leres_state_dict(seed=2), dev),
-                             UnetMergeEngine(synth_weights.make_pix2pix_state_dict(seed=1), dev), dev, 0)
+        from depthmap_b200.depthmap_generation import DptBeitEngine, DptVitEngine, LeresEngine
+        t = int(sys.argv[sys.argv.index("--boost-model-type") + 1]) if "--boost-model-type" in sys.argv else 0
+        if t == 0:
+            base = LeresEngine(synth_weights.make_leres_state_dict(seed=2), dev)
+        else:
+            name = {1: 'beitl16_512', 2: 'beitl16_384', 3: 'vitl16_384'}[t]
+            base = (DptVitEngine if t == 3 else DptBeitEngine)(synth_weights.make_beit_dpt_state_dict(name, seed=3), name, dev)
+        pipe = BoostPipeline(base, UnetMergeEngine(synth_weights.make_pix2pix_state_dict(seed=1), dev), dev, t)
         img = synth_rgb(300, 420, 12)
         info = {}
         sharded = pipe.run(img, 1600, group=dist.group.WORLD, info=info)
         single = pipe.run(img, 1600)
         same = np.array_equal(sharded, single)
         ok = ok and same
-        boost_note = f" boost_patches={len(info['rects'])} boost_equal={same}"
+        boost_note = f" boost_model_type={t} boost_patches={len(info['rects'])} boost_equal={same}"
     flag = torch.tensor([1 if ok else 0], device=dev)
     dist.all_reduce(flag, op=dist.ReduceOp.MIN)
     if rank == 0:
