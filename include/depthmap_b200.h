@@ -218,6 +218,28 @@ int dm_zoe_clb_final(const void *o32, int ldo, const float *ze, int ldz, const f
 /* out[b] = mean(crop(bicubic(d[2b])), unflip(crop(bicubic(d[2b+1])))): d fp32 [2B,nh,nw] -> out fp32 [B,H,W] */
 int dm_zoe_tta_combine(const float *d, int B, int nh, int nw, int pad_h, int pad_w, int H, int W, float *out, void *stream);
 
+/* Single-head ZoeDepth (ZoeDepth-N, model type 7, softplus bins; ZoeDepth-K, model type 8, "normed" bins), the head of
+ * dzoedepth/models/zoedepth/zoedepth_v1.py:124-192 on the same DPT-BEiT core, TTA, pre-processing and dm_zoe_tta_combine.
+ * No router.  Inverse attractors with alpha 300, gamma 2, kind "mean".
+ * Seed bin centres: seed fp32 [rows, ld] (seed MLP output before its last activation, columns 0..63) -> out fp32 [rows, 64].
+ * normed = 0: softplus(seed).  normed = 1: B = relu(seed) + 1e-3, widths = (max-min) B / sum B, centres = midpoints of
+ * cumsum([min, widths]), out = (centres - min) / (max - min). */
+int dm_zoe_seed_bins(const float *seed, int ld, long long rows, int normed, float min_depth, float max_depth, float *out, void *stream);
+/* Attractor level with n_attractors in {16, 8, 4, 1}: A fp32 [F*H*W, lda] attractor MLP output before its last activation;
+ * normed = 0: a_i = softplus(A[:, i]); normed = 1: a_i = relu(A[:, 2i]) + 1e-3.  b_prev fp32 [F,Hp,Wp,64] is resized
+ * (bilinear, align_corners) to H x W; b_out fp32 [F,H,W,64] = b + mean_i dx_i / (1 + 300 dx_i^2), dx_i = a_i - b, or with
+ * sort_clip = 1 (normed only; the level whose centres the log-binomial consumes) clip(sort((max-min) b_new + min), min, max)
+ * over each pixel's 64 bins.  DM_E_UNSUPPORTED for another attractor count. */
+int dm_zoe_attractor_single(const float *A, int lda, int n_attractors, int normed, const float *b_prev, int F, int Hp, int Wp, int H, int W,
+                            int sort_clip, float min_depth, float max_depth, float *b_out, void *stream);
+/* ConditionalLogBinomial(33, 128, 64) (hidden 80) + expectation over the 64 bin centres, per net pixel.  o32 fp16 [F,nh,nw,ldo]
+ * relu'd out_conv activation (32 channels used); the 33rd input, the core's relative depth relu(wr . o32 + br), is computed
+ * in-kernel (wr fp32 [32]).  ze fp32 [F,h3,w3,ldz] = W_e . b_emb (80 used); bc fp32 [F,h3,w3,64] bin centres; wo [33][80]
+ * (input channel major), b0 [80], w2 [4][80], b2 [4] fp32 device arrays; out fp32 [F,nh,nw] */
+int dm_zoe_clb_single(const void *o32, int ldo, const float *ze, int ldz, const float *bc, const float *wo, const float *b0, const float *w2,
+                      const float *b2, const float *wr, float br, int F, int nh, int nw, int h3, int w3, float min_temp, float max_temp,
+                      float *out, void *stream);
+
 /* ---------------------------------------------------------------------------------------------------------------
  * §8(f) rank 1 — video mode's cross-frame normalisation.    replaces  src/video_mode.py:103-128 (process_predicitons)
  * Frames are fp32 [count, hw] device arrays.  Each step is its own call so that, when the frames of a clip are sharded

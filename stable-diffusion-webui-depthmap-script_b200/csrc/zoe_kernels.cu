@@ -375,6 +375,206 @@ __global__ void __launch_bounds__(256) tta_combine_kernel(const float *__restric
     out[idx] = (a + c) / 2.f;
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// Single-head ZoeDepth (ZoeDepth-N, model type 7: softplus bins; ZoeDepth-K, model type 8: "normed" bins), the head of
+// dzoedepth/models/zoedepth/zoedepth_v1.py:124-192.  No router: the kernels below have no head index.
+
+// seed bin centres, one warp per row of 64 (two bins per lane).  softplus: SeedBinRegressorUnnormed, c = softplus(s).
+// normed: SeedBinRegressor (localbins_layers.py:52-68), B = relu(s) + 1e-3, widths = (max-min) B / sum B, edges = cumsum of
+// [min, widths], c = edge midpoints; then b_prev = (c - min) / (max - min) (zoedepth_v1.py:155-157).
+__global__ void __launch_bounds__(256) seed_bins_kernel(const float *__restrict__ seed, int ld, long long rows, int normed, float dmin,
+                                                        float dmax, float *__restrict__ out) {
+    const long long r = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31;
+    if (r >= rows) return;                               // whole warps leave together
+    const float2 s = *reinterpret_cast<const float2 *>(seed + r * ld + 2 * lane);
+    float2 o;
+    if (!normed) {
+        o = make_float2(softplus_f(s.x), softplus_f(s.y));
+    } else {
+        const float b0 = fmaxf(s.x, 0.f) + 1e-3f, b1 = fmaxf(s.y, 0.f) + 1e-3f;
+        float tot = b0 + b1;
+#pragma unroll
+        for (int m = 16; m > 0; m >>= 1) tot += __shfl_xor_sync(0xffffffffu, tot, m);
+        const float rng = dmax - dmin;
+        const float w0 = rng * (b0 / tot), w1 = rng * (b1 / tot);
+        float inc = w0 + w1;                             // inclusive prefix over lanes of the pair sums
+#pragma unroll
+        for (int m = 1; m < 32; m <<= 1) {
+            const float t = __shfl_up_sync(0xffffffffu, inc, m);
+            if (lane >= m) inc += t;
+        }
+        const float e0 = dmin + (inc - (w0 + w1));       // edge 2*lane
+        const float e1 = e0 + w0, e2 = e1 + w1;
+        o = make_float2((0.5f * (e0 + e1) - dmin) / rng, (0.5f * (e1 + e2) - dmin) / rng);
+    }
+    *reinterpret_cast<float2 *>(out + r * 64 + 2 * lane) = o;
+}
+
+// AttractorLayerUnnormed (NORMED = false: a_i = softplus(A[., i])) / AttractorLayer (NORMED = true: a_i = relu(A[., 2i]) + 1e-3,
+// the A_normed override of attractor.py:104-106) with NA attractors, kind "mean", inverse attractor with alpha 300, gamma 2:
+// b_new = b + mean_i dx_i / (1 + 300 dx_i^2), dx_i = a_i - b, b = bilinear_align_corners(b_prev).  Thread layout as
+// attractor_kernel: one thread per (pixel, bin), a block = 4 whole pixels.  sort_clip (the last level of the normed head, where
+// the centres are consumed): out = clip(sort((max - min) b_new + min), min, max) over the 64 bins of the pixel, sorted by a
+// bitonic network in shared memory; otherwise out = b_new (the next level's b_prev, unsorted as in the reference).
+template <int NA, bool NORMED>
+__global__ void __launch_bounds__(256) attractor_single_kernel(const float *__restrict__ A, int lda, const float *__restrict__ bprev, int Hp, int Wp,
+                                                               int H, int W, float sy, float sx, int sort_clip, float dmin, float dmax,
+                                                               float *__restrict__ bout) {
+    __shared__ float s_c[256];
+    const int y = blockIdx.y, f = blockIdx.z;
+    const int t = blockIdx.x * 256 + threadIdx.x;
+    const int x = t >> 6, k = t & 63;
+    const int lane = threadIdx.x & 31;
+    const bool ok = x < W;
+    const int xc = ok ? x : W - 1;
+    const float fy = sy * (float)y, fx = sx * (float)xc;
+    const int y0 = min((int)fy, Hp - 1), x0 = min((int)fx, Wp - 1);
+    const int y1 = min(y0 + 1, Hp - 1), x1 = min(x0 + 1, Wp - 1);
+    const float ly = fy - (float)y0, lx = fx - (float)x0, hy = 1.f - ly, hx = 1.f - lx;
+    const float *bp = bprev + (size_t)f * Hp * Wp * 64 + k;
+    const float b = hy * (hx * bp[(size_t)(y0 * Wp + x0) * 64] + lx * bp[(size_t)(y0 * Wp + x1) * 64]) +
+                    ly * (hx * bp[(size_t)(y1 * Wp + x0) * 64] + lx * bp[(size_t)(y1 * Wp + x1) * 64]);
+    const float *arow = A + ((size_t)(f * H + y) * W + xc) * lda;
+    const int ai = lane & (NA - 1);                      // lanes 0..NA-1 hold the pixel's attractor points
+    const float a_mine = NORMED ? fmaxf(arow[2 * ai], 0.f) + 1e-3f : softplus_f(arow[ai]);
+    float delta = 0.f;
+#pragma unroll
+    for (int i = 0; i < NA; ++i) {
+        const float dx = __shfl_sync(0xffffffffu, a_mine, i) - b;
+        delta += __fdividef(dx, 1.f + 300.f * (dx * dx));
+    }
+    const float bn = b + delta / (float)NA;
+    const size_t o = ((size_t)(f * H + y) * W + x) * 64 + k;
+    if (!NORMED || !sort_clip) {
+        if (ok) bout[o] = bn;
+        return;
+    }
+    s_c[threadIdx.x] = (dmax - dmin) * bn + dmin;        // sort_clip is uniform over the grid: every thread reaches the barriers
+    __syncthreads();
+    const int base = threadIdx.x & ~63;
+#pragma unroll
+    for (int size = 2; size <= 64; size <<= 1) {
+#pragma unroll
+        for (int stride = size >> 1; stride > 0; stride >>= 1) {
+            const int partner = k ^ stride;
+            if (partner > k) {
+                const float u = s_c[base + k], v = s_c[base + partner];
+                if ((u > v) == ((k & size) == 0)) { s_c[base + k] = v; s_c[base + partner] = u; }
+            }
+            __syncthreads();
+        }
+    }
+    if (ok) bout[o] = fminf(fmaxf(s_c[threadIdx.x], dmin), dmax);
+}
+
+// ConditionalLogBinomial(33, 128, 64) + expectation of the single head, per net pixel: as clb_final_kernel, with 33 main inputs
+// (the 32 out_conv channels and the core's relative depth, zoedepth_v1.py:171-186) and an 80-wide hidden layer.  The relative depth
+// is the DPT output at the same size, relu(wr . out_conv + br) (base_models/midas.py:268), computed here from the out_conv values
+// this thread reads anyway.
+constexpr int CLB1_IN = 33, CLB1_HID = 80;
+struct ClbSingleParams {
+    const __half *o32; int ldo;          // [F, nh, nw, ldo] relu'd out_conv activation, channels 0..31
+    const float *ze; int ldz;            // [F, h3, w3, ldz]: W_e . b_emb, columns 0..79
+    const float *bc;                     // [F, h3, w3, 64] bin centres
+    const float *wo;                     // [33][80] (input channel major; row 32 = relative depth)
+    const float *b0;                     // [80]
+    const float *w2;                     // [4][80]
+    const float *b2;                     // [4]
+    const float *wr; float br;           // [32], scalar: the core's final 1x1 conv
+    int F, nh, nw, h3, w3;
+    float sy, sx, min_temp, max_temp;
+    float *out;                          // [F, nh, nw]
+};
+
+__global__ void __launch_bounds__(128) clb_single_kernel(ClbSingleParams p) {
+    __shared__ float s_wo[CLB1_IN * CLB1_HID], s_b0[CLB1_HID], s_w2[4 * CLB1_HID], s_b2[4], s_lb[64], s_wr[32];
+    const int f = blockIdx.z;
+    for (int i = threadIdx.x; i < CLB1_IN * CLB1_HID; i += 128) s_wo[i] = p.wo[i];
+    for (int i = threadIdx.x; i < 4 * CLB1_HID; i += 128) s_w2[i] = p.w2[i];
+    if (threadIdx.x < CLB1_HID) s_b0[threadIdx.x] = p.b0[threadIdx.x];
+    if (threadIdx.x < 4) s_b2[threadIdx.x] = p.b2[threadIdx.x];
+    if (threadIdx.x < 64) s_lb[threadIdx.x] = log_binom_f(63.f, (float)threadIdx.x);
+    if (threadIdx.x < 32) s_wr[threadIdx.x] = p.wr[threadIdx.x];
+    __syncthreads();
+    const int y = blockIdx.y, x = blockIdx.x * 128 + threadIdx.x;
+    if (x >= p.nw) return;
+    const float fy = p.sy * (float)y, fx = p.sx * (float)x;
+    const int y0 = min((int)fy, p.h3 - 1), y1 = min(y0 + 1, p.h3 - 1), x0 = min((int)fx, p.w3 - 1), x1 = min(x0 + 1, p.w3 - 1);
+    const float ly = fy - (float)y0, hy = 1.f - ly, lx = fx - (float)x0, hx = 1.f - lx;
+    const size_t i00 = ((size_t)f * p.h3 + y0) * p.w3 + x0, i01 = ((size_t)f * p.h3 + y0) * p.w3 + x1;
+    const size_t i10 = ((size_t)f * p.h3 + y1) * p.w3 + x0, i11 = ((size_t)f * p.h3 + y1) * p.w3 + x1;
+    float pre[CLB1_HID];
+    {
+        const float4 *z00 = reinterpret_cast<const float4 *>(p.ze + i00 * p.ldz), *z01 = reinterpret_cast<const float4 *>(p.ze + i01 * p.ldz);
+        const float4 *z10 = reinterpret_cast<const float4 *>(p.ze + i10 * p.ldz), *z11 = reinterpret_cast<const float4 *>(p.ze + i11 * p.ldz);
+#pragma unroll
+        for (int k = 0; k < CLB1_HID / 4; ++k) {
+            const float4 a = __ldg(z00 + k), b = __ldg(z01 + k), c = __ldg(z10 + k), d = __ldg(z11 + k);
+            pre[4 * k + 0] = s_b0[4 * k + 0] + (hy * (hx * a.x + lx * b.x) + ly * (hx * c.x + lx * d.x));
+            pre[4 * k + 1] = s_b0[4 * k + 1] + (hy * (hx * a.y + lx * b.y) + ly * (hx * c.y + lx * d.y));
+            pre[4 * k + 2] = s_b0[4 * k + 2] + (hy * (hx * a.z + lx * b.z) + ly * (hx * c.z + lx * d.z));
+            pre[4 * k + 3] = s_b0[4 * k + 3] + (hy * (hx * a.w + lx * b.w) + ly * (hx * c.w + lx * d.w));
+        }
+    }
+    float rel = 0.f;
+    {
+        const uint4 *op = reinterpret_cast<const uint4 *>(p.o32 + (((size_t)f * p.nh + y) * p.nw + x) * p.ldo);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            const uint4 u = __ldg(op + q);
+            const __half2 *h2 = reinterpret_cast<const __half2 *>(&u);
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const float2 o2 = __half22float2(h2[e]);
+                const int c = q * 8 + 2 * e;
+                rel = fmaf(s_wr[c + 1], o2.y, fmaf(s_wr[c], o2.x, rel));
+                const float *w0 = s_wo + c * CLB1_HID, *w1 = w0 + CLB1_HID;
+#pragma unroll
+                for (int k = 0; k < CLB1_HID; ++k) pre[k] = fmaf(w1[k], o2.y, fmaf(w0[k], o2.x, pre[k]));
+            }
+        }
+    }
+    rel = fmaxf(rel + p.br, 0.f);
+    {
+        const float *wrel = s_wo + 32 * CLB1_HID;
+#pragma unroll
+        for (int k = 0; k < CLB1_HID; ++k) pre[k] = fmaf(wrel[k], rel, pre[k]);
+    }
+    float pt[4] = {s_b2[0], s_b2[1], s_b2[2], s_b2[3]};
+#pragma unroll
+    for (int k = 0; k < CLB1_HID; ++k) {
+        const float g = 0.5f * pre[k] * (1.f + erff(pre[k] * 0.70710678118654752f));                 // nn.GELU (erf form)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) pt[j] = fmaf(s_w2[j * CLB1_HID + k], g, pt[j]);
+    }
+    const float pa = softplus_f(pt[0]) + 1e-4f, pb = softplus_f(pt[1]) + 1e-4f, ta = softplus_f(pt[2]) + 1e-4f, tb = softplus_f(pt[3]) + 1e-4f;
+    const float prob = pa / (pa + pb);
+    const float temp = (p.max_temp - p.min_temp) * (ta / (ta + tb)) + p.min_temp;
+    const float lp = logf(fminf(fmaxf(prob, 1e-4f), 1.f)), lq = logf(fminf(fmaxf(1.f - prob, 1e-4f), 1.f));
+    const float inv_t = 1.f / temp;
+    float mx = -INFINITY;
+#pragma unroll 8
+    for (int k = 0; k < 64; ++k) mx = fmaxf(mx, (s_lb[k] + (float)k * lp + (float)(63 - k) * lq) * inv_t);
+    const float4 *c00 = reinterpret_cast<const float4 *>(p.bc + i00 * 64), *c01 = reinterpret_cast<const float4 *>(p.bc + i01 * 64);
+    const float4 *c10 = reinterpret_cast<const float4 *>(p.bc + i10 * 64), *c11 = reinterpret_cast<const float4 *>(p.bc + i11 * 64);
+    float den = 0.f, num = 0.f;
+#pragma unroll 4
+    for (int k4 = 0; k4 < 16; ++k4) {
+        const float4 a = __ldg(c00 + k4), b = __ldg(c01 + k4), c = __ldg(c10 + k4), d = __ldg(c11 + k4);
+        const float bcv[4] = {hy * (hx * a.x + lx * b.x) + ly * (hx * c.x + lx * d.x), hy * (hx * a.y + lx * b.y) + ly * (hx * c.y + lx * d.y),
+                              hy * (hx * a.z + lx * b.z) + ly * (hx * c.z + lx * d.z), hy * (hx * a.w + lx * b.w) + ly * (hx * c.w + lx * d.w)};
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const int k = 4 * k4 + e;
+            const float ek = expf((s_lb[k] + (float)k * lp + (float)(63 - k) * lq) * inv_t - mx);
+            den += ek;
+            num = fmaf(ek, bcv[e], num);
+        }
+    }
+    p.out[((size_t)f * p.nh + y) * p.nw + x] = num / den;
+}
+
 }  // namespace dm
 
 #define DM_EXPORT extern "C" __attribute__((visibility("default")))
@@ -478,5 +678,74 @@ DM_EXPORT int dm_zoe_tta_combine(const float *d, int B, int nh, int nw, int pad_
     const long long total = (long long)B * H * W;
     tta_combine_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream_>>>(d, B, nh, nw, H + 2 * pad_h, W + 2 * pad_w, pad_h, pad_w, H, W, out);
     DM_LAUNCH_CHECK("tta_combine_kernel");
+    return DM_OK;
+}
+
+DM_EXPORT int dm_zoe_seed_bins(const float *seed, int ld, long long rows, int normed, float min_depth, float max_depth, float *out, void *stream_) {
+    using namespace dm;
+    if (!seed || !out || rows < 0 || ld < 64 || ld % 2 || (normed != 0 && normed != 1) || (normed && !(max_depth > min_depth))) {
+        set_error("dm_zoe_seed_bins: bad arguments (ld >= 64 and even, normed 0 / 1, max_depth > min_depth)");
+        return DM_E_INVALID;
+    }
+    if (rows == 0) return DM_OK;
+    seed_bins_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, (cudaStream_t)stream_>>>(seed, ld, rows, normed, min_depth, max_depth, out);
+    DM_LAUNCH_CHECK("seed_bins_kernel");
+    return DM_OK;
+}
+
+DM_EXPORT int dm_zoe_attractor_single(const float *A, int lda, int n_attractors, int normed, const float *b_prev, int F, int Hp, int Wp, int H,
+                                      int W, int sort_clip, float min_depth, float max_depth, float *b_out, void *stream_) {
+    using namespace dm;
+    if (n_attractors != 16 && n_attractors != 8 && n_attractors != 4 && n_attractors != 1) {
+        set_error("dm_zoe_attractor_single: %d attractors (implemented: 16, 8, 4, 1)", n_attractors);
+        return DM_E_UNSUPPORTED;
+    }
+    if (!A || !b_prev || !b_out || (normed != 0 && normed != 1) || (sort_clip != 0 && sort_clip != 1) || (sort_clip && !normed) ||
+        lda < (normed ? 2 : 1) * n_attractors || F < 1 || Hp < 1 || Wp < 1 || H < 1 || W < 1 || H > 65535 || F > 65535 ||
+        (normed && !(max_depth > min_depth))) {
+        set_error("dm_zoe_attractor_single: bad arguments (lda >= %d, sort_clip only for the normed head, max_depth > min_depth)",
+                  (normed ? 2 : 1) * n_attractors);
+        return DM_E_INVALID;
+    }
+    const float sy = H > 1 ? (float)(Hp - 1) / (float)(H - 1) : 0.f;
+    const float sx = W > 1 ? (float)(Wp - 1) / (float)(W - 1) : 0.f;
+    const dim3 grid((unsigned)((W * 64 + 255) / 256), (unsigned)H, (unsigned)F);
+    cudaStream_t st = (cudaStream_t)stream_;
+#define DM_ATT1(NA, NORMED) attractor_single_kernel<NA, NORMED><<<grid, 256, 0, st>>>(A, lda, b_prev, Hp, Wp, H, W, sy, sx, sort_clip, min_depth, max_depth, b_out)
+    switch (n_attractors * 2 + normed) {
+        case 32: DM_ATT1(16, false); break;
+        case 33: DM_ATT1(16, true); break;
+        case 16: DM_ATT1(8, false); break;
+        case 17: DM_ATT1(8, true); break;
+        case 8: DM_ATT1(4, false); break;
+        case 9: DM_ATT1(4, true); break;
+        case 2: DM_ATT1(1, false); break;
+        default: DM_ATT1(1, true); break;
+    }
+#undef DM_ATT1
+    DM_LAUNCH_CHECK("attractor_single_kernel");
+    return DM_OK;
+}
+
+DM_EXPORT int dm_zoe_clb_single(const void *o32, int ldo, const float *ze, int ldz, const float *bc, const float *wo, const float *b0, const float *w2,
+                                const float *b2, const float *wr, float br, int F, int nh, int nw, int h3, int w3, float min_temp, float max_temp,
+                                float *out, void *stream_) {
+    using namespace dm;
+    if (!o32 || !ze || !bc || !wo || !b0 || !w2 || !b2 || !wr || !out || F < 1 || nh < 1 || nw < 1 || h3 < 1 || w3 < 1 || nh > 65535 || F > 65535) {
+        set_error("dm_zoe_clb_single: bad shape or null pointer");
+        return DM_E_INVALID;
+    }
+    if (ldo % 8 || ldo < 32 || ldz % 4 || ldz < CLB1_HID) {
+        set_error("dm_zoe_clb_single: ldo must be a multiple of 8 and >= 32, ldz a multiple of 4 and >= %d", CLB1_HID);
+        return DM_E_INVALID;
+    }
+    ClbSingleParams p;
+    p.o32 = (const __half *)o32; p.ldo = ldo; p.ze = ze; p.ldz = ldz; p.bc = bc;
+    p.wo = wo; p.b0 = b0; p.w2 = w2; p.b2 = b2; p.wr = wr; p.br = br; p.F = F; p.nh = nh; p.nw = nw; p.h3 = h3; p.w3 = w3;
+    p.sy = nh > 1 ? (float)(h3 - 1) / (float)(nh - 1) : 0.f;
+    p.sx = nw > 1 ? (float)(w3 - 1) / (float)(nw - 1) : 0.f;
+    p.min_temp = min_temp; p.max_temp = max_temp; p.out = out;
+    clb_single_kernel<<<dim3((unsigned)((nw + 127) / 128), (unsigned)nh, (unsigned)F), 128, 0, (cudaStream_t)stream_>>>(p);
+    DM_LAUNCH_CHECK("clb_single_kernel");
     return DM_OK;
 }

@@ -7,8 +7,8 @@
 the bench.  The network forward is a sequence of C-ABI calls (wgmma GEMM / implicit-GEMM conv / fused attention /
 LayerNorm / resize kernels, include/depthmap_b200.h); PyTorch only owns device memory and the stream.
 
-Implemented model types: 1, 2 (MiDaS 3.1 DPT-BEiT-L 512 / 384), 3 (MiDaS 3.0 DPT-Large 384), 9 (ZoeDepth-NK) and 12, 13, 14
-(Depth-Anything-V2 S/B/L).  Others raise NotImplementedError naming the type.
+Implemented model types: 0 (LeReS res101), 1, 2 (MiDaS 3.1 DPT-BEiT-L 512 / 384), 3 (MiDaS 3.0 DPT-Large 384), 7, 8, 9
+(ZoeDepth-N, -K, -NK) and 12, 13, 14 (Depth-Anything-V2 S/B/L).  Others raise NotImplementedError naming the type.
 Weights: a state_dict in the upstream checkpoint layout (``depth_anything_v2_vit{s,b,l}.pth``), packed once at load
 into the kernels' layout (fp16 GEMM operands, (ky,kx,cin)-ordered conv filters, ConvTranspose as GEMM + pixel shuffle).
 """
@@ -1318,6 +1318,183 @@ class ZoeDepthNKEngine(DptBeitEngine):
         return out
 
 
+# ZoeDepth-N / -K: get_config("zoedepth", "infer") and its "kitti" version.  Neither sets min_depth / max_depth, so both keep
+# ZoeDepth.__init__'s 1e-3 / 10 (dzoedepth/models/zoedepth/zoedepth_v1.py:39); K's centres are clipped at 10 like the reference's.
+ZOE_SINGLE_CONFIG = dict(n_bins=64, bin_embedding_dim=128, n_attractors=[16, 8, 4, 1], min_temp=0.0212, max_temp=50.0, min_depth=1e-3, max_depth=10.0)
+ZOE_SINGLE_VARIANTS = {'n': dict(model_type=7, bin_centers_type='softplus', checkpoint='ZoeD_M12_N.pt'),
+                       'k': dict(model_type=8, bin_centers_type='normed', checkpoint='ZoeD_M12_K.pt')}
+
+
+class ZoeDepthEngine(DptBeitEngine):
+    """Single-head ZoeDepth on the sm_90a kernels: ZoeDepth-N (variant 'n', model type 7, softplus bin centres) and ZoeDepth-K
+    ('k', model type 8, bin centres normed to [min_depth, max_depth]).  Same core, pre-processing and pad + flip test-time
+    augmentation as ZoeDepthNKEngine (image b and its flip are forwards 2b / 2b+1); the head is ZoeDepth.forward
+    (dzoedepth/models/zoedepth/zoedepth_v1.py:124-192): seed bins, four attractor levels with [16, 8, 4, 1] attractors, and a
+    log-binomial whose 33rd input is the core's own relative depth.  Bin centres, attractor points and the log-binomial stay in
+    fp32.  Checkpoint layout as ZoeDepth-NK: MiDaS weights under "core.core.", head weights at the top level."""
+
+    def __init__(self, state_dict, device, variant, core_name='beitl16_384'):
+        if variant not in ZOE_SINGLE_VARIANTS:
+            raise ValueError(f"ZoeDepthEngine: variant must be 'n' or 'k', not {variant!r}")
+        self.variant = variant
+        self.normed = ZOE_SINGLE_VARIANTS[variant]['bin_centers_type'] == 'normed'
+        core_sd = {k[len("core.core."):]: v for k, v in state_dict.items() if k.startswith("core.core.")}
+        head_sd = {k: v for k, v in state_dict.items() if not k.startswith("core.")}
+        super().__init__(core_sd, core_name, device)
+        self._pack_head(head_sd)
+        self._zbuf_key, self._zbufs = None, {}
+
+    def _pack(self, sd):
+        self._oc2_weight = sd['scratch.output_conv.2.weight'].detach()
+        self._oc2_bias = sd['scratch.output_conv.2.bias'].detach()
+        super()._pack(sd)
+
+    def _pack_head(self, sd):
+        import torch
+        dev = self.device
+
+        def W(key, rows=None):                 # 1x1 conv weight -> fp16 [rows, cin] (zero padded rows)
+            t = sd[key + '.weight'].detach().to(dev).float()
+            t = t.reshape(t.shape[0], -1)
+            o = torch.zeros(rows or t.shape[0], t.shape[1], dtype=torch.float16, device=dev)
+            o[:t.shape[0]] = t.to(torch.float16)
+            return o
+
+        def Bv(key, n=None):
+            t = sd[key + '.bias'].detach().to(dev).float().reshape(-1)
+            o = torch.zeros(n or t.numel(), dtype=torch.float32, device=dev)
+            o[:t.numel()] = t
+            return o
+
+        def mlp(key):
+            return ((W(key + '._net.0'), Bv(key + '._net.0')), (W(key + '._net.2'), Bv(key + '._net.2')))
+
+        z = {'conv2': (W('conv2'), Bv('conv2')), 'seed': mlp('seed_bin_regressor'), 'sproj': mlp('seed_projector'),
+             'proj': [mlp(f'projectors.{i}') for i in range(4)]}
+        if z['seed'][1][0].shape[0] != ZOE_SINGLE_CONFIG['n_bins']:
+            raise ValueError(f"ZoeDepthEngine: the seed bin regressor has {z['seed'][1][0].shape[0]} outputs, not 64 bins")
+        per = 2 if self.normed else 1
+        att = []
+        for i, n in enumerate(ZOE_SINGLE_CONFIG['n_attractors']):
+            key = f'attractors.{i}._net.2'
+            if sd[key + '.weight'].shape[0] != per * n:
+                raise ValueError(f"ZoeDepthEngine({self.variant!r}): {key} has {sd[key + '.weight'].shape[0]} outputs, expected {per * n} "
+                                 f"({n} attractors{' x 2 for the normed layer' if self.normed else ''})")
+            att.append(((W(f'attractors.{i}._net.0'), Bv(f'attractors.{i}._net.0')), (W(key, rows=32), Bv(key, 32))))
+        z['att'] = att
+        # conditional log-binomial: mlp.0 over cat(out_conv (32), rel_depth (1), b_emb (128)), 80 outputs.  Its out_conv and
+        # rel-depth part is evaluated per pixel in clb_single, its bin-embedding part is a GEMM before the up-sampling (a 1x1 conv
+        # commutes with bilinear interpolation), as in ZoeDepth-NK
+        m0 = sd['conditional_log_binomial.mlp.0.weight'].detach().to(dev).float()
+        if tuple(m0.shape[:2]) != (80, 161):
+            raise ValueError(f"ZoeDepthEngine: conditional_log_binomial.mlp.0 is {tuple(m0.shape)}, expected (80, 161, 1, 1)")
+        m0 = m0.reshape(80, 161)
+        we = torch.zeros(128, 128, dtype=torch.float16, device=dev)
+        we[:80] = m0[:, 33:].to(torch.float16)
+        z['clb'] = (we, m0[:, :33].t().contiguous(), Bv('conditional_log_binomial.mlp.0'),
+                    sd['conditional_log_binomial.mlp.2.weight'].detach().to(dev).float().reshape(4, 80).contiguous(),
+                    Bv('conditional_log_binomial.mlp.2'))
+        z['oc2_w'] = _conv_w(self._oc2_weight.to(dev), self.F2p, 32)
+        z['oc2_b'] = self._oc2_bias.to(dev).float().contiguous()
+        self.z = z
+
+    def _zbuffers(self, F, nh, nw, b):
+        import torch
+        key = (F, nh, nw)
+        if self._zbuf_key == key:
+            return self._zbufs
+        dev = self.device
+        h16 = lambda *s: torch.empty(*s, dtype=torch.float16, device=dev)
+        f32 = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
+        s3 = b['sizes'][3]
+        n0 = s3[0] * s3[1]
+        levels = list(b['up_sizes'])                       # (h, w) of refinenet4..1 outputs
+        zb = dict(x16=h16(F * n0, self.Fp), s0=h16(F * n0, 256), seed=f32(F * n0, 64), bprev=f32(F * n0, 64), p0=h16(F * n0, 128),
+                  pemb=h16(F * n0, 128), n0=n0, levels=levels)
+        zb['t'] = [h16(F * h * w, 128) for h, w in levels]
+        zb['bemb'] = [h16(F * h * w, 128) for h, w in levels]
+        zb['xin'] = [h16(F * h * w, 128) for h, w in levels]
+        zb['a0'] = [h16(F * h * w, 128) for h, w in levels]
+        zb['A'] = [f32(F * h * w, 32) for h, w in levels]
+        zb['bnew'] = [f32(F * h * w, 64) for h, w in levels]
+        zb['ze'] = f32(F * levels[3][0] * levels[3][1], 128)
+        zb['o32'] = h16(F, nh, nw, 32)
+        zb['d'] = f32(F, nh, nw)
+        self._zbufs, self._zbuf_key = zb, key
+        return zb
+
+    def forward_batch(self, rgb, net_w, net_h=None, out_hw=None):
+        """rgb: uint8 CUDA [B,H,W,3] -> float32 CUDA [B,H,W] metric depth (what estimatezoedepth returns; invert = True)."""
+        import torch
+        L = self.ops.L
+        ops, z = self.ops, self.z
+        st = _lib.stream_ptr
+        cfg = ZOE_SINGLE_CONFIG
+        dmin, dmax = cfg['min_depth'], cfg['max_depth']
+        B, H, W, _ = rgb.shape
+        net_h = net_h if net_h is not None else net_w
+        pad_h, pad_w = int(np.sqrt(H / 2) * 3.0), int(np.sqrt(W / 2) * 3.0)       # depth_model.py:80-82 (fh = fw = 3)
+        Hp, Wp = H + 2 * pad_h, W + 2 * pad_w
+        nw, nh = midas_net_size(Wp, Hp, net_w, net_h)                               # PrepForMidas: keep aspect, x32, "minimal"
+        F = 2 * B
+        b = self._buffers(F, nh, nw)
+        _lib.check(L.dm_zoe_preprocess_patchify(rgb.data_ptr(), B, H, W, pad_h, pad_w, nh, nw, self.PATCH, b['patches'].data_ptr(), self.kpad, st()),
+                   "dm_zoe_preprocess_patchify")
+        ops.launches += 1
+        self.run_network(b, F, nh, nw)
+        zb = self._zbuffers(F, nh, nw, b)
+        Fp = self.Fp
+        E_, A_ = _lib, _lib
+        # out_conv activation (MidasCore hooks output_conv[3], the 32-channel ReLU); the core's relative depth, the final 1x1 conv
+        # + ReLU on it, is evaluated inside clb_single
+        t = b['up_sizes'][3]
+        ops.conv3x3(b['path'][3], F, t[0], t[1], Fp, self.w['oc1_w'], self.F2p, bias=self.w['oc1_b'], C=b['oc1'])
+        ops.resize_nhwc(b['oc1'], F, t[0], t[1], self.F2p, b['oc1u'], nh, nw)
+        ops.conv3x3(b['oc1u'], F, nh, nw, self.F2p, z['oc2_w'], 32, act=A_.ACT_RELU, bias=z['oc2_b'], C=zb['o32'])
+        n0, s3 = zb['n0'], b['sizes'][3]
+
+        def lin(a, lda, wb, M, N, K, out=None, act=A_.ACT_NONE, f32out=None):
+            wt, bias = wb
+            if f32out is not None:
+                ops.gemm(a, lda, wt, K, M, N, K, epi=E_.EPI_STORE_F32, act=act, bias=bias, X=f32out, ldx=N)
+            else:
+                ops.gemm(a, lda, wt, K, M, N, K, act=act, bias=bias, C=out, ldc=N)
+
+        # x = conv2(bottleneck); seed bins (zoedepth_v1.py:151-159) and seed embedding (:161)
+        lin(b['l'][3], Fp, z['conv2'], F * n0, Fp, Fp, out=zb['x16'])
+        lin(zb['x16'], Fp, z['seed'][0], F * n0, 256, Fp, out=zb['s0'], act=A_.ACT_RELU)
+        lin(zb['s0'], 256, z['seed'][1], F * n0, 64, 256, f32out=zb['seed'])
+        _lib.check(L.dm_zoe_seed_bins(zb['seed'].data_ptr(), 64, F * n0, int(self.normed), dmin, dmax, zb['bprev'].data_ptr(), st()), "dm_zoe_seed_bins")
+        lin(zb['x16'], Fp, z['sproj'][0], F * n0, 128, Fp, out=zb['p0'], act=A_.ACT_RELU)
+        lin(zb['p0'], 128, z['sproj'][1], F * n0, 128, 128, out=zb['pemb'])
+        ops.launches += 1
+        # attractor levels (:164-169); the normed head's last level hands on sorted, clipped centres
+        bprev, pemb, (hp, wp) = zb['bprev'], zb['pemb'], s3
+        for i, (h, w) in enumerate(zb['levels']):
+            M = F * h * w
+            lin(b['path'][i], Fp, z['proj'][i][0], M, 128, Fp, out=zb['t'][i], act=A_.ACT_RELU)
+            lin(zb['t'][i], 128, z['proj'][i][1], M, 128, 128, out=zb['bemb'][i])
+            _lib.check(L.dm_resize_add_nhwc_f16(zb['bemb'][i].data_ptr(), pemb.data_ptr(), F, hp, wp, 128, zb['xin'][i].data_ptr(), h, w, st()),
+                       "dm_resize_add_nhwc_f16")
+            lin(zb['xin'][i], 128, z['att'][i][0], M, 128, 128, out=zb['a0'][i], act=A_.ACT_RELU)
+            lin(zb['a0'][i], 128, z['att'][i][1], M, 32, 128, f32out=zb['A'][i])
+            sort_clip = int(self.normed and i == len(zb['levels']) - 1)
+            _lib.check(L.dm_zoe_attractor_single(zb['A'][i].data_ptr(), 32, cfg['n_attractors'][i], int(self.normed), bprev.data_ptr(), F, hp, wp,
+                                                 h, w, sort_clip, dmin, dmax, zb['bnew'][i].data_ptr(), st()), "dm_zoe_attractor_single")
+            ops.launches += 2
+            bprev, pemb, (hp, wp) = zb['bnew'][i], zb['bemb'][i], (h, w)
+        # conditional log-binomial on cat(out_conv, rel_depth) + expectation (:171-192), then un-pad / un-flip / average
+        we, wo, b0, w2c, b2c = z['clb']
+        ops.gemm(zb['bemb'][3], 128, we, 128, F * hp * wp, 128, 128, epi=E_.EPI_STORE_F32, X=zb['ze'], ldx=128)
+        _lib.check(L.dm_zoe_clb_single(zb['o32'].data_ptr(), 32, zb['ze'].data_ptr(), 128, bprev.data_ptr(), wo.data_ptr(), b0.data_ptr(),
+                                       w2c.data_ptr(), b2c.data_ptr(), self.w['oc3_w'].data_ptr(), self.oc3_b, F, nh, nw, hp, wp,
+                                       cfg['min_temp'], cfg['max_temp'], zb['d'].data_ptr(), st()), "dm_zoe_clb_single")
+        out = torch.empty(B, H, W, dtype=torch.float32, device=self.device)
+        _lib.check(L.dm_zoe_tta_combine(zb['d'].data_ptr(), B, nh, nw, pad_h, pad_w, H, W, out.data_ptr(), st()), "dm_zoe_tta_combine")
+        ops.launches += 2
+        return out
+
+
 class ModelHolder:
     """Same public surface as the reference's ModelHolder (src/depthmap_generation.py:40-403)."""
 
@@ -1422,9 +1599,22 @@ class ModelHolder:
                 if "model" in sd:           # dzoedepth/models/model_io.py:52-53
                     sd = sd["model"]
             model = ZoeDepthNKEngine(sd, torch.device(device))
+        elif model_type in (7, 8):  # zoedepth_n (indoor) / zoedepth_k (outdoor) (src/depthmap_generation.py:196-204)
+            variant = {7: 'n', 8: 'k'}[model_type]
+            if self.weights_provider is not None:
+                sd = self.weights_provider(model_type)
+            else:
+                model_path = "./models/zoedepth/" + ZOE_SINGLE_VARIANTS[variant]['checkpoint']
+                if not os.path.exists(model_path):
+                    raise FileNotFoundError(f"{model_path} not found (depthmap_b200 does not download checkpoints)")
+                sd = torch.load(model_path, map_location='cpu')
+            if "model" in sd:               # dzoedepth/models/model_io.py:52-53
+                sd = sd["model"]
+            model = ZoeDepthEngine(sd, torch.device(device), variant)
         else:
             raise NotImplementedError(f"model_type {model_type} is not implemented in depthmap_b200 yet "
-                                      f"(implemented: 0 = LeReS res101; 1, 2 = DPT-BEiT-L 512/384; 3 = DPT-Large 384; 9 = ZoeDepth-NK; 12, 13, 14 = Depth-Anything-V2 S/B/L)")
+                                      f"(implemented: 0 = LeReS res101; 1, 2 = DPT-BEiT-L 512/384; 3 = DPT-Large 384; 7 = ZoeDepth-N; "
+                                      f"8 = ZoeDepth-K; 9 = ZoeDepth-NK; 12, 13, 14 = Depth-Anything-V2 S/B/L)")
         if boost:      # reference :284-299: the pix2pix merge network ('latest_net_G.pth', netG = unet_1024, norm none)
             from .boost import BoostPipeline, UnetMergeEngine
             if self.weights_provider is not None:
@@ -1489,7 +1679,7 @@ class ModelHolder:
             import torch
             preds = [self.pix2pix_model.run(rgb[i].cpu().numpy(), self.boost_rmax, to_host=False) for i in range(rgb.shape[0])]
             return torch.stack(preds), self.depth_model_type in [0, 7, 8, 9, 10]
-        if self.depth_model_type in (0, 1, 2, 3, 9, 12, 13, 14):
+        if self.depth_model_type in (0, 1, 2, 3, 7, 8, 9, 12, 13, 14):
             pred = self.depth_model.forward_batch(rgb, net_width, net_height)
         else:
             raise NotImplementedError(f"model_type {self.depth_model_type}")
