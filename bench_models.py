@@ -430,7 +430,7 @@ class BoostRes101:
         torch.cuda.synchronize()
         if world > 1:
             dist.barrier()
-        n0 = self.pipe.launches + self.pipe.depth.ops.launches + self.pipe.merge.ops.launches
+        n0 = self.pipe.ops.launches + self.pipe.depth.ops.launches + self.pipe.merge.ops.launches
         sampler = ClockSampler(local_rank) if rank == 0 else None
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
@@ -444,7 +444,7 @@ class BoostRes101:
         if world > 1:
             dist.barrier()
         clocks = sampler.stop() if sampler else None
-        launches = self.pipe.launches + self.pipe.depth.ops.launches + self.pipe.merge.ops.launches - n0
+        launches = self.pipe.ops.launches + self.pipe.depth.ops.launches + self.pipe.merge.ops.launches - n0
         t = torch.tensor([e0.elapsed_time(e1)], dtype=torch.float64, device=dev)
         if world > 1:
             dist.all_reduce(t, op=dist.ReduceOp.MAX)

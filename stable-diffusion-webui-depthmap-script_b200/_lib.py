@@ -3,6 +3,7 @@ from __future__ import annotations
 
 import ctypes
 import os
+import sys
 import threading
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -229,3 +230,88 @@ def require_cuda():
 def stream_ptr():
     import torch
     return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+def _ptr(t):
+    return t.data_ptr() if t is not None else None
+
+
+def _gemm_desc(M, N, K, epi, act, bias, C, ldc, C2, R, ldr, R2, ldr2, X, ldx, gamma, head_b2, ps=None):
+    return GemmDesc(M, N, K, epi, act, _ptr(bias), _ptr(C), ldc, _ptr(C2), _ptr(R), ldr, _ptr(R2), ldr2, _ptr(X), ldx, _ptr(gamma), head_b2,
+                    *(ps or (0, 0, 0, 0)))
+
+
+class Ops:
+    """Checked kernel calls on the current torch stream, with a running count of the kernels they issue (`launches`)."""
+
+    def __init__(self):
+        import torch
+        self._tensor = torch.Tensor
+        self.L = load()
+        for name in ("dm_gemm_ex", "dm_conv3x3_ex", "dm_attention_f16", "dm_layernorm_f16"):
+            if not hasattr(self.L, name):
+                raise RuntimeError(f"depthmap_b200: native library lacks {name}; rebuild csrc (no fallback exists)")
+        self.launches = 0
+
+    def call(self, name, *args, launches=1):
+        """L.name(*args, stream): a tensor goes in as its data pointer, None as NULL; a status other than DM_OK raises.
+        `launches`: the kernels this call issues."""
+        T = self._tensor
+        check(getattr(self.L, name)(*[a.data_ptr() if isinstance(a, T) else a for a in args], stream_ptr()), name)
+        self.launches += launches
+
+    def gemm(self, A, lda, W, ldw, M, N, K, epi=EPI_STORE_F16, act=ACT_NONE, bias=None, C=None, ldc=0, C2=None,
+             R=None, ldr=0, R2=None, ldr2=0, X=None, ldx=0, gamma=None, head_b2=0.0, ps=None):
+        d = _gemm_desc(M, N, K, epi, act, bias, C, ldc, C2, R, ldr, R2, ldr2, X, ldx, gamma, head_b2, ps)
+        self.call("dm_gemm_ex", A, lda, W, ldw, ctypes.byref(d))
+
+    def conv3x3(self, act_t, B, H, W_, Cin, Wt, Cout, epi=EPI_STORE_F16, act=ACT_NONE, bias=None, C=None, C2=None,
+                R=None, R2=None, X=None, gamma=None, head_b2=0.0, ldx=1):
+        d = _gemm_desc(0, Cout, 0, epi, act, bias, C, Cout, C2, R, Cout, R2, Cout, X, ldx, gamma, head_b2)
+        self.call("dm_conv3x3_ex", act_t, B, H, W_, Cin, Wt, ctypes.byref(d))
+
+
+class GraphCache:
+    """CUDA-graph replay of a fixed launch sequence, keyed by shape.  At a key, the first call runs eagerly (it allocates), the
+    second captures and later calls replay; inside a capture someone else started the kernels are plain launches.  A failed
+    capture is reported once and leaves the caller eager: the graph is an optimisation over the same kernels.  A replay adds the
+    captured kernels to ops.launches.  `env` = "0" keeps everything eager."""
+
+    def __init__(self, ops, env, what):
+        self.ops, self.what = ops, what
+        self.enabled = os.environ.get(env, "1") != "0"
+        self._graphs, self._calls = {}, {}
+
+    def clear(self):
+        self._graphs.clear()
+        self._calls.clear()
+
+    def run(self, key, fn, *inputs, copy_out=False):
+        """fn(*inputs) -> output tensor.  A replay copies `inputs` into the captured ones and returns the captured output buffer,
+        which the next replay at this key overwrites, or with copy_out a copy of it."""
+        import torch
+        capturing = torch.cuda.is_current_stream_capturing()
+        g = self._graphs.get(key)
+        if g is not None and not capturing:
+            graph, static_in, out, n = g
+            for s, x in zip(static_in, inputs):
+                s.copy_(x)
+            graph.replay()
+            self.ops.launches += n
+            return out.clone() if copy_out else out
+        calls = self._calls[key] = self._calls.get(key, 0) + 1
+        if self.enabled and calls >= 2 and not capturing:
+            try:
+                graph = torch.cuda.CUDAGraph()
+                static_in = [x.clone() for x in inputs]
+                n0 = self.ops.launches
+                with torch.cuda.graph(graph):
+                    out = fn(*static_in)
+                self._graphs[key] = (graph, static_in, out, self.ops.launches - n0)
+                graph.replay()
+                return out.clone() if copy_out else out
+            except Exception as e:  # noqa: BLE001 — an optimisation only: the same kernels run eagerly
+                sys.stderr.write(f"[depthmap_b200] {self.what} graph capture failed ({e}); running eagerly\n")
+                torch.cuda.synchronize()
+                self.enabled = False
+        return fn(*inputs)

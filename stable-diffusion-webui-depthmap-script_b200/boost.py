@@ -19,7 +19,7 @@ are dealt round-robin to the ranks, the fitted 1024^2 patches are exchanged with
 (order-dependent) blend itself."""
 from __future__ import annotations
 
-import ctypes
+import contextlib
 import math
 
 import numpy as np
@@ -150,14 +150,6 @@ def plan(img_f64, model_type, whole_size_threshold):
 # ---------------------------------------------------------------------------------------------------------------------
 # merge network
 # ---------------------------------------------------------------------------------------------------------------------
-class _NullCtx:
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *a):
-        return False
-
-
 class UnetMergeEngine:
     """pix2pix `unet_1024` generator (2 -> 1 channels, 10 levels, norm 'none'): down = [LeakyReLU(0.2), Conv 4x4/2], up = [ReLU,
     ConvTranspose 4x4/2] with skip concatenation, tanh at the end (pix2pix/models/networks.py:444-543).  Activations stay fp32 NHWC;
@@ -172,8 +164,7 @@ class UnetMergeEngine:
         import torch
         self.device, self.split, self.kc = device, bool(split), kc
         self.copies = 3 if split else 1
-        from .depthmap_generation import _Ops
-        self.ops = _Ops()
+        self.ops = _lib.Ops()
         sd = {k[7:] if k.startswith("module.") else k: v for k, v in state_dict.items()}
         self.down, self.up = [], []
         prefix = "model."
@@ -215,10 +206,8 @@ class UnetMergeEngine:
             prefix = child
         self._bufs = {}
         # every call has the same shapes: after one eager call (allocations) the ~600 launches of a forward are captured into a CUDA
-        # graph and replayed (DEPTHMAP_B200_UNET_GRAPH=0 keeps it eager)
-        import os
-        self._use_graph = os.environ.get("DEPTHMAP_B200_UNET_GRAPH", "1") != "0"
-        self._graph, self._static_in, self._static_out, self._calls = None, None, None, 0
+        # graph and replayed
+        self._graphs = _lib.GraphCache(self.ops, "DEPTHMAP_B200_UNET_GRAPH", "merge-net")
         self._streams = [torch.cuda.Stream(device=device) for _ in range(8)] if self.split else []
 
     def _operand(self, m):
@@ -260,17 +249,12 @@ class UnetMergeEngine:
         for s_ in streams:
             s_.wait_stream(main)
         for li, (cols, K, w, M, N, k0, kk, dst) in enumerate(launches):
-            d = _lib.GemmDesc()
-            d.M, d.N, d.K, d.epi, d.act = M, N, kk, _lib.EPI_STORE_F32, _lib.ACT_NONE
-            d.X, d.ldx = dst.data_ptr(), N
-            with torch.cuda.stream(streams[li % len(streams)]) if streams else _NullCtx():
-                _lib.check(self.ops.L.dm_gemm_ex(cols.data_ptr() + k0 * 2, K, w.data_ptr() + k0 * 2, K, ctypes.byref(d), _lib.stream_ptr()), "dm_gemm_ex")
-            self.ops.launches += 1
+            with torch.cuda.stream(streams[li % len(streams)]) if streams else contextlib.nullcontext():
+                self.ops.gemm(cols[:, k0:], K, w[:, k0:], K, M, N, kk, epi=_lib.EPI_STORE_F32, X=dst, ldx=N)
         for s_ in streams:
             main.wait_stream(s_)
         for ws, n, M, N, gamma, out in jobs:
-            _lib.check(self.ops.L.dm_sum_chunks_f32(ws.data_ptr(), n, M * N, N, gamma.data_ptr(), out.data_ptr(), _lib.stream_ptr()), "dm_sum_chunks_f32")
-            self.ops.launches += 1
+            self.ops.call("dm_sum_chunks_f32", ws, n, M * N, N, gamma, out)
 
     def _buf(self, name, shape, dtype):
         import torch
@@ -283,33 +267,11 @@ class UnetMergeEngine:
 
     def forward(self, x2):
         """x2: fp32 CUDA [1024, 1024, 2] (real_A as NHWC) -> fp32 CUDA [1024, 1024] in (-1, 1)"""
-        import torch
-        if self._graph is not None and x2.shape == self._static_in.shape and not torch.cuda.is_current_stream_capturing():
-            self._static_in.copy_(x2)
-            self._graph.replay()
-            self.ops.launches += self._graph_launches                # the kernels inside the graph still launch
-            return self._static_out.clone()
-        self._calls += 1
-        if self._use_graph and self._calls == 2 and not torch.cuda.is_current_stream_capturing():
-            try:
-                self._static_in = x2.clone()
-                g = torch.cuda.CUDAGraph()
-                n0 = self.ops.launches
-                with torch.cuda.graph(g):
-                    self._static_out = self._forward(self._static_in)
-                self._graph, self._graph_launches = g, self.ops.launches - n0
-                g.replay()
-                return self._static_out.clone()
-            except Exception as e:  # noqa: BLE001 — capture is an optimisation; the eager path below is the same kernels
-                import sys
-                sys.stderr.write(f"[depthmap_b200] merge-net graph capture failed ({e}); running eagerly\n")
-                torch.cuda.synchronize()
-                self._graph, self._use_graph = None, False
-        return self._forward(x2)
+        return self._graphs.run(tuple(x2.shape), self._forward, x2, copy_out=True)
 
     def _forward(self, x2):
         import torch
-        L, ops, st, cp = self.ops.L, self.ops, _lib.stream_ptr, self.copies
+        ops, cp = self.ops, self.copies
         S = int(x2.shape[0])
         assert x2.shape == (S, S, 2) and S % 1024 == 0 and x2.dtype == torch.float32
         h = []
@@ -320,18 +282,16 @@ class UnetMergeEngine:
             K = (64 if d == 0 else 16 * cin) * cp
             if d == 0 and self.split:
                 out = self._buf("h0", (M, cout), torch.float32)
-                _lib.check(L.dm_unet_first(x2.data_ptr(), Hin, Hin, self.first_w.data_ptr(), out.data_ptr(), st()), "dm_unet_first")
-                ops.launches += 1
+                ops.call("dm_unet_first", x2, Hin, Hin, self.first_w, out)
                 h.append(out)
                 continue
             cols = self._buf("cols", (M, K), torch.float16)
             if d == 0:
-                _lib.check(L.dm_unet_first_cols(x2.data_ptr(), Hin, Hin, cols.data_ptr(), int(self.split), st()), "dm_unet_first_cols")
+                ops.call("dm_unet_first_cols", x2, Hin, Hin, cols, int(self.split))
             else:
-                _lib.check(L.dm_unet_down_cols(h[d - 1].data_ptr(), Hin, Hin, cin, cols.data_ptr(), int(self.split), st()), "dm_unet_down_cols")
+                ops.call("dm_unet_down_cols", h[d - 1], Hin, Hin, cin, cols, int(self.split))
             out = self._buf(f"h{d}", (M, cout), torch.float32)
             self._gemms([(cols, K, self.down[d], M, cout, out)])
-            ops.launches += 1
             h.append(out)
         u, cu = None, 0
         for d in range(9, -1, -1):
@@ -340,25 +300,22 @@ class UnetMergeEngine:
             c1 = self.CH[d][1]
             if d == 0 and self.split:
                 out = torch.empty(2 * Hs, 2 * Hs, dtype=torch.float32, device=self.device)
-                _lib.check(L.dm_unet_last(h[0].data_ptr(), c1, u.data_ptr(), cu, Hs, Hs, self.last_w.data_ptr(), self.bias, out.data_ptr(), st()), "dm_unet_last")
-                ops.launches += 1
+                ops.call("dm_unet_last", h[0], c1, u, cu, Hs, Hs, self.last_w, self.bias, out)
                 break
             K = 4 * (c1 + cu) * cp
             cols = self._buf("cols", (4, M, K), torch.float16)
-            _lib.check(L.dm_unet_up_cols(h[d].data_ptr(), c1, u.data_ptr() if u is not None else None, cu, Hs, Hs, cols.data_ptr(), int(self.split), st()),
-                       "dm_unet_up_cols")
+            ops.call("dm_unet_up_cols", h[d], c1, u, cu, Hs, Hs, cols, int(self.split))
             weights, cout = self.up[d]
             N = max(cout, 32)
             tmp = self._buf("tmp", (4, M, N), torch.float32)
             self._gemms([(cols[par], K, weights[par], M, N, tmp[par]) for par in range(4)])
             if d > 0:
                 u = self._buf(f"u{d}", (2 * Hs, 2 * Hs, cout), torch.float32)
-                _lib.check(L.dm_unet_interleave(tmp.data_ptr(), Hs, Hs, N, cout, u.data_ptr(), st()), "dm_unet_interleave")
+                ops.call("dm_unet_interleave", tmp, Hs, Hs, N, cout, u)
                 cu = cout
             else:
                 out = torch.empty(2 * Hs, 2 * Hs, dtype=torch.float32, device=self.device)
-                _lib.check(L.dm_unet_final(tmp.data_ptr(), Hs, Hs, N, self.bias, out.data_ptr(), st()), "dm_unet_final")
-            ops.launches += 2
+                ops.call("dm_unet_final", tmp, Hs, Hs, N, self.bias, out)
         return out
 
 
@@ -378,27 +335,23 @@ class BoostPipeline:
                                       f"not model type {model_type}")
         self.depth, self.merge, self.device, self.model_type = depth_engine, merge_engine, device, model_type
         self.midas = model_type != 0      # estimatemidasBoost: crop-size min-max normalisation of every estimate
-        self.L = _lib.load()
-        self.P = int(self.L.dm_boost_partials())
+        self.ops = _lib.Ops()
+        self.P = int(self.ops.L.dm_boost_partials())
         self.profile = torch.from_numpy(mask_profile()).to(device)
         self._degenerate = torch.zeros(1, dtype=torch.int32, device=device)
-        self.launches = 0
 
     # -- small device helpers ---------------------------------------------------------------------------------------
     def _cubic(self, src, pitch, hin, win, hout, wout, planes=1, src_plane=0, out=None):
         import torch
         if out is None:
             out = torch.empty((planes, hout, wout) if planes > 1 else (hout, wout), dtype=torch.float32, device=self.device)
-        _lib.check(self.L.dm_boost_resize_cubic(src, pitch, src_plane, hin, win, out.data_ptr(), wout, hout * wout, hout, wout, planes, _lib.stream_ptr()),
-                   "dm_boost_resize_cubic")
-        self.launches += 1
+        self.ops.call("dm_boost_resize_cubic", src, pitch, src_plane, hin, win, out, wout, hout * wout, hout, wout, planes)
         return out
 
     def _minmax(self, x):
         import torch
         p = torch.empty(self.P * 2, dtype=torch.float32, device=self.device)
-        _lib.check(self.L.dm_boost_minmax(x.data_ptr(), x.numel(), p.data_ptr(), _lib.stream_ptr()), "dm_boost_minmax")
-        self.launches += 1
+        self.ops.call("dm_boost_minmax", x, x.numel(), p)
         return p
 
     def _merge(self, outer, inner):
@@ -407,18 +360,14 @@ class BoostPipeline:
         n = outer.numel()
         x2 = torch.empty(PIX2PIX_SIZE, PIX2PIX_SIZE, 2, dtype=torch.float32, device=self.device)
         po, pi = self._minmax(outer), self._minmax(inner)
-        _lib.check(self.L.dm_boost_merge_input(outer.data_ptr(), inner.data_ptr(), n, po.data_ptr(), pi.data_ptr(), x2.data_ptr(), _lib.stream_ptr()),
-                   "dm_boost_merge_input")
-        self.launches += 1
+        self.ops.call("dm_boost_merge_input", outer, inner, n, po, pi, x2)
         return self.merge.forward(x2)
 
     def _post(self, t, normalise):
         import torch
         out = torch.empty_like(t)
         p = self._minmax(t) if normalise else None
-        _lib.check(self.L.dm_boost_post(t.data_ptr(), t.numel(), p.data_ptr() if p is not None else None, int(normalise), out.data_ptr(),
-                                        _lib.stream_ptr()), "dm_boost_post")
-        self.launches += 1
+        self.ops.call("dm_boost_post", t, t.numel(), p, int(normalise), out)
         return out
 
     def _normalise_estimate(self, est):
@@ -427,9 +376,7 @@ class BoostPipeline:
         import torch
         out = torch.empty_like(est)
         p = self._minmax(est)
-        _lib.check(self.L.dm_boost_minmax_normalise(est.data_ptr(), est.numel(), p.data_ptr(), out.data_ptr(), self._degenerate.data_ptr(),
-                                                    _lib.stream_ptr()), "dm_boost_minmax_normalise")
-        self.launches += 1
+        self.ops.call("dm_boost_minmax_normalise", est, est.numel(), p, out, self._degenerate)
         return out
 
     def _estimate_1024(self, planar, rect, msize):
@@ -481,15 +428,12 @@ class BoostPipeline:
         base1024 = self._cubic(base.data_ptr() + 4 * (y * pitch + x), pitch, h, w, PIX2PIX_SIZE, PIX2PIX_SIZE)
         mapped = self._post(self._merge(base1024, est), False)
         sums = torch.empty(self.P * 4, dtype=torch.float64, device=self.device)
-        _lib.check(self.L.dm_boost_fit_sums(mapped.data_ptr(), base1024.data_ptr(), mapped.numel(), sums.data_ptr(), _lib.stream_ptr()), "dm_boost_fit_sums")
-        self.launches += 1
+        self.ops.call("dm_boost_fit_sums", mapped, base1024, mapped.numel(), sums)
         return mapped, sums
 
     def blend(self, updated, mapped, sums, rect):
         x, y, w, h = rect
-        _lib.check(self.L.dm_boost_blend(mapped.data_ptr(), PIX2PIX_SIZE, sums.data_ptr(), self.profile.data_ptr(), MASK_SIZE, updated.data_ptr(),
-                                         int(updated.shape[1]), x, y, w, h, _lib.stream_ptr()), "dm_boost_blend")
-        self.launches += 1
+        self.ops.call("dm_boost_blend", mapped, PIX2PIX_SIZE, sums, self.profile, MASK_SIZE, updated, int(updated.shape[1]), x, y, w, h)
 
     # -- the whole thing ----------------------------------------------------------------------------------------------
     def run(self, rgb_u8, whole_size_threshold, group=None, info=None, precomputed=None, to_host=True):
@@ -511,8 +455,7 @@ class BoostPipeline:
         rf = p["rf"]
         dev_rgb = torch.from_numpy(rgb_u8).to(self.device)
         img = torch.empty(3, H, W, dtype=torch.float32, device=self.device)
-        _lib.check(self.L.dm_boost_u8_to_planar(dev_rgb.data_ptr(), H, W, img.data_ptr(), _lib.stream_ptr()), "dm_boost_u8_to_planar")
-        self.launches += 1
+        self.ops.call("dm_boost_u8_to_planar", dev_rgb, H, W, img)
         whole = self.double_estimate(img, (0, 0, W, H), rf, p["whole"])
         a, b = p["target"]
         big = self._cubic(img.data_ptr(), W, H, W, a, b, planes=3, src_plane=H * W)

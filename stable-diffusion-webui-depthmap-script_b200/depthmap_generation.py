@@ -15,10 +15,10 @@ into the kernels' layout (fp16 GEMM operands, (ky,kx,cin)-ordered conv filters, 
 from __future__ import annotations
 
 import ctypes
+import functools
 import gc
 import math
 import os
-import sys
 
 import numpy as np
 
@@ -53,98 +53,6 @@ def dav2_net_size(width, height, target, multiple_of=14):
         sw = sh
     return (_constrain_to_multiple_of(sw * width, multiple_of, min_val=target),
             _constrain_to_multiple_of(sh * height, multiple_of, min_val=target))
-
-
-class _Ops:
-    """Thin typed wrappers over the C-ABI; every method is asynchronous on the current torch stream."""
-
-    def __init__(self):
-        self.L = _lib.load()
-        for name in ("dm_gemm_ex", "dm_conv3x3_ex", "dm_attention_f16", "dm_layernorm_f16"):
-            if not hasattr(self.L, name):
-                raise RuntimeError(f"depthmap_b200: native library lacks {name}; rebuild csrc (no fallback exists)")
-        self.launches = 0
-
-    def gemm(self, A, lda, W, ldw, M, N, K, epi=_lib.EPI_STORE_F16, act=_lib.ACT_NONE, bias=None, C=None, ldc=0, C2=None,
-             R=None, ldr=0, R2=None, ldr2=0, X=None, ldx=0, gamma=None, head_b2=0.0, ps=None):
-        d = _lib.GemmDesc()
-        d.M, d.N, d.K, d.epi, d.act = M, N, K, epi, act
-        d.bias = bias.data_ptr() if bias is not None else None
-        d.C = C.data_ptr() if C is not None else None
-        d.ldc = ldc
-        d.C2 = C2.data_ptr() if C2 is not None else None
-        d.R = R.data_ptr() if R is not None else None
-        d.ldr = ldr
-        d.R2 = R2.data_ptr() if R2 is not None else None
-        d.ldr2 = ldr2
-        d.X = X.data_ptr() if X is not None else None
-        d.ldx = ldx
-        d.gamma = gamma.data_ptr() if gamma is not None else None
-        d.head_b2 = head_b2
-        if ps is not None:
-            d.ps_s, d.ps_cout, d.ps_h, d.ps_w = ps
-        _lib.check(self.L.dm_gemm_ex(A.data_ptr(), lda, W.data_ptr(), ldw, ctypes.byref(d), _lib.stream_ptr()), "dm_gemm_ex")
-        self.launches += 1
-
-    def conv3x3(self, act_t, B, H, W_, Cin, Wt, Cout, epi=_lib.EPI_STORE_F16, act=_lib.ACT_NONE, bias=None, C=None, C2=None,
-                R=None, R2=None, X=None, gamma=None, head_b2=0.0, ldx=1):
-        d = _lib.GemmDesc()
-        d.N, d.epi, d.act = Cout, epi, act
-        d.bias = bias.data_ptr() if bias is not None else None
-        d.C = C.data_ptr() if C is not None else None
-        d.ldc = Cout
-        d.C2 = C2.data_ptr() if C2 is not None else None
-        d.R = R.data_ptr() if R is not None else None
-        d.ldr = Cout
-        d.R2 = R2.data_ptr() if R2 is not None else None
-        d.ldr2 = Cout
-        d.X = X.data_ptr() if X is not None else None
-        d.ldx = ldx
-        d.gamma = gamma.data_ptr() if gamma is not None else None
-        d.head_b2 = head_b2
-        _lib.check(self.L.dm_conv3x3_ex(act_t.data_ptr(), B, H, W_, Cin, Wt.data_ptr(), ctypes.byref(d), _lib.stream_ptr()), "dm_conv3x3_ex")
-        self.launches += 1
-
-    def attention(self, qkv, B, N, H, scale, out, bias=None, bias_ld=0):
-        _lib.check(self.L.dm_attention_f16(qkv.data_ptr(), B, N, H, float(scale), bias.data_ptr() if bias is not None else None,
-                                           bias_ld, out.data_ptr(), _lib.stream_ptr()), "dm_attention_f16")
-        self.launches += 1
-
-    def attention_relpos(self, qkv, B, gh, gw, H, scale, table, nrd, out):
-        _lib.check(self.L.dm_attention_relpos_f16(qkv.data_ptr(), B, gh, gw, H, float(scale), table.data_ptr(), nrd,
-                                                  out.data_ptr(), _lib.stream_ptr()), "dm_attention_relpos_f16")
-        self.launches += 1
-
-    def layernorm(self, x, rows, C, w, b, out, tokens_per_img=1, drop_first=0, eps=1e-6):
-        _lib.check(self.L.dm_layernorm_f16(x.data_ptr(), rows, C, w.data_ptr(), b.data_ptr(), eps, out.data_ptr(), tokens_per_img,
-                                           drop_first, _lib.stream_ptr()), "dm_layernorm_f16")
-        self.launches += 1
-
-    def patchify(self, rgb, B, H, W, nh, nw, patch, mean, std, cmap, out, kpad):
-        m = (ctypes.c_float * 3)(*mean)
-        s = (ctypes.c_float * 3)(*std)
-        c = (ctypes.c_int * 3)(*cmap)
-        _lib.check(self.L.dm_preprocess_patchify(rgb.data_ptr(), B, H, W, nh, nw, patch, m, s, c, out.data_ptr(), kpad, _lib.stream_ptr()),
-                   "dm_preprocess_patchify")
-        self.launches += 2 if kpad > 3 * patch * patch else 1
-
-    def tokens(self, pe, cls, pos, X, B, Np, C):
-        _lib.check(self.L.dm_assemble_tokens(pe.data_ptr(), cls.data_ptr(), pos.data_ptr() if pos is not None else None, X.data_ptr(),
-                                             B, Np, C, _lib.stream_ptr()), "dm_assemble_tokens")
-        self.launches += 1
-
-    def resize_nhwc(self, x, B, Hin, Win, C, out, Hout, Wout):
-        _lib.check(self.L.dm_resize_bilinear_nhwc_f16(x.data_ptr(), B, Hin, Win, C, out.data_ptr(), Hout, Wout, _lib.stream_ptr()),
-                   "dm_resize_bilinear_nhwc_f16")
-        self.launches += 1
-
-    def resize_f32(self, x, B, Hin, Win, out, Hout, Wout, mode):
-        _lib.check(self.L.dm_resize_f32(x.data_ptr(), B, Hin, Win, out.data_ptr(), Hout, Wout, mode, _lib.stream_ptr()), "dm_resize_f32")
-        self.launches += 1
-
-    def im2col_s2(self, x, B, H, W, C, out):
-        _lib.check(self.L.dm_im2col_s2_f16(x.data_ptr(), B, H, W, C, out.data_ptr(), _lib.stream_ptr()), "dm_im2col_s2_f16")
-        self.launches += 1
 
 
 def _conv_w(w, cin_pad, cout_pad):
@@ -185,11 +93,10 @@ class DepthAnythingV2Engine:
         self.cfg = self.CONFIGS[encoder]
         self.encoder = encoder
         self.device = device
-        self.ops = _Ops()
+        self.ops = _lib.Ops()
         self._buf_key = None
         self._bufs = {}
         self._pos_cache = {}
-        self.probe = None  # bench hook: {'fc1': (start_event, end_event)} records the block-0 fc1 GEMM launch
         self._pack(state_dict)
 
     # ---- weight packing --------------------------------------------------------------------------------------------
@@ -258,24 +165,23 @@ class DepthAnythingV2Engine:
         self.oc3_b = float(sd[h + 'scratch.output_conv2.2.bias'].detach().float().reshape(-1)[0])
         self.w = w
 
+    POS_EMBED = "dm_dinov2_pos_embed"    # interpolate_pos_encoding (dinov2.py:179-210); identity for the native 37x37 grid
+
     def _pos(self, gh, gw):
-        """interpolate_pos_encoding (dinov2.py:179-210); identity for the native 37x37 grid.  Setup-time, cached."""
+        """the position embedding resized to a gh x gw grid by the host routine POS_EMBED.  Setup-time, cached."""
         import torch
-        import torch.nn.functional as F
         key = (gh, gw)
-        if key in self._pos_cache:
-            return self._pos_cache[key]
-        pe = self._pos_embed
-        C = pe.shape[-1]
-        N = pe.shape[1] - 1
-        n = int(round(math.sqrt(N)))
-        # host arithmetic shared with the model-level C-ABI (csrc/model.cu), so both paths use bit-identical tables
-        src = np.ascontiguousarray(pe.reshape(N + 1, C).cpu().numpy(), dtype=np.float32)
-        dst = np.empty((gh * gw + 1, C), dtype=np.float32)
-        _lib.check(self.ops.L.dm_dinov2_pos_embed(src.ctypes.data, n, C, gh, gw, dst.ctypes.data), "dm_dinov2_pos_embed")
-        out = torch.from_numpy(dst).to(self.device)
-        self._pos_cache[key] = out
-        return out
+        if key not in self._pos_cache:
+            pe = self._pos_embed
+            C = pe.shape[-1]
+            N = pe.shape[1] - 1
+            n = int(round(math.sqrt(N)))
+            # host arithmetic shared with the model-level C-ABI (csrc/model.cu), so both paths use bit-identical tables
+            src = np.ascontiguousarray(pe.reshape(N + 1, C).cpu().numpy(), dtype=np.float32)
+            dst = np.empty((gh * gw + 1, C), dtype=np.float32)
+            _lib.check(getattr(self.ops.L, self.POS_EMBED)(src.ctypes.data, n, C, gh, gw, dst.ctypes.data), self.POS_EMBED)
+            self._pos_cache[key] = torch.from_numpy(dst).to(self.device)
+        return self._pos_cache[key]
 
     # ---- activation buffers ----------------------------------------------------------------------------------------
     def _buffers(self, B, nh, nw):
@@ -329,38 +235,22 @@ class DepthAnythingV2Engine:
         return dav2_net_size(W, H, net_w)  # estimatedepthanything_v2 passes w as input_size (:552)
 
     def attention(self, i, b, B, N, heads, C, gh, gw):
-        self.ops.attention(b['qkv'], B, N, heads, (C // heads) ** -0.5, b['att'])
-
-    def _probed_attention(self, i, b, B, N, heads, C, gh, gw):
-        """bench hook: probe['attn'] collects one (start, end) CUDA event pair per attention launch"""
-        if self.probe is not None and 'attn' in self.probe:
-            import torch
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            self.attention(i, b, B, N, heads, C, gh, gw)
-            e1.record()
-            self.probe['attn'].append((e0, e1))
-        else:
-            self.attention(i, b, B, N, heads, C, gh, gw)
+        self.ops.call("dm_attention_f16", b['qkv'], B, N, heads, (C // heads) ** -0.5, None, 0, b['att'])
 
     def emit_feature(self, b, fi, B, N, C):
         """get_intermediate_layers(norm=True) without the class token (dinov2.py:297-321)."""
-        self.ops.layernorm(b['x'], B * N, C, self.w['norm_w'], self.w['norm_b'], b['feat'][fi], tokens_per_img=N, drop_first=1)
+        self.ops.call("dm_layernorm_f16", b['x'], B * N, C, self.w['norm_w'], self.w['norm_b'], 1e-6, b['feat'][fi], N, 1)
 
     # ---- forward ---------------------------------------------------------------------------------------------------
     def forward_batch(self, rgb, net_w, net_h=None, out_hw=None):
         """rgb: uint8 CUDA [B,H,W,3] -> float32 CUDA [B,H,W] raw prediction (what the reference's estimate* returns)."""
-        import torch
-        ops, w, cfg = self.ops, self.w, self.cfg
         B, H, W, _ = rgb.shape
         nw, nh = self.net_size(W, H, net_w, net_h if net_h is not None else net_w)
-        C, heads, Fp = cfg['embed_dim'], cfg['heads'], self.Fp
         P_ = self.PATCH
-        gh, gw = nh // P_, nw // P_
-        Np, N = gh * gw, gh * gw + 1
         b = self._buffers(B, nh, nw)
-        # image2tensor
-        ops.patchify(rgb, B, H, W, nh, nw, P_, self.MEAN, self.STD, self.CHAN_MAP, b['patches'], self.kpad)
+        # image2tensor; the kernel zero-fills the patch matrix's K padding first, if it has any
+        self.ops.call("dm_preprocess_patchify", rgb, B, H, W, nh, nw, P_, (ctypes.c_float * 3)(*self.MEAN), (ctypes.c_float * 3)(*self.STD),
+                      (ctypes.c_int * 3)(*self.CHAN_MAP), b['patches'], self.kpad, launches=1 + (self.kpad > 3 * P_ * P_))
         self.run_network(b, B, nh, nw)
         return self.run_head(b, B, H, W, nh, nw, out_hw)
 
@@ -372,24 +262,19 @@ class DepthAnythingV2Engine:
         P_ = self.PATCH
         gh, gw = nh // P_, nw // P_
         Np, N = gh * gw, gh * gw + 1
-        E, A = _lib, _lib
         # patch embedding + tokens
         ops.gemm(b['patches'], self.kpad, w['pe_w'], self.kpad, B * Np, C, self.kpad, bias=w['pe_b'], C=b['pe'], ldc=C)
-        ops.tokens(b['pe'], w['cls'], self._pos(gh, gw) if self._pos_embed is not None else None, b['x'], B, Np, C)
+        ops.call("dm_assemble_tokens", b['pe'], w['cls'], self._pos(gh, gw) if self._pos_embed is not None else None, b['x'], B, Np, C)
         rows = B * N
         fi = 0
         for i, blk in enumerate(w['blocks']):
-            ops.layernorm(b['x'], rows, C, blk['ln1_w'], blk['ln1_b'], b['h'])
+            ops.call("dm_layernorm_f16", b['x'], rows, C, blk['ln1_w'], blk['ln1_b'], 1e-6, b['h'], 1, 0)
             ops.gemm(b['h'], C, blk['qkv_w'], C, rows, 3 * C, C, bias=blk['qkv_b'], C=b['qkv'], ldc=3 * C)
-            self._probed_attention(i, b, B, N, heads, C, gh, gw)
-            ops.gemm(b['att'], C, blk['proj_w'], C, rows, C, C, epi=E.EPI_RESID_F32, bias=blk['proj_b'], X=b['x'], ldx=C, gamma=blk['ls1'])
-            ops.layernorm(b['x'], rows, C, blk['ln2_w'], blk['ln2_b'], b['h'])
-            if self.probe is not None and 'fc1' in self.probe and i == 0:
-                self.probe['fc1'][0].record()
-            ops.gemm(b['h'], C, blk['fc1_w'], C, rows, 4 * C, C, act=A.ACT_GELU, bias=blk['fc1_b'], C=b['mlp'], ldc=4 * C)
-            if self.probe is not None and 'fc1' in self.probe and i == 0:
-                self.probe['fc1'][1].record()
-            ops.gemm(b['mlp'], 4 * C, blk['fc2_w'], 4 * C, rows, C, 4 * C, epi=E.EPI_RESID_F32, bias=blk['fc2_b'], X=b['x'], ldx=C, gamma=blk['ls2'])
+            self.attention(i, b, B, N, heads, C, gh, gw)
+            ops.gemm(b['att'], C, blk['proj_w'], C, rows, C, C, epi=_lib.EPI_RESID_F32, bias=blk['proj_b'], X=b['x'], ldx=C, gamma=blk['ls1'])
+            ops.call("dm_layernorm_f16", b['x'], rows, C, blk['ln2_w'], blk['ln2_b'], 1e-6, b['h'], 1, 0)
+            ops.gemm(b['h'], C, blk['fc1_w'], C, rows, 4 * C, C, act=_lib.ACT_GELU, bias=blk['fc1_b'], C=b['mlp'], ldc=4 * C)
+            ops.gemm(b['mlp'], 4 * C, blk['fc2_w'], 4 * C, rows, C, 4 * C, epi=_lib.EPI_RESID_F32, bias=blk['fc2_b'], X=b['x'], ldx=C, gamma=blk['ls2'])
             if i in cfg['layers']:
                 self.emit_feature(b, fi, B, N, C)
                 fi += 1
@@ -397,12 +282,12 @@ class DepthAnythingV2Engine:
         sizes = b['sizes']
         for i in range(4):
             ops.gemm(b['feat'][i], C, w[f'proj{i}_w'], C, B * Np, self.ocp[i], C, bias=w[f'proj{i}_b'], C=b['p'][i], ldc=self.ocp[i])
-        ops.gemm(b['p'][0], self.ocp[0], w['up0_w'], self.ocp[0], B * Np, 16 * self.ocp[0], self.ocp[0], epi=E.EPI_PIXSHUF, bias=w['up0_b'],
+        ops.gemm(b['p'][0], self.ocp[0], w['up0_w'], self.ocp[0], B * Np, 16 * self.ocp[0], self.ocp[0], epi=_lib.EPI_PIXSHUF, bias=w['up0_b'],
                  C=b['r'][0], ps=(4, self.ocp[0], gh, gw))
-        ops.gemm(b['p'][1], self.ocp[1], w['up1_w'], self.ocp[1], B * Np, 4 * self.ocp[1], self.ocp[1], epi=E.EPI_PIXSHUF, bias=w['up1_b'],
+        ops.gemm(b['p'][1], self.ocp[1], w['up1_w'], self.ocp[1], B * Np, 4 * self.ocp[1], self.ocp[1], epi=_lib.EPI_PIXSHUF, bias=w['up1_b'],
                  C=b['r'][1], ps=(2, self.ocp[1], gh, gw))
         r2 = b['p'][2]
-        ops.im2col_s2(b['p'][3], B, gh, gw, self.ocp[3], b['cols3'])
+        ops.call("dm_im2col_s2_f16", b['p'][3], B, gh, gw, self.ocp[3], b['cols3'])
         ops.gemm(b['cols3'], 9 * self.ocp[3], w['down3_w'], 9 * self.ocp[3], B * sizes[3][0] * sizes[3][1], self.ocp[3], 9 * self.ocp[3],
                  bias=w['down3_b'], C=b['r'][3], ldc=self.ocp[3])
         rs = [b['r'][0], b['r'][1], r2, b['r'][3]]
@@ -412,23 +297,23 @@ class DepthAnythingV2Engine:
         # interpolation (a per-pixel channel mix against per-channel spatial weights that sum to one), so it runs BEFORE the
         # up-sample: a quarter of the MACs and no full-resolution intermediate (dmidas/blocks.py:425-437 has it after).
         s3 = sizes[3]
-        ops.conv3x3(b['lr'][3], B, s3[0], s3[1], Fp, w['rf4_u2c1_w'], Fp, act=A.ACT_RELU, bias=w['rf4_u2c1_b'], C=b['t3'])
+        ops.conv3x3(b['lr'][3], B, s3[0], s3[1], Fp, w['rf4_u2c1_w'], Fp, act=_lib.ACT_RELU, bias=w['rf4_u2c1_b'], C=b['t3'])
         ops.conv3x3(b['t3'], B, s3[0], s3[1], Fp, w['rf4_u2c2_w'], Fp, bias=w['rf4_u2c2_b'], C=b['u3'], R=b['l'][3])
         up = b['up_sizes']
         ops.gemm(b['u3'], Fp, w['rf4_out_w'], Fp, B * s3[0] * s3[1], Fp, Fp, bias=w['rf4_out_b'], C=b['v'][0], ldc=Fp)
-        ops.resize_nhwc(b['v'][0], B, s3[0], s3[1], Fp, b['path'][0], up[0][0], up[0][1])
+        ops.call("dm_resize_bilinear_nhwc_f16", b['v'][0], B, s3[0], s3[1], Fp, b['path'][0], up[0][0], up[0][1])
         # refinenet3, 2, 1: output = path + RCU1(l_i); output = RCU2(output); out_conv; resize (commuted, see above)
         for step, (li, rf) in enumerate(((2, 3), (1, 2), (0, 1))):
             s = sizes[li]
             path = b['path'][step]
-            ops.conv3x3(b['lr'][li], B, s[0], s[1], Fp, w[f'rf{rf}_u1c1_w'], Fp, act=A.ACT_RELU, bias=w[f'rf{rf}_u1c1_b'], C=b[f't{li}'])
+            ops.conv3x3(b['lr'][li], B, s[0], s[1], Fp, w[f'rf{rf}_u1c1_w'], Fp, act=_lib.ACT_RELU, bias=w[f'rf{rf}_u1c1_b'], C=b[f't{li}'])
             ops.conv3x3(b[f't{li}'], B, s[0], s[1], Fp, w[f'rf{rf}_u1c2_w'], Fp, bias=w[f'rf{rf}_u1c2_b'], C=b[f'o{li}'], C2=b[f'or{li}'],
                         R=b['l'][li], R2=path)
-            ops.conv3x3(b[f'or{li}'], B, s[0], s[1], Fp, w[f'rf{rf}_u2c1_w'], Fp, act=A.ACT_RELU, bias=w[f'rf{rf}_u2c1_b'], C=b[f't{li}'])
+            ops.conv3x3(b[f'or{li}'], B, s[0], s[1], Fp, w[f'rf{rf}_u2c1_w'], Fp, act=_lib.ACT_RELU, bias=w[f'rf{rf}_u2c1_b'], C=b[f't{li}'])
             ops.conv3x3(b[f't{li}'], B, s[0], s[1], Fp, w[f'rf{rf}_u2c2_w'], Fp, bias=w[f'rf{rf}_u2c2_b'], C=b[f'u{li}'], R=b[f'o{li}'])
             t = up[step + 1]
             ops.gemm(b[f'u{li}'], Fp, w[f'rf{rf}_out_w'], Fp, B * s[0] * s[1], Fp, Fp, bias=w[f'rf{rf}_out_b'], C=b['v'][step + 1], ldc=Fp)
-            ops.resize_nhwc(b['v'][step + 1], B, s[0], s[1], Fp, b['path'][step + 1], t[0], t[1])
+            ops.call("dm_resize_bilinear_nhwc_f16", b['v'][step + 1], B, s[0], s[1], Fp, b['path'][step + 1], t[0], t[1])
 
     def run_head(self, b, B, H, W, nh, nw, out_hw=None, resize=True):
         """output_conv (dpt.py:139-150 / dpt_depth.py:150-158) + the final resize to the image size.  resize=False returns the
@@ -436,18 +321,17 @@ class DepthAnythingV2Engine:
         import torch
         ops, w = self.ops, self.w
         Fp = self.Fp
-        E, A = _lib, _lib
         t = b['up_sizes'][3]
         ops.conv3x3(b['path'][3], B, t[0], t[1], Fp, w['oc1_w'], self.F2p, bias=w['oc1_b'], C=b['oc1'])
-        ops.resize_nhwc(b['oc1'], B, t[0], t[1], self.F2p, b['oc1u'], nh, nw)
+        ops.call("dm_resize_bilinear_nhwc_f16", b['oc1'], B, t[0], t[1], self.F2p, b['oc1u'], nh, nw)
         # conv3x3 -> ReLU -> conv1x1 -> ReLU (+ the outer F.relu, idempotent) fused into one epilogue
-        ops.conv3x3(b['oc1u'], B, nh, nw, self.F2p, w['oc2_w'], 32, epi=E.EPI_HEAD, act=A.ACT_RELU, bias=w['oc2_b'], X=b['d'], gamma=w['oc3_w'],
-                    head_b2=self.oc3_b)
+        ops.conv3x3(b['oc1u'], B, nh, nw, self.F2p, w['oc2_w'], 32, epi=_lib.EPI_HEAD, act=_lib.ACT_RELU, bias=w['oc2_b'], X=b['d'],
+                    gamma=w['oc3_w'], head_b2=self.oc3_b)
         if not resize:
             return b['d']
         oh, ow = out_hw if out_hw is not None else (H, W)
         out = torch.empty(B, oh, ow, dtype=torch.float32, device=self.device)
-        ops.resize_f32(b['d'], B, nh, nw, out, oh, ow, self.FINAL_RESIZE_MODE)
+        ops.call("dm_resize_f32", b['d'], B, nh, nw, out, oh, ow, self.FINAL_RESIZE_MODE)
         return out
 
     def to(self, device):
@@ -588,7 +472,7 @@ class DptBeitEngine(DepthAnythingV2Engine):
 
     def attention(self, i, b, B, N, heads, C, gh, gw):
         tabs, nrd = self.rel_tables(gh, gw)
-        self.ops.attention_relpos(b['qkv'], B, gh, gw, heads, (C // heads) ** -0.5, tabs[i], nrd, b['att'])
+        self.ops.call("dm_attention_relpos_f16", b['qkv'], B, gh, gw, heads, (C // heads) ** -0.5, tabs[i], nrd, b['att'])
 
     # ---- BOOST: estimatemidasBoost on float crops ---------------------------------------------------------------------
     BOOST_MEAN = (0.485, 0.456, 0.406)
@@ -607,7 +491,6 @@ class DptBeitEngine(DepthAnythingV2Engine):
         upper-bound net size for msize, then cv2-cubic back to the crop.  Crops clipped at the image border are not square, so the
         crops are grouped by net shape, one batched forward per shape."""
         import torch
-        L, st = self.ops.L, _lib.stream_ptr
         hi, wi = int(planar.shape[1]), int(planar.shape[2])
         if planar.dtype != torch.float32 or planar.dim() != 3 or planar.shape[0] != 3 or not planar.is_contiguous():
             raise ValueError("planar must be a contiguous float32 tensor [3, H, W]")
@@ -625,24 +508,21 @@ class DptBeitEngine(DepthAnythingV2Engine):
             B = len(ks)
             r = torch.tensor([[int(v) for v in rects[k]] for k in ks], dtype=torch.int32).to(self.device)
             b = self._buffers(B, nh, nw)
-            _lib.check(L.dm_preprocess_patchify_f32_crops(planar.data_ptr(), hi, wi, r.data_ptr(), B, nh, nw, self.PATCH, m, sd, cm,
-                                                           b['patches'].data_ptr(), self.kpad, st()), "dm_preprocess_patchify_f32_crops")
-            self.ops.launches += 1
+            self.ops.call("dm_preprocess_patchify_f32_crops", planar, hi, wi, r, B, nh, nw, self.PATCH, m, sd, cm, b['patches'], self.kpad,
+                          launches=1 + (self.kpad > 3 * self.PATCH ** 2))
             self.run_network(b, B, nh, nw)
             d = self.run_head(b, B, nh, nw, nh, nw, resize=False)
             for i, k in enumerate(ks):
                 w, h = int(rects[k][2]), int(rects[k][3])
                 o = torch.empty(h, w, dtype=torch.float32, device=self.device)
-                _lib.check(L.dm_boost_resize_cubic(d[i].data_ptr(), nw, 0, nh, nw, o.data_ptr(), w, 0, h, w, 1, st()), "dm_boost_resize_cubic")
-                self.ops.launches += 1
+                self.ops.call("dm_boost_resize_cubic", d[i], nw, 0, nh, nw, o, w, 0, h, w, 1)
                 out[k] = o
         return out
 
     def emit_feature(self, b, fi, B, N, C):
         """forward hook on the raw block output + ProjectReadout: GELU(Linear(cat(tokens, cls)))."""
         rw, rb = self.w['readout'][fi]
-        _lib.check(self.ops.L.dm_concat_readout_f16(b['x'].data_ptr(), B, N, C, b['cat'].data_ptr(), _lib.stream_ptr()), "dm_concat_readout_f16")
-        self.ops.launches += 1
+        self.ops.call("dm_concat_readout_f16", b['x'], B, N, C, b['cat'])
         self.ops.gemm(b['cat'], 2 * C, rw, 2 * C, B * (N - 1), C, 2 * C, act=_lib.ACT_GELU, bias=rb, C=b['feat'][fi], ldc=C)
 
 
@@ -675,23 +555,8 @@ class DptVitEngine(DptBeitEngine):
             blk['qkv_b'] = sd[p + f'blocks.{i}.attn.qkv.bias'].detach().to(self.device, torch.float32).contiguous()
         self._pos_embed = sd[p + 'pos_embed'].detach().to(self.device, torch.float32).contiguous()
 
-    def _pos(self, gh, gw):
-        """_resize_pos_embed (vit.py:16-31) through the host routine the model-level C-ABI uses (bit-identical tables)."""
-        import torch
-        key = (gh, gw)
-        if key not in self._pos_cache:
-            pe = self._pos_embed
-            C = pe.shape[-1]
-            N = pe.shape[1] - 1
-            n = int(round(math.sqrt(N)))
-            src = np.ascontiguousarray(pe.reshape(N + 1, C).cpu().numpy(), dtype=np.float32)
-            dst = np.empty((gh * gw + 1, C), dtype=np.float32)
-            _lib.check(self.ops.L.dm_vit_pos_embed(src.ctypes.data, n, C, gh, gw, dst.ctypes.data), "dm_vit_pos_embed")
-            self._pos_cache[key] = torch.from_numpy(dst).to(self.device)
-        return self._pos_cache[key]
-
-    def attention(self, i, b, B, N, heads, C, gh, gw):
-        self.ops.attention(b['qkv'], B, N, heads, (C // heads) ** -0.5, b['att'])
+    POS_EMBED = "dm_vit_pos_embed"      # _resize_pos_embed (vit.py:16-31)
+    attention = DepthAnythingV2Engine.attention     # plain attention, no relative-position bias
 
 
 class LeresEngine:
@@ -711,11 +576,11 @@ class LeresEngine:
 
     def __init__(self, state_dict, device):
         self.device = device
-        self.ops = _Ops()
-        self._bufs, self._buf_key = {}, None
-        self._graphs, self._graph_calls = {}, {}
+        self.ops = _lib.Ops()
+        self._bufs = {}
+        # from the second call on at a given (B, net size) the ~500 launches of the network replay from a CUDA graph
+        self._graphs = _lib.GraphCache(self.ops, "DEPTHMAP_B200_LERES_GRAPH", "LeReS")
         self._pooled_bytes, self._pool_limit = 0, None
-        self._use_graph = os.environ.get("DEPTHMAP_B200_LERES_GRAPH", "1") != "0"
         self._pack(state_dict)
 
     # ---- weights -------------------------------------------------------------------------------------------------------
@@ -810,48 +675,20 @@ class LeresEngine:
         if self._pooled_bytes > self._pool_limit and not torch.cuda.is_current_stream_capturing():
             torch.cuda.synchronize(self.device)
             self._graphs.clear()
-            self._graph_calls.clear()
             self._bufs.clear()
             self._pooled_bytes = 0
             torch.cuda.empty_cache()
 
     # ---- forward ---------------------------------------------------------------------------------------------------
     def _network(self, B, net_h, net_w, cols):
-        """stem GEMM .. decoder output [B, net_h, net_w] fp32 (a pooled buffer).  From the second call on at a given (B, net size) the
-        ~500 launches replay from a CUDA graph (DEPTHMAP_B200_LERES_GRAPH=0: eager)."""
-        import torch
-        key = (B, net_h, net_w)
-        capturing = torch.cuda.is_current_stream_capturing()       # inside somebody else's capture: plain launches
-        g = self._graphs.get(key)
-        if g is not None and not capturing:
-            g[0].replay()
-            self.ops.launches += g[2]                                # the kernels inside the graph still launch
-            return g[1]
-        n = self._graph_calls.get(key, 0) + 1
-        self._graph_calls[key] = n
-        if self._use_graph and g is None and n >= 2 and not capturing:
-            try:
-                graph = torch.cuda.CUDAGraph()
-                n0 = self.ops.launches
-                with torch.cuda.graph(graph):
-                    dn = self._network_eager(B, net_h, net_w, cols)
-                self._graphs[key] = (graph, dn, self.ops.launches - n0)
-                graph.replay()
-                return dn
-            except Exception as e:  # noqa: BLE001 — an optimisation only: same kernels eagerly
-                sys.stderr.write(f"[depthmap_b200] LeReS graph capture failed ({e}); running eagerly\n")
-                torch.cuda.synchronize()
-                self._use_graph = False
-        return self._network_eager(B, net_h, net_w, cols)
+        """stem GEMM .. decoder output [B, net_h, net_w] fp32 (a pooled buffer)"""
+        return self._graphs.run((B, net_h, net_w), lambda: self._network_eager(B, net_h, net_w, cols))
 
     def forward_batch(self, rgb, net_w, net_h=None, out_hw=None, planar=None):
         """rgb: uint8 CUDA [B,H,W,3] -> float32 CUDA [B,H,W] (what estimateleres returns; invert = True).
         planar = (fp32 CUDA [3,Hi,Wi] image in network channel order, (x0, y0, w, h)) instead of `rgb`: estimateleres on a float
         crop, as BOOST calls it (src/depthmap_generation.py:1053-1056) — one image, result [1, h, w]."""
         import torch
-        ops, w, L = self.ops, self.w, self.ops.L
-        st = _lib.stream_ptr
-        A = _lib
         if planar is None:
             B, H, W, _ = rgb.shape
         else:
@@ -868,10 +705,9 @@ class LeresEngine:
         m = (ctypes.c_float * 3)(*self.MEAN)
         s = (ctypes.c_float * 3)(*self.STD)
         if planar is None:
-            _lib.check(L.dm_leres_stem_im2col(rgb.data_ptr(), B, H, W, net_h, net_w, m, s, cols.data_ptr(), st()), "dm_leres_stem_im2col")
+            self.ops.call("dm_leres_stem_im2col", rgb, B, H, W, net_h, net_w, m, s, cols)
         else:
-            _lib.check(L.dm_leres_stem_im2col_f32(pl_img.data_ptr(), pl_hi, pl_wi, rect[0], rect[1], rect[2], rect[3], net_h, net_w, m, s, cols.data_ptr(),
-                                                  st()), "dm_leres_stem_im2col_f32")
+            self.ops.call("dm_leres_stem_im2col_f32", pl_img, pl_hi, pl_wi, rect[0], rect[1], rect[2], rect[3], net_h, net_w, m, s, cols)
         dn = self._network(B, net_h, net_w, cols)
         hh, ww = net_h // 2, net_w // 2
         oh, ow = out_hw if out_hw is not None else (H, W)
@@ -879,8 +715,7 @@ class LeresEngine:
         if (oh, ow) == (2 * hh, 2 * ww):
             out.copy_(dn)                                      # cv2.resize to the same size is a copy
         else:
-            ops.resize_f32(dn, B, 2 * hh, 2 * ww, out, oh, ow, 1)   # cv2.INTER_CUBIC (A = -0.75, replicated borders)
-        ops.launches += 1
+            self.ops.call("dm_resize_f32", dn, B, 2 * hh, 2 * ww, out, oh, ow, 1)   # cv2.INTER_CUBIC (A = -0.75, replicated borders)
         return out
 
     def forward_crops(self, planar, rects, net):
@@ -901,23 +736,18 @@ class LeresEngine:
         cols = self._buf('stem_cols', (B * h1 * h1, 192))
         m = (ctypes.c_float * 3)(*self.MEAN)
         sdev = (ctypes.c_float * 3)(*self.STD)
-        _lib.check(self.ops.L.dm_leres_stem_im2col_f32_batch(planar.data_ptr(), hi, wi, r.data_ptr(), B, net, net, m, sdev, cols.data_ptr(), _lib.stream_ptr()),
-                   "dm_leres_stem_im2col_f32_batch")
-        self.ops.launches += 1
+        self.ops.call("dm_leres_stem_im2col_f32_batch", planar, hi, wi, r, B, net, net, m, sdev, cols)
         return self._network(B, net, net, cols)
 
     def _network_eager(self, B, net_h, net_w, cols):
         import torch
-        ops, w, L = self.ops, self.w, self.ops.L
-        st = _lib.stream_ptr
-        A = _lib
+        ops, w = self.ops, self.w
         h1, w1 = (net_h + 6 - 7) // 2 + 1, (net_w + 6 - 7) // 2 + 1
         x = self._buf('stem', (B, h1, w1, 64))
-        ops.gemm(cols, 192, w['stem'][0], 192, B * h1 * w1, 64, 192, act=A.ACT_RELU, bias=w['stem'][1], C=x, ldc=64)
+        ops.gemm(cols, 192, w['stem'][0], 192, B * h1 * w1, 64, 192, act=_lib.ACT_RELU, bias=w['stem'][1], C=x, ldc=64)
         h, wd = (h1 + 2 - 3) // 2 + 1, (w1 + 2 - 3) // 2 + 1
         xp = self._buf('pool', (B, h, wd, 64))
-        _lib.check(L.dm_maxpool3x3s2_nhwc_f16(x.data_ptr(), B, h1, w1, 64, xp.data_ptr(), st()), "dm_maxpool3x3s2_nhwc_f16")
-        ops.launches += 2
+        ops.call("dm_maxpool3x3s2_nhwc_f16", x, B, h1, w1, 64, xp)
         x, cin = xp, 64
         feats = []
         bi_global = 0
@@ -928,24 +758,23 @@ class LeresEngine:
                 width, cout, stride = blk['width'], blk['cout'], blk['stride']
                 M = B * h * wd
                 t1 = self._buf(tag + '_t1', (B, h, wd, width))
-                ops.gemm(x, cin, blk['c1'][0], cin, M, width, cin, act=A.ACT_RELU, bias=blk['c1'][1], C=t1, ldc=width)
+                ops.gemm(x, cin, blk['c1'][0], cin, M, width, cin, act=_lib.ACT_RELU, bias=blk['c1'][1], C=t1, ldc=width)
                 if stride == 1:
                     ho, wo = h, wd
                     t2 = self._buf(tag + '_t2', (B, ho, wo, width))
-                    ops.conv3x3(t1, B, h, wd, width, blk['c2'][0], width, act=A.ACT_RELU, bias=blk['c2'][1], C=t2)
+                    ops.conv3x3(t1, B, h, wd, width, blk['c2'][0], width, act=_lib.ACT_RELU, bias=blk['c2'][1], C=t2)
                 else:
                     ho, wo = (h + 2 - 3) // 2 + 1, (wd + 2 - 3) // 2 + 1
                     c2 = self._buf(tag + '_cols', (B * ho * wo, 9 * width))
-                    ops.im2col_s2(t1, B, h, wd, width, c2)
+                    ops.call("dm_im2col_s2_f16", t1, B, h, wd, width, c2)
                     t2 = self._buf(tag + '_t2', (B, ho, wo, width))
-                    ops.gemm(c2, 9 * width, blk['c2'][0], 9 * width, B * ho * wo, width, 9 * width, act=A.ACT_RELU, bias=blk['c2'][1], C=t2, ldc=width)
+                    ops.gemm(c2, 9 * width, blk['c2'][0], 9 * width, B * ho * wo, width, 9 * width, act=_lib.ACT_RELU, bias=blk['c2'][1], C=t2, ldc=width)
                 Mo = B * ho * wo
                 if blk['down'] is not None:
                     xs = x
                     if stride == 2:
                         xs = self._buf(tag + '_xs', (B, ho, wo, cin))
-                        _lib.check(L.dm_subsample2_nhwc_f16(x.data_ptr(), B, h, wd, cin, xs.data_ptr(), st()), "dm_subsample2_nhwc_f16")
-                        ops.launches += 1
+                        ops.call("dm_subsample2_nhwc_f16", x, B, h, wd, cin, xs)
                     idn = self._buf(tag + '_idn', (B, ho, wo, cout))
                     ops.gemm(xs, cin, blk['down'][0], cin, Mo, cout, cin, bias=blk['down'][1], C=idn, ldc=cout)
                 else:
@@ -958,20 +787,20 @@ class LeresEngine:
                 bi_global += 1
             feats.append((x, h, wd, cin))
 
-        def conv(name, xin, hh, ww, ci, wb, co, act=A.ACT_NONE, R=None, C2=False):
+        def conv(name, xin, hh, ww, ci, wb, co, act=_lib.ACT_NONE, R=None, C2=False):
             outp = self._buf(name, (B, hh, ww, co))
             out2 = self._buf(name + '_r', (B, hh, ww, co)) if C2 else None
             ops.conv3x3(xin, B, hh, ww, ci, wb[0], co, act=act, bias=wb[1], C=outp, C2=out2, R=R)
             return out2 if C2 else outp
 
         def ftb(name, xin, hh, ww, ci, f, cm):
-            x1 = conv(name + '_x1', xin, hh, ww, ci, f['c1'], cm, act=A.ACT_RELU)           # the in-place ReLU also rewrites the skip operand
-            b1 = conv(name + '_b1', x1, hh, ww, cm, f['b1'], cm, act=A.ACT_RELU)
+            x1 = conv(name + '_x1', xin, hh, ww, ci, f['c1'], cm, act=_lib.ACT_RELU)           # the in-place ReLU also rewrites the skip operand
+            b1 = conv(name + '_b1', x1, hh, ww, cm, f['b1'], cm, act=_lib.ACT_RELU)
             return conv(name + '_o', b1, hh, ww, cm, f['b4'], cm, R=x1, C2=True)             # relu(x1 + branch)
 
         def up2(name, xin, hh, ww, c):
             outp = self._buf(name, (B, 2 * hh, 2 * ww, c))
-            ops.resize_nhwc(xin, B, hh, ww, c, outp, 2 * hh, 2 * ww)
+            ops.call("dm_resize_bilinear_nhwc_f16", xin, B, hh, ww, c, outp, 2 * hh, 2 * ww)
             return outp
 
         f3, h3, w3, c3 = feats[3]
@@ -984,17 +813,15 @@ class LeresEngine:
             assert (hl, wl) == (hh, ww)
             a1 = ftb(k + 'a', low, hl, wl, cl, w[k][0], 256)
             sm = self._buf(k + '_sum', (B, hl, wl, 256))
-            _lib.check(L.dm_add_f16(a1.data_ptr(), x.data_ptr(), sm.data_ptr(), sm.numel(), st()), "dm_add_f16")
-            ops.launches += 1
+            ops.call("dm_add_f16", a1, x, sm, sm.numel())
             x = ftb(k + 'b', sm, hl, wl, 256, w[k][1], 256)
             x = up2(k + '_up', x, hl, wl, 256)
             hh, ww = 2 * hl, 2 * wl
-        x = conv('ao0', x, hh, ww, 256, w['ao0'], 128, act=A.ACT_RELU)
+        x = conv('ao0', x, hh, ww, 256, w['ao0'], 128, act=_lib.ACT_RELU)
         d32 = self._buf('ao3', (B * hh * ww, 32), torch.float32)
-        ops.conv3x3(x, B, hh, ww, 128, w['ao3'][0], 32, epi=A.EPI_STORE_F32, bias=w['ao3'][1], X=d32, ldx=32)
+        ops.conv3x3(x, B, hh, ww, 128, w['ao3'][0], 32, epi=_lib.EPI_STORE_F32, bias=w['ao3'][1], X=d32, ldx=32)
         dn = self._buf('dnet', (B, 2 * hh, 2 * ww), torch.float32)
-        _lib.check(L.dm_resize_f32_ld(d32.data_ptr(), 32, B, hh, ww, dn.data_ptr(), 2 * hh, 2 * ww, 0, st()), "dm_resize_f32_ld")
-        ops.launches += 1
+        ops.call("dm_resize_f32_ld", d32, 32, B, hh, ww, dn, 2 * hh, 2 * ww, 0)
         assert (2 * hh, 2 * ww) == (net_h, net_w)
         return dn
 
@@ -1086,55 +913,163 @@ class NativeDepthModel:
 ZOE_CONFIG = dict(n_bins=64, emb=128, min_temp=0.0212, max_temp=50.0, router_dim=128, router_heads=4, router_layers=4)
 
 
-class ZoeDepthNKEngine(DptBeitEngine):
-    """ZoeDepth-NK (model types 7-9 share this head family; 9 = zoedepth_nk) on the sm_90a kernels: DepthModel.infer_pil
-    (pad + flip test-time augmentation, dzoedepth/models/depth_model.py:57-152), PrepForMidas (base_models/midas.py:175-186),
-    the DPT-BEiT-L-384 core with MidasCore's hooks (midas.py:258-319) and the metric head of ZoeDepthNK.forward
-    (zoedepth_nk/zoedepth_nk_v1.py:159-243).  Image b and its horizontal flip run as forwards 2b / 2b+1 of ONE batch; the
-    router picks nyu / kitti per forward on the device (argmax of two logits, no host sync, no cross-image vote).
-    Checkpoint layout: MiDaS weights under "core.core.", head weights at the top level."""
+def _zoe_w(sd, dev, key, rows=None):
+    """1x1 conv / linear weight -> fp16 [rows, cin] (zero padded rows)"""
+    import torch
+    t = sd[key + '.weight'].detach().to(dev).float()
+    t = t.reshape(t.shape[0], -1)
+    o = torch.zeros(rows or t.shape[0], t.shape[1], dtype=torch.float16, device=dev)
+    o[:t.shape[0]] = t.to(torch.float16)
+    return o
+
+
+def _zoe_b(sd, dev, key, n=None):
+    """bias -> fp32 [n] (zero padded)"""
+    import torch
+    t = sd[key + '.bias'].detach().to(dev).float().reshape(-1)
+    o = torch.zeros(n or t.numel(), dtype=torch.float32, device=dev)
+    o[:t.numel()] = t
+    return o
+
+
+def _zoe_lin(sd, dev, key, rows=None):
+    """(weight, bias) of one 1x1 conv / linear layer, output rows zero padded to `rows`"""
+    return _zoe_w(sd, dev, key, rows), _zoe_b(sd, dev, key, rows)
+
+
+def _zoe_mlp(sd, dev, key):
+    """the two layers of a ZoeDepth MLP block (key._net.0, key._net.2)"""
+    return _zoe_lin(sd, dev, key + '._net.0'), _zoe_lin(sd, dev, key + '._net.2')
+
+
+class _ZoeDepthBase(DptBeitEngine):
+    """What ZoeDepth-NK and ZoeDepth-N / -K share on the sm_90a kernels: DepthModel.infer_pil's pad + flip test-time augmentation
+    (dzoedepth/models/depth_model.py:57-152; image b and its horizontal flip run as forwards 2b / 2b+1 of ONE batch), PrepForMidas
+    (base_models/midas.py:175-186), the DPT-BEiT-L-384 core with MidasCore's hooks (midas.py:258-319), the seed projector, the
+    attractor levels (projector -> resize-add of the previous bin embedding -> attractor MLP -> attractor kernel) and the
+    log-binomial's bin-embedding GEMM.  Subclasses supply the seed bins, the attractor kernel, the log-binomial kernel and the
+    layer widths below.  Checkpoint layout: MiDaS weights under "core.core.", head weights at the top level."""
+
+    PROJ = ATT_HID = ATT_OUT = None     # hidden width of the projectors, of the attractor MLPs, and the attractor MLPs' output
 
     def __init__(self, state_dict, device, core_name='beitl16_384'):
         core_sd = {k[len("core.core."):]: v for k, v in state_dict.items() if k.startswith("core.core.")}
-        self._head_sd = {k: v for k, v in state_dict.items() if not k.startswith("core.")}
         super().__init__(core_sd, core_name, device)
-        self._pack_head(self._head_sd)
+        self._pack_head({k: v for k, v in state_dict.items() if not k.startswith("core.")})
+        # output_conv.2, whose 32-channel ReLU output MidasCore hooks, stored as its own activation
+        self.z['oc2_w'] = _conv_w(self._oc2_weight.to(device), self.F2p, 32)
+        self.z['oc2_b'] = self._oc2_bias.to(device).float().contiguous()
         self._zbuf_key, self._zbufs = None, {}
+
+    def _pack(self, sd):
+        self._oc2_weight = sd['scratch.output_conv.2.weight'].detach()
+        self._oc2_bias = sd['scratch.output_conv.2.bias'].detach()
+        super()._pack(sd)
+
+    def _zbuffers(self, F, nh, nw, b):
+        import torch
+        key = (F, nh, nw)
+        if self._zbuf_key == key:
+            return self._zbufs
+        dev = self.device
+        h16 = lambda *s: torch.empty(*s, dtype=torch.float16, device=dev)
+        f32 = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
+        s3 = b['sizes'][3]
+        n0 = s3[0] * s3[1]
+        levels = list(b['up_sizes'])                       # (h, w) of refinenet4..1 outputs
+        zb = dict(x16=h16(F * n0, self.Fp), bprev=f32(F * n0, 64), p0=h16(F * n0, self.PROJ), pemb=h16(F * n0, 128), n0=n0, levels=levels)
+        zb['t'] = [h16(F * h * w, self.PROJ) for h, w in levels]
+        zb['bemb'] = [h16(F * h * w, 128) for h, w in levels]
+        zb['xin'] = [h16(F * h * w, 128) for h, w in levels]
+        zb['a0'] = [h16(F * h * w, self.ATT_HID) for h, w in levels]
+        zb['A'] = [f32(F * h * w, self.ATT_OUT) for h, w in levels]
+        zb['bnew'] = [f32(F * h * w, 64) for h, w in levels]
+        zb['ze'] = f32(F * levels[3][0] * levels[3][1], 128)
+        zb['o32'] = h16(F, nh, nw, 32)
+        zb['d'] = f32(F, nh, nw)
+        zb.update(self._seed_buffers(F, n0, h16, f32))
+        self._zbufs, self._zbuf_key = zb, key
+        return zb
+
+    def lin(self, a, lda, wb, M, N, K, out=None, act=_lib.ACT_NONE, f32out=None, resid=None):
+        """a [M, K] (row pitch lda) times a (weight, bias) pair -> fp16 `out`, fp32 `f32out`, or added into the fp32 stream `resid`"""
+        wt, bias = wb
+        if resid is not None:
+            self.ops.gemm(a, lda, wt, K, M, N, K, epi=_lib.EPI_RESID_F32, bias=bias, X=resid, ldx=N, gamma=self.z['ones128'])
+        elif f32out is not None:
+            self.ops.gemm(a, lda, wt, K, M, N, K, epi=_lib.EPI_STORE_F32, act=act, bias=bias, X=f32out, ldx=N)
+        else:
+            self.ops.gemm(a, lda, wt, K, M, N, K, act=act, bias=bias, C=out, ldc=N)
+
+    def forward_batch(self, rgb, net_w, net_h=None, out_hw=None):
+        """rgb: uint8 CUDA [B,H,W,3] -> float32 CUDA [B,H,W] metric depth (what estimatezoedepth returns; invert = True)."""
+        import torch
+        ops, z, P, RELU = self.ops, self.z, self.PROJ, _lib.ACT_RELU
+        B, H, W, _ = rgb.shape
+        net_h = net_h if net_h is not None else net_w
+        pad_h, pad_w = int(np.sqrt(H / 2) * 3.0), int(np.sqrt(W / 2) * 3.0)       # depth_model.py:80-82 (fh = fw = 3)
+        Hp, Wp = H + 2 * pad_h, W + 2 * pad_w
+        nw, nh = midas_net_size(Wp, Hp, net_w, net_h)                               # PrepForMidas: keep aspect, x32, "minimal"
+        F = 2 * B
+        b = self._buffers(F, nh, nw)
+        ops.call("dm_zoe_preprocess_patchify", rgb, B, H, W, pad_h, pad_w, nh, nw, self.PATCH, b['patches'], self.kpad)
+        self.run_network(b, F, nh, nw)
+        zb = self._zbuffers(F, nh, nw, b)
+        Fp = self.Fp
+        # out_conv activation (MidasCore hooks output_conv[3], the 32-channel ReLU)
+        t = b['up_sizes'][3]
+        ops.conv3x3(b['path'][3], F, t[0], t[1], Fp, self.w['oc1_w'], self.F2p, bias=self.w['oc1_b'], C=b['oc1'])
+        ops.call("dm_resize_bilinear_nhwc_f16", b['oc1'], F, t[0], t[1], self.F2p, b['oc1u'], nh, nw)
+        ops.conv3x3(b['oc1u'], F, nh, nw, self.F2p, z['oc2_w'], 32, act=RELU, bias=z['oc2_b'], C=zb['o32'])
+        n0 = zb['n0']
+        # x = conv2(bottleneck); seed bins; seed embedding
+        self.lin(b['l'][3], Fp, z['conv2'], F * n0, Fp, Fp, out=zb['x16'])
+        self.seed_bins(zb, F)
+        self.lin(zb['x16'], Fp, z['sproj'][0], F * n0, P, Fp, out=zb['p0'], act=RELU)
+        self.lin(zb['p0'], P, z['sproj'][1], F * n0, 128, P, out=zb['pemb'])
+        # attractor levels
+        bprev, pemb, (hp, wp) = zb['bprev'], zb['pemb'], b['sizes'][3]
+        for i, (h, w) in enumerate(zb['levels']):
+            M = F * h * w
+            self.lin(b['path'][i], Fp, z['proj'][i][0], M, P, Fp, out=zb['t'][i], act=RELU)
+            self.lin(zb['t'][i], P, z['proj'][i][1], M, 128, P, out=zb['bemb'][i])
+            ops.call("dm_resize_add_nhwc_f16", zb['bemb'][i], pemb, F, hp, wp, 128, zb['xin'][i], h, w)
+            self.lin(zb['xin'][i], 128, z['att'][i][0], M, self.ATT_HID, 128, out=zb['a0'][i], act=RELU)
+            self.lin(zb['a0'][i], self.ATT_HID, z['att'][i][1], M, self.ATT_OUT, self.ATT_HID, f32out=zb['A'][i])
+            self.attractor(i, zb, bprev, F, hp, wp, h, w)
+            bprev, pemb, (hp, wp) = zb['bnew'][i], zb['bemb'][i], (h, w)
+        # conditional log-binomial + expectation, then un-pad / un-flip / average (depth_model.py:88-129)
+        ops.gemm(zb['bemb'][3], 128, z['clb'][0], 128, F * hp * wp, 128, 128, epi=_lib.EPI_STORE_F32, X=zb['ze'], ldx=128)
+        self.log_binomial(zb, bprev, F, nh, nw, hp, wp)
+        out = torch.empty(B, H, W, dtype=torch.float32, device=self.device)
+        ops.call("dm_zoe_tta_combine", zb['d'], B, nh, nw, pad_h, pad_w, H, W, out)
+        return out
+
+
+class ZoeDepthNKEngine(_ZoeDepthBase):
+    """ZoeDepth-NK (model type 9, zoedepth_nk): the metric head of ZoeDepthNK.forward (zoedepth_nk/zoedepth_nk_v1.py:159-243) on
+    the shared ZoeDepth skeleton.  The router picks nyu / kitti per forward on the device (argmax of two logits, no host sync, no
+    cross-image vote); both heads' layers are packed side by side."""
+
+    PROJ, ATT_HID, ATT_OUT = 64, 256, 64
 
     # ---- weights -------------------------------------------------------------------------------------------------------
     def _pack_head(self, sd):
         import torch
         dev = self.device
-        z = {}
-
-        def W(key, rows=None, cols=None):      # 1x1 conv / linear weight -> fp16 [rows, cols] (zero padded)
-            t = sd[key + '.weight'].detach().to(dev).float()
-            t = t.reshape(t.shape[0], -1)
-            r, c = rows or t.shape[0], cols or t.shape[1]
-            o = torch.zeros(r, c, dtype=torch.float16, device=dev)
-            o[:t.shape[0], :t.shape[1]] = t.to(torch.float16)
-            return o
-
-        def Bv(key, n=None):
-            t = sd[key + '.bias'].detach().to(dev).float().reshape(-1)
-            o = torch.zeros(n or t.numel(), dtype=torch.float32, device=dev)
-            o[:t.numel()] = t
-            return o
-
-        z['conv2'] = (W('conv2'), Bv('conv2'))
-        z['emb'] = (W('patch_transformer.embedding_convPxP'), Bv('patch_transformer.embedding_convPxP'))
+        W, Bv, lin = (functools.partial(f, sd, dev) for f in (_zoe_w, _zoe_b, _zoe_lin))
+        z = {'conv2': lin('conv2'), 'emb': lin('patch_transformer.embedding_convPxP')}
         layers = []
         for i in range(ZOE_CONFIG['router_layers']):
             q = f'patch_transformer.transformer_encoder.layers.{i}'
             f32 = lambda k: sd[k].detach().to(dev).float().contiguous()
             layers.append(dict(
                 in_w=sd[q + '.self_attn.in_proj_weight'].detach().to(dev, torch.float16).contiguous(), in_b=f32(q + '.self_attn.in_proj_bias'),
-                out=(W(q + '.self_attn.out_proj'), Bv(q + '.self_attn.out_proj')),
-                l1=(W(q + '.linear1'), Bv(q + '.linear1')), l2=(W(q + '.linear2'), Bv(q + '.linear2')),
+                out=lin(q + '.self_attn.out_proj'), l1=lin(q + '.linear1'), l2=lin(q + '.linear2'),
                 n1=(f32(q + '.norm1.weight'), f32(q + '.norm1.bias')), n2=(f32(q + '.norm2.weight'), f32(q + '.norm2.bias'))))
         z['layers'] = layers
-        z['cls0'] = (W('mlp_classifier.0'), Bv('mlp_classifier.0'))
-        z['cls2'] = (W('mlp_classifier.2', rows=32), Bv('mlp_classifier.2', 32))
+        z['cls0'] = lin('mlp_classifier.0')
+        z['cls2'] = lin('mlp_classifier.2', 32)
         z['ones128'] = torch.ones(128, dtype=torch.float32, device=dev)
         z['zeros128'] = torch.zeros(128, dtype=torch.float32, device=dev)
         names = ('nyu', 'kitti')
@@ -1144,8 +1079,8 @@ class ZoeDepthNKEngine(DptBeitEngine):
         for k, n in enumerate(names):
             w2[64 * k:64 * k + 64, 64 * k:64 * k + 64] = W(f'seed_bin_regressors.{n}._net.2')
         z['seed2'] = (w2, torch.cat([Bv(f'seed_bin_regressors.{n}._net.2') for n in names]))
-        z['sproj'] = ((W('seed_projector._net.0'), Bv('seed_projector._net.0')), (W('seed_projector._net.2'), Bv('seed_projector._net.2')))
-        z['proj'] = [((W(f'projectors.{i}._net.0'), Bv(f'projectors.{i}._net.0')), (W(f'projectors.{i}._net.2'), Bv(f'projectors.{i}._net.2'))) for i in range(4)]
+        z['sproj'] = _zoe_mlp(sd, dev, 'seed_projector')
+        z['proj'] = [_zoe_mlp(sd, dev, f'projectors.{i}') for i in range(4)]
         att = []
         for i in range(4):
             a0 = (torch.cat([W(f'attractors.{n}.{i}._net.0') for n in names]), torch.cat([Bv(f'attractors.{n}.{i}._net.0') for n in names]))
@@ -1174,17 +1109,8 @@ class ZoeDepthNKEngine(DptBeitEngine):
             w2c[k] = sd[f'conditional_log_binomial.{n}.mlp.2.weight'].detach().to(dev).float().reshape(4, 40)
             b2c[k] = sd[f'conditional_log_binomial.{n}.mlp.2.bias'].detach().to(dev).float()
         z['clb'] = (we, wo.contiguous(), b0.contiguous(), w2c.contiguous(), b2c.contiguous())
-        # out_conv with 64 output channels (32 real + 32 zero) so the stored activation is a valid GEMM-friendly NHWC tensor
-        h = 'depth_head.'
-        z['oc2_w'] = _conv_w(self._oc2_weight.to(dev), self.F2p, 32)
-        z['oc2_b'] = self._oc2_bias.to(dev).float().contiguous()
         self.z = z
         self._pe_cache = {}
-
-    def _pack(self, sd):
-        self._oc2_weight = sd['scratch.output_conv.2.weight'].detach()
-        self._oc2_bias = sd['scratch.output_conv.2.bias'].detach()
-        super()._pack(sd)
 
     def _router_pe(self, S):
         """PositionalEncodingPermute1D replacement of patch_transformer.py:45-62: sin | cos of position * 10000^(-2i/E)."""
@@ -1198,124 +1124,43 @@ class ZoeDepthNKEngine(DptBeitEngine):
             self._pe_cache = {S: torch.cat([torch.sin(pe), torch.cos(pe)], dim=1).contiguous()}
         return self._pe_cache[S]
 
-    def _zbuffers(self, F, nh, nw, b):
-        import torch
-        key = (F, nh, nw)
-        if self._zbuf_key == key:
-            return self._zbufs
-        dev = self.device
-        h16 = lambda *s: torch.empty(*s, dtype=torch.float16, device=dev)
-        f32 = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
-        s3 = b['sizes'][3]
-        n0 = s3[0] * s3[1]
+    def _seed_buffers(self, F, n0, h16, f32):
         S = n0 + 1
-        levels = list(b['up_sizes'])                       # (h, w) of refinenet4..1 outputs
-        zb = dict(x16=h16(F * n0, self.Fp), emb=h16(F * n0, 128), X=f32(F * S, 128), h=h16(F * S, 128), qkv=h16(F * S, 384), att=h16(F * S, 128),
-                  ff=h16(F * S, 1024), c1=h16(F, 128), logits=f32(F, 32), s0=h16(F * n0, 128), seed=f32(F * n0, 128), bprev=f32(F * n0, 64),
-                  p0=h16(F * n0, 64), pemb=h16(F * n0, 128), S=S, n0=n0, levels=levels)
-        zb['t'] = [h16(F * h * w, 64) for h, w in levels]
-        zb['bemb'] = [h16(F * h * w, 128) for h, w in levels]
-        zb['xin'] = [h16(F * h * w, 128) for h, w in levels]
-        zb['a0'] = [h16(F * h * w, 256) for h, w in levels]
-        zb['A'] = [f32(F * h * w, 64) for h, w in levels]
-        zb['bnew'] = [f32(F * h * w, 64) for h, w in levels]
-        zb['ze'] = f32(F * levels[3][0] * levels[3][1], 128)
-        zb['o32'] = h16(F, nh, nw, 32)
-        zb['d'] = f32(F, nh, nw)
-        self._zbufs, self._zbuf_key = zb, key
-        return zb
+        return dict(emb=h16(F * n0, 128), X=f32(F * S, 128), h=h16(F * S, 128), qkv=h16(F * S, 384), att=h16(F * S, 128), ff=h16(F * S, 1024),
+                    c1=h16(F, 128), logits=f32(F, 32), s0=h16(F * n0, 128), seed=f32(F * n0, 128), S=S)
 
-    # ---- forward -------------------------------------------------------------------------------------------------------
-    def forward_batch(self, rgb, net_w, net_h=None, out_hw=None):
-        """rgb: uint8 CUDA [B,H,W,3] -> float32 CUDA [B,H,W] metric depth (what estimatezoedepth returns; invert = True)."""
-        import torch
-        L = self.ops.L
-        ops, z = self.ops, self.z
-        st = _lib.stream_ptr
-        B, H, W, _ = rgb.shape
-        net_h = net_h if net_h is not None else net_w
-        pad_h, pad_w = int(np.sqrt(H / 2) * 3.0), int(np.sqrt(W / 2) * 3.0)       # depth_model.py:80-82 (fh = fw = 3)
-        Hp, Wp = H + 2 * pad_h, W + 2 * pad_w
-        nw, nh = midas_net_size(Wp, Hp, net_w, net_h)                               # PrepForMidas: keep aspect, x32, "minimal"
-        F = 2 * B
-        b = self._buffers(F, nh, nw)
-        _lib.check(L.dm_zoe_preprocess_patchify(rgb.data_ptr(), B, H, W, pad_h, pad_w, nh, nw, self.PATCH, b['patches'].data_ptr(), self.kpad, st()),
-                   "dm_zoe_preprocess_patchify")
-        ops.launches += 1
-        self.run_network(b, F, nh, nw)
-        zb = self._zbuffers(F, nh, nw, b)
-        Fp = self.Fp
-        E_, A_ = _lib, _lib
-        # out_conv activation (MidasCore hooks output_conv[3], the 32-channel ReLU)
-        t = b['up_sizes'][3]
-        ops.conv3x3(b['path'][3], F, t[0], t[1], Fp, self.w['oc1_w'], self.F2p, bias=self.w['oc1_b'], C=b['oc1'])
-        ops.resize_nhwc(b['oc1'], F, t[0], t[1], self.F2p, b['oc1u'], nh, nw)
-        ops.conv3x3(b['oc1u'], F, nh, nw, self.F2p, z['oc2_w'], 32, act=A_.ACT_RELU, bias=z['oc2_b'], C=zb['o32'])
-        n0, S = zb['n0'], zb['S']
-        s3 = b['sizes'][3]
-
-        def lin(a, lda, wb, M, N, K, out=None, ldc=None, act=A_.ACT_NONE, f32out=None, resid=None):
-            wt, bias = wb
-            if resid is not None:
-                ops.gemm(a, lda, wt, K, M, N, K, epi=E_.EPI_RESID_F32, bias=bias, X=resid, ldx=N, gamma=z['ones128'])
-            elif f32out is not None:
-                ops.gemm(a, lda, wt, K, M, N, K, epi=E_.EPI_STORE_F32, act=act, bias=bias, X=f32out, ldx=N)
-            else:
-                ops.gemm(a, lda, wt, K, M, N, K, act=act, bias=bias, C=out, ldc=ldc or N)
-
-        # x = conv2(bottleneck) (zoedepth_nk_v1.py:176-178)
-        lin(b['l'][3], Fp, z['conv2'], F * n0, Fp, Fp, out=zb['x16'])
-        # ---- router: PatchTransformerEncoder (patch size 1) + MLP classifier (:186-195) ----
-        lin(zb['x16'], Fp, z['emb'], F * n0, 128, Fp, out=zb['emb'])
-        ops.tokens(zb['emb'], z['zeros128'], self._router_pe(S), zb['X'], F, n0, 128)
-        _lib.check(L.dm_cast_f32_f16(zb['X'].data_ptr(), F * S * 128, zb['h'].data_ptr(), st()), "dm_cast_f32_f16")
-        ops.launches += 1
+    # ---- the NK-specific steps of the forward --------------------------------------------------------------------------
+    def seed_bins(self, zb, F):
+        """router: PatchTransformerEncoder (patch size 1) + MLP classifier (zoedepth_nk_v1.py:186-195); the seed bins of both heads
+        and the routed head's softplus (:197-206)"""
+        ops, z, RELU = self.ops, self.z, _lib.ACT_RELU
+        n0, S, Fp = zb['n0'], zb['S'], self.Fp
+        self.lin(zb['x16'], Fp, z['emb'], F * n0, 128, Fp, out=zb['emb'])
+        ops.call("dm_assemble_tokens", zb['emb'], z['zeros128'], self._router_pe(S), zb['X'], F, n0, 128)
+        ops.call("dm_cast_f32_f16", zb['X'], F * S * 128, zb['h'])
         for lay in z['layers']:
-            lin(zb['h'], 128, (lay['in_w'], lay['in_b']), F * S, 384, 128, out=zb['qkv'])
-            _lib.check(L.dm_attention_small_f16(zb['qkv'].data_ptr(), F, S, ZOE_CONFIG['router_heads'], 1.0 / math.sqrt(32.0), zb['att'].data_ptr(), st()),
-                       "dm_attention_small_f16")
-            lin(zb['att'], 128, lay['out'], F * S, 128, 128, resid=zb['X'])
-            _lib.check(L.dm_layernorm_post_f16(zb['X'].data_ptr(), F * S, 128, lay['n1'][0].data_ptr(), lay['n1'][1].data_ptr(), 1e-5, zb['h'].data_ptr(), st()),
-                       "dm_layernorm_post_f16")
-            lin(zb['h'], 128, lay['l1'], F * S, 1024, 128, out=zb['ff'], act=A_.ACT_RELU)
-            lin(zb['ff'], 1024, lay['l2'], F * S, 128, 1024, resid=zb['X'])
-            _lib.check(L.dm_layernorm_post_f16(zb['X'].data_ptr(), F * S, 128, lay['n2'][0].data_ptr(), lay['n2'][1].data_ptr(), 1e-5, zb['h'].data_ptr(), st()),
-                       "dm_layernorm_post_f16")
-            ops.launches += 3
-        lin(zb['h'], S * 128, z['cls0'], F, 128, 128, out=zb['c1'], act=A_.ACT_RELU)       # token 0 of every forward (row pitch S*128)
-        lin(zb['c1'], 128, z['cls2'], F, 32, 128, f32out=zb['logits'])
-        lg = zb['logits']
-        # ---- seed bins + seed embedding (:197-206) ----
-        lin(zb['x16'], Fp, z['seed0'], F * n0, 128, Fp, out=zb['s0'], act=A_.ACT_RELU)
-        lin(zb['s0'], 128, z['seed2'], F * n0, 128, 128, f32out=zb['seed'])
-        _lib.check(L.dm_zoe_select_softplus(zb['seed'].data_ptr(), 128, lg.data_ptr(), 32, F, n0, zb['bprev'].data_ptr(), st()), "dm_zoe_select_softplus")
-        lin(zb['x16'], Fp, z['sproj'][0], F * n0, 64, Fp, out=zb['p0'], act=A_.ACT_RELU)
-        lin(zb['p0'], 64, z['sproj'][1], F * n0, 128, 64, out=zb['pemb'])
-        ops.launches += 1
-        # ---- attractor levels (:207-214) ----
-        bprev, pemb, (hp, wp) = zb['bprev'], zb['pemb'], s3
-        for i, (h, w) in enumerate(zb['levels']):
-            M = F * h * w
-            lin(b['path'][i], Fp, z['proj'][i][0], M, 64, Fp, out=zb['t'][i], act=A_.ACT_RELU)
-            lin(zb['t'][i], 64, z['proj'][i][1], M, 128, 64, out=zb['bemb'][i])
-            _lib.check(L.dm_resize_add_nhwc_f16(zb['bemb'][i].data_ptr(), pemb.data_ptr(), F, hp, wp, 128, zb['xin'][i].data_ptr(), h, w, st()),
-                       "dm_resize_add_nhwc_f16")
-            lin(zb['xin'][i], 128, z['att'][i][0], M, 256, 128, out=zb['a0'][i], act=A_.ACT_RELU)
-            lin(zb['a0'][i], 256, z['att'][i][1], M, 64, 256, f32out=zb['A'][i])
-            _lib.check(L.dm_zoe_attractor(zb['A'][i].data_ptr(), 64, lg.data_ptr(), 32, bprev.data_ptr(), F, hp, wp, h, w, zb['bnew'][i].data_ptr(), st()),
-                       "dm_zoe_attractor")
-            ops.launches += 2
-            bprev, pemb, (hp, wp) = zb['bnew'][i], zb['bemb'][i], (h, w)
-        # ---- conditional log-binomial + expectation (:216-236), then un-pad / un-flip / average (depth_model.py:88-129) ----
-        we, wo, b0, w2c, b2c = z['clb']
-        ops.gemm(zb['bemb'][3], 128, we, 128, F * hp * wp, 128, 128, epi=E_.EPI_STORE_F32, X=zb['ze'], ldx=128)
-        _lib.check(L.dm_zoe_clb_final(zb['o32'].data_ptr(), 32, zb['ze'].data_ptr(), 128, bprev.data_ptr(), lg.data_ptr(), 32, wo.data_ptr(), b0.data_ptr(),
-                                      w2c.data_ptr(), b2c.data_ptr(), F, nh, nw, hp, wp, ZOE_CONFIG['min_temp'], ZOE_CONFIG['max_temp'],
-                                      zb['d'].data_ptr(), st()), "dm_zoe_clb_final")
-        out = torch.empty(B, H, W, dtype=torch.float32, device=self.device)
-        _lib.check(L.dm_zoe_tta_combine(zb['d'].data_ptr(), B, nh, nw, pad_h, pad_w, H, W, out.data_ptr(), st()), "dm_zoe_tta_combine")
-        ops.launches += 2
-        return out
+            self.lin(zb['h'], 128, (lay['in_w'], lay['in_b']), F * S, 384, 128, out=zb['qkv'])
+            ops.call("dm_attention_small_f16", zb['qkv'], F, S, ZOE_CONFIG['router_heads'], 1.0 / math.sqrt(32.0), zb['att'])
+            self.lin(zb['att'], 128, lay['out'], F * S, 128, 128, resid=zb['X'])
+            ops.call("dm_layernorm_post_f16", zb['X'], F * S, 128, lay['n1'][0], lay['n1'][1], 1e-5, zb['h'])
+            self.lin(zb['h'], 128, lay['l1'], F * S, 1024, 128, out=zb['ff'], act=RELU)
+            self.lin(zb['ff'], 1024, lay['l2'], F * S, 128, 1024, resid=zb['X'])
+            ops.call("dm_layernorm_post_f16", zb['X'], F * S, 128, lay['n2'][0], lay['n2'][1], 1e-5, zb['h'])
+        self.lin(zb['h'], S * 128, z['cls0'], F, 128, 128, out=zb['c1'], act=RELU)       # token 0 of every forward (row pitch S*128)
+        self.lin(zb['c1'], 128, z['cls2'], F, 32, 128, f32out=zb['logits'])
+        self.lin(zb['x16'], Fp, z['seed0'], F * n0, 128, Fp, out=zb['s0'], act=RELU)
+        self.lin(zb['s0'], 128, z['seed2'], F * n0, 128, 128, f32out=zb['seed'])
+        ops.call("dm_zoe_select_softplus", zb['seed'], 128, zb['logits'], 32, F, n0, zb['bprev'])
+
+    def attractor(self, i, zb, bprev, F, hp, wp, h, w):
+        """(:207-214)"""
+        self.ops.call("dm_zoe_attractor", zb['A'][i], 64, zb['logits'], 32, bprev, F, hp, wp, h, w, zb['bnew'][i])
+
+    def log_binomial(self, zb, bprev, F, nh, nw, hp, wp):
+        """(:216-236)"""
+        _, wo, b0, w2c, b2c = self.z['clb']
+        self.ops.call("dm_zoe_clb_final", zb['o32'], 32, zb['ze'], 128, bprev, zb['logits'], 32, wo, b0, w2c, b2c, F, nh, nw, hp, wp,
+                      ZOE_CONFIG['min_temp'], ZOE_CONFIG['max_temp'], zb['d'])
 
 
 # ZoeDepth-N / -K: get_config("zoedepth", "infer") and its "kitti" version.  Neither sets min_depth / max_depth, so both keep
@@ -1325,52 +1170,28 @@ ZOE_SINGLE_VARIANTS = {'n': dict(model_type=7, bin_centers_type='softplus', chec
                        'k': dict(model_type=8, bin_centers_type='normed', checkpoint='ZoeD_M12_K.pt')}
 
 
-class ZoeDepthEngine(DptBeitEngine):
-    """Single-head ZoeDepth on the sm_90a kernels: ZoeDepth-N (variant 'n', model type 7, softplus bin centres) and ZoeDepth-K
-    ('k', model type 8, bin centres normed to [min_depth, max_depth]).  Same core, pre-processing and pad + flip test-time
-    augmentation as ZoeDepthNKEngine (image b and its flip are forwards 2b / 2b+1); the head is ZoeDepth.forward
+class ZoeDepthEngine(_ZoeDepthBase):
+    """Single-head ZoeDepth: ZoeDepth-N (variant 'n', model type 7, softplus bin centres) and ZoeDepth-K ('k', model type 8, bin
+    centres normed to [min_depth, max_depth]) on the shared ZoeDepth skeleton.  The head is ZoeDepth.forward
     (dzoedepth/models/zoedepth/zoedepth_v1.py:124-192): seed bins, four attractor levels with [16, 8, 4, 1] attractors, and a
     log-binomial whose 33rd input is the core's own relative depth.  Bin centres, attractor points and the log-binomial stay in
-    fp32.  Checkpoint layout as ZoeDepth-NK: MiDaS weights under "core.core.", head weights at the top level."""
+    fp32."""
+
+    PROJ, ATT_HID, ATT_OUT = 128, 128, 32
 
     def __init__(self, state_dict, device, variant, core_name='beitl16_384'):
         if variant not in ZOE_SINGLE_VARIANTS:
             raise ValueError(f"ZoeDepthEngine: variant must be 'n' or 'k', not {variant!r}")
         self.variant = variant
         self.normed = ZOE_SINGLE_VARIANTS[variant]['bin_centers_type'] == 'normed'
-        core_sd = {k[len("core.core."):]: v for k, v in state_dict.items() if k.startswith("core.core.")}
-        head_sd = {k: v for k, v in state_dict.items() if not k.startswith("core.")}
-        super().__init__(core_sd, core_name, device)
-        self._pack_head(head_sd)
-        self._zbuf_key, self._zbufs = None, {}
-
-    def _pack(self, sd):
-        self._oc2_weight = sd['scratch.output_conv.2.weight'].detach()
-        self._oc2_bias = sd['scratch.output_conv.2.bias'].detach()
-        super()._pack(sd)
+        super().__init__(state_dict, device, core_name)
 
     def _pack_head(self, sd):
         import torch
         dev = self.device
-
-        def W(key, rows=None):                 # 1x1 conv weight -> fp16 [rows, cin] (zero padded rows)
-            t = sd[key + '.weight'].detach().to(dev).float()
-            t = t.reshape(t.shape[0], -1)
-            o = torch.zeros(rows or t.shape[0], t.shape[1], dtype=torch.float16, device=dev)
-            o[:t.shape[0]] = t.to(torch.float16)
-            return o
-
-        def Bv(key, n=None):
-            t = sd[key + '.bias'].detach().to(dev).float().reshape(-1)
-            o = torch.zeros(n or t.numel(), dtype=torch.float32, device=dev)
-            o[:t.numel()] = t
-            return o
-
-        def mlp(key):
-            return ((W(key + '._net.0'), Bv(key + '._net.0')), (W(key + '._net.2'), Bv(key + '._net.2')))
-
-        z = {'conv2': (W('conv2'), Bv('conv2')), 'seed': mlp('seed_bin_regressor'), 'sproj': mlp('seed_projector'),
-             'proj': [mlp(f'projectors.{i}') for i in range(4)]}
+        lin = functools.partial(_zoe_lin, sd, dev)
+        z = {'conv2': lin('conv2'), 'seed': _zoe_mlp(sd, dev, 'seed_bin_regressor'), 'sproj': _zoe_mlp(sd, dev, 'seed_projector'),
+             'proj': [_zoe_mlp(sd, dev, f'projectors.{i}') for i in range(4)]}
         if z['seed'][1][0].shape[0] != ZOE_SINGLE_CONFIG['n_bins']:
             raise ValueError(f"ZoeDepthEngine: the seed bin regressor has {z['seed'][1][0].shape[0]} outputs, not 64 bins")
         per = 2 if self.normed else 1
@@ -1380,7 +1201,7 @@ class ZoeDepthEngine(DptBeitEngine):
             if sd[key + '.weight'].shape[0] != per * n:
                 raise ValueError(f"ZoeDepthEngine({self.variant!r}): {key} has {sd[key + '.weight'].shape[0]} outputs, expected {per * n} "
                                  f"({n} attractors{' x 2 for the normed layer' if self.normed else ''})")
-            att.append(((W(f'attractors.{i}._net.0'), Bv(f'attractors.{i}._net.0')), (W(key, rows=32), Bv(key, 32))))
+            att.append((lin(f'attractors.{i}._net.0'), lin(key, 32)))
         z['att'] = att
         # conditional log-binomial: mlp.0 over cat(out_conv (32), rel_depth (1), b_emb (128)), 80 outputs.  Its out_conv and
         # rel-depth part is evaluated per pixel in clb_single, its bin-embedding part is a GEMM before the up-sampling (a 1x1 conv
@@ -1391,108 +1212,71 @@ class ZoeDepthEngine(DptBeitEngine):
         m0 = m0.reshape(80, 161)
         we = torch.zeros(128, 128, dtype=torch.float16, device=dev)
         we[:80] = m0[:, 33:].to(torch.float16)
-        z['clb'] = (we, m0[:, :33].t().contiguous(), Bv('conditional_log_binomial.mlp.0'),
+        z['clb'] = (we, m0[:, :33].t().contiguous(), _zoe_b(sd, dev, 'conditional_log_binomial.mlp.0'),
                     sd['conditional_log_binomial.mlp.2.weight'].detach().to(dev).float().reshape(4, 80).contiguous(),
-                    Bv('conditional_log_binomial.mlp.2'))
-        z['oc2_w'] = _conv_w(self._oc2_weight.to(dev), self.F2p, 32)
-        z['oc2_b'] = self._oc2_bias.to(dev).float().contiguous()
+                    _zoe_b(sd, dev, 'conditional_log_binomial.mlp.2'))
         self.z = z
 
-    def _zbuffers(self, F, nh, nw, b):
-        import torch
-        key = (F, nh, nw)
-        if self._zbuf_key == key:
-            return self._zbufs
-        dev = self.device
-        h16 = lambda *s: torch.empty(*s, dtype=torch.float16, device=dev)
-        f32 = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
-        s3 = b['sizes'][3]
-        n0 = s3[0] * s3[1]
-        levels = list(b['up_sizes'])                       # (h, w) of refinenet4..1 outputs
-        zb = dict(x16=h16(F * n0, self.Fp), s0=h16(F * n0, 256), seed=f32(F * n0, 64), bprev=f32(F * n0, 64), p0=h16(F * n0, 128),
-                  pemb=h16(F * n0, 128), n0=n0, levels=levels)
-        zb['t'] = [h16(F * h * w, 128) for h, w in levels]
-        zb['bemb'] = [h16(F * h * w, 128) for h, w in levels]
-        zb['xin'] = [h16(F * h * w, 128) for h, w in levels]
-        zb['a0'] = [h16(F * h * w, 128) for h, w in levels]
-        zb['A'] = [f32(F * h * w, 32) for h, w in levels]
-        zb['bnew'] = [f32(F * h * w, 64) for h, w in levels]
-        zb['ze'] = f32(F * levels[3][0] * levels[3][1], 128)
-        zb['o32'] = h16(F, nh, nw, 32)
-        zb['d'] = f32(F, nh, nw)
-        self._zbufs, self._zbuf_key = zb, key
-        return zb
+    def _seed_buffers(self, F, n0, h16, f32):
+        return dict(s0=h16(F * n0, 256), seed=f32(F * n0, 64))
 
-    def forward_batch(self, rgb, net_w, net_h=None, out_hw=None):
-        """rgb: uint8 CUDA [B,H,W,3] -> float32 CUDA [B,H,W] metric depth (what estimatezoedepth returns; invert = True)."""
-        import torch
-        L = self.ops.L
-        ops, z = self.ops, self.z
-        st = _lib.stream_ptr
+    # ---- the N / K-specific steps of the forward -----------------------------------------------------------------------
+    def seed_bins(self, zb, F):
+        """seed bins (zoedepth_v1.py:151-159)"""
+        cfg, z, n0, Fp = ZOE_SINGLE_CONFIG, self.z, zb['n0'], self.Fp
+        self.lin(zb['x16'], Fp, z['seed'][0], F * n0, 256, Fp, out=zb['s0'], act=_lib.ACT_RELU)
+        self.lin(zb['s0'], 256, z['seed'][1], F * n0, 64, 256, f32out=zb['seed'])
+        self.ops.call("dm_zoe_seed_bins", zb['seed'], 64, F * n0, int(self.normed), cfg['min_depth'], cfg['max_depth'], zb['bprev'])
+
+    def attractor(self, i, zb, bprev, F, hp, wp, h, w):
+        """(:164-169); the normed head's last level hands on sorted, clipped centres"""
         cfg = ZOE_SINGLE_CONFIG
-        dmin, dmax = cfg['min_depth'], cfg['max_depth']
-        B, H, W, _ = rgb.shape
-        net_h = net_h if net_h is not None else net_w
-        pad_h, pad_w = int(np.sqrt(H / 2) * 3.0), int(np.sqrt(W / 2) * 3.0)       # depth_model.py:80-82 (fh = fw = 3)
-        Hp, Wp = H + 2 * pad_h, W + 2 * pad_w
-        nw, nh = midas_net_size(Wp, Hp, net_w, net_h)                               # PrepForMidas: keep aspect, x32, "minimal"
-        F = 2 * B
-        b = self._buffers(F, nh, nw)
-        _lib.check(L.dm_zoe_preprocess_patchify(rgb.data_ptr(), B, H, W, pad_h, pad_w, nh, nw, self.PATCH, b['patches'].data_ptr(), self.kpad, st()),
-                   "dm_zoe_preprocess_patchify")
-        ops.launches += 1
-        self.run_network(b, F, nh, nw)
-        zb = self._zbuffers(F, nh, nw, b)
-        Fp = self.Fp
-        E_, A_ = _lib, _lib
-        # out_conv activation (MidasCore hooks output_conv[3], the 32-channel ReLU); the core's relative depth, the final 1x1 conv
-        # + ReLU on it, is evaluated inside clb_single
-        t = b['up_sizes'][3]
-        ops.conv3x3(b['path'][3], F, t[0], t[1], Fp, self.w['oc1_w'], self.F2p, bias=self.w['oc1_b'], C=b['oc1'])
-        ops.resize_nhwc(b['oc1'], F, t[0], t[1], self.F2p, b['oc1u'], nh, nw)
-        ops.conv3x3(b['oc1u'], F, nh, nw, self.F2p, z['oc2_w'], 32, act=A_.ACT_RELU, bias=z['oc2_b'], C=zb['o32'])
-        n0, s3 = zb['n0'], b['sizes'][3]
+        sort_clip = int(self.normed and i == len(zb['levels']) - 1)
+        self.ops.call("dm_zoe_attractor_single", zb['A'][i], 32, cfg['n_attractors'][i], int(self.normed), bprev, F, hp, wp, h, w, sort_clip,
+                      cfg['min_depth'], cfg['max_depth'], zb['bnew'][i])
 
-        def lin(a, lda, wb, M, N, K, out=None, act=A_.ACT_NONE, f32out=None):
-            wt, bias = wb
-            if f32out is not None:
-                ops.gemm(a, lda, wt, K, M, N, K, epi=E_.EPI_STORE_F32, act=act, bias=bias, X=f32out, ldx=N)
-            else:
-                ops.gemm(a, lda, wt, K, M, N, K, act=act, bias=bias, C=out, ldc=N)
+    def log_binomial(self, zb, bprev, F, nh, nw, hp, wp):
+        """on cat(out_conv, rel_depth) + expectation (:171-192); the core's relative depth, the final 1x1 conv + ReLU on out_conv,
+        is evaluated inside clb_single"""
+        _, wo, b0, w2c, b2c = self.z['clb']
+        self.ops.call("dm_zoe_clb_single", zb['o32'], 32, zb['ze'], 128, bprev, wo, b0, w2c, b2c, self.w['oc3_w'], self.oc3_b, F, nh, nw, hp, wp,
+                      ZOE_SINGLE_CONFIG['min_temp'], ZOE_SINGLE_CONFIG['max_temp'], zb['d'])
 
-        # x = conv2(bottleneck); seed bins (zoedepth_v1.py:151-159) and seed embedding (:161)
-        lin(b['l'][3], Fp, z['conv2'], F * n0, Fp, Fp, out=zb['x16'])
-        lin(zb['x16'], Fp, z['seed'][0], F * n0, 256, Fp, out=zb['s0'], act=A_.ACT_RELU)
-        lin(zb['s0'], 256, z['seed'][1], F * n0, 64, 256, f32out=zb['seed'])
-        _lib.check(L.dm_zoe_seed_bins(zb['seed'].data_ptr(), 64, F * n0, int(self.normed), dmin, dmax, zb['bprev'].data_ptr(), st()), "dm_zoe_seed_bins")
-        lin(zb['x16'], Fp, z['sproj'][0], F * n0, 128, Fp, out=zb['p0'], act=A_.ACT_RELU)
-        lin(zb['p0'], 128, z['sproj'][1], F * n0, 128, 128, out=zb['pemb'])
-        ops.launches += 1
-        # attractor levels (:164-169); the normed head's last level hands on sorted, clipped centres
-        bprev, pemb, (hp, wp) = zb['bprev'], zb['pemb'], s3
-        for i, (h, w) in enumerate(zb['levels']):
-            M = F * h * w
-            lin(b['path'][i], Fp, z['proj'][i][0], M, 128, Fp, out=zb['t'][i], act=A_.ACT_RELU)
-            lin(zb['t'][i], 128, z['proj'][i][1], M, 128, 128, out=zb['bemb'][i])
-            _lib.check(L.dm_resize_add_nhwc_f16(zb['bemb'][i].data_ptr(), pemb.data_ptr(), F, hp, wp, 128, zb['xin'][i].data_ptr(), h, w, st()),
-                       "dm_resize_add_nhwc_f16")
-            lin(zb['xin'][i], 128, z['att'][i][0], M, 128, 128, out=zb['a0'][i], act=A_.ACT_RELU)
-            lin(zb['a0'][i], 128, z['att'][i][1], M, 32, 128, f32out=zb['A'][i])
-            sort_clip = int(self.normed and i == len(zb['levels']) - 1)
-            _lib.check(L.dm_zoe_attractor_single(zb['A'][i].data_ptr(), 32, cfg['n_attractors'][i], int(self.normed), bprev.data_ptr(), F, hp, wp,
-                                                 h, w, sort_clip, dmin, dmax, zb['bnew'][i].data_ptr(), st()), "dm_zoe_attractor_single")
-            ops.launches += 2
-            bprev, pemb, (hp, wp) = zb['bnew'][i], zb['bemb'][i], (h, w)
-        # conditional log-binomial on cat(out_conv, rel_depth) + expectation (:171-192), then un-pad / un-flip / average
-        we, wo, b0, w2c, b2c = z['clb']
-        ops.gemm(zb['bemb'][3], 128, we, 128, F * hp * wp, 128, 128, epi=E_.EPI_STORE_F32, X=zb['ze'], ldx=128)
-        _lib.check(L.dm_zoe_clb_single(zb['o32'].data_ptr(), 32, zb['ze'].data_ptr(), 128, bprev.data_ptr(), wo.data_ptr(), b0.data_ptr(),
-                                       w2c.data_ptr(), b2c.data_ptr(), self.w['oc3_w'].data_ptr(), self.oc3_b, F, nh, nw, hp, wp,
-                                       cfg['min_temp'], cfg['max_temp'], zb['d'].data_ptr(), st()), "dm_zoe_clb_single")
-        out = torch.empty(B, H, W, dtype=torch.float32, device=self.device)
-        _lib.check(L.dm_zoe_tta_combine(zb['d'].data_ptr(), B, nh, nw, pad_h, pad_w, H, W, out.data_ptr(), st()), "dm_zoe_tta_combine")
-        ops.launches += 2
-        return out
+
+def _unwrap_key(key, where):
+    """training checkpoints wrap the weights in a dict; a flat state dict never has these top-level keys"""
+    return lambda sd: sd[key] if where in sd else sd
+
+
+def _unwrap_leres(sd):
+    """src/depthmap_generation.py:113-116: strip_prefix_if_present(checkpoint['depth_model'], "module.")"""
+    if "depth_model" not in sd:
+        return sd
+    return {(k[len("module."):] if k.startswith("module.") else k): v for k, v in sd["depth_model"].items()}
+
+
+_flat = lambda sd: sd
+_midas = _unwrap_key("model", "optimizer")      # dmidas/base_model.py:13
+_zoe = _unwrap_key("model", "model")            # dzoedepth/models/model_io.py:52-53
+_native = lambda sd, t, dev, boost: NativeDepthModel(sd, t, dev)
+# model type -> (default checkpoint path, unwrap, engine(state_dict, model type, device, boost)).  The MiDaS DPT
+# models run through the op-level engine under BOOST (float crops, estimatemidasBoost) and through the model-level handle otherwise.
+CHECKPOINTS = {
+    0: ("./models/leres/res101.pth", _unwrap_leres, lambda sd, t, dev, boost: LeresEngine(sd, dev)),
+    1: ("./models/midas/dpt_beit_large_512.pt", _midas,
+        lambda sd, t, dev, boost: DptBeitEngine(sd, 'beitl16_512', dev) if boost else NativeDepthModel(sd, t, dev)),
+    2: ("./models/midas/dpt_beit_large_384.pt", _midas,
+        lambda sd, t, dev, boost: DptBeitEngine(sd, 'beitl16_384', dev) if boost else NativeDepthModel(sd, t, dev)),
+    3: ("./models/midas/dpt_large-midas-2f21e586.pt", _midas,
+        lambda sd, t, dev, boost: DptVitEngine(sd, 'vitl16_384', dev) if boost else NativeDepthModel(sd, t, dev)),
+    7: ("./models/zoedepth/" + ZOE_SINGLE_VARIANTS['n']['checkpoint'], _zoe, lambda sd, t, dev, boost: ZoeDepthEngine(sd, dev, 'n')),
+    8: ("./models/zoedepth/" + ZOE_SINGLE_VARIANTS['k']['checkpoint'], _zoe, lambda sd, t, dev, boost: ZoeDepthEngine(sd, dev, 'k')),
+    9: ("./models/zoedepth/ZoeD_M12_NK.pt", _zoe, lambda sd, t, dev, boost: ZoeDepthNKEngine(sd, dev)),
+    12: ("./models/depth_anything_v2/depth_anything_v2_vits.pth", _flat, _native),
+    13: ("./models/depth_anything_v2/depth_anything_v2_vitb.pth", _flat, _native),
+    14: ("./models/depth_anything_v2/depth_anything_v2_vitl.pth", _flat, _native),
+}
+PIX2PIX_CHECKPOINT = "./models/pix2pix/latest_net_G.pth"
 
 
 class ModelHolder:
@@ -1543,94 +1327,33 @@ class ModelHolder:
             # silently ignoring the setting
             raise NotImplementedError("no_half (fp32 network) is not implemented in depthmap_b200: the tensor-core path uses fp16 operands "
                                       "with fp32 accumulation; unset the setting")
-        if model_type in (12, 13, 14):
-            letter = {12: 's', 13: 'b', 14: 'l'}[model_type]
-            if self.weights_provider is not None:
-                sd = self.weights_provider(model_type)
-            else:
-                model_path = f"./models/depth_anything_v2/depth_anything_v2_vit{letter}.pth"
-                if not os.path.exists(model_path):
-                    raise FileNotFoundError(f"{model_path} not found (depthmap_b200 does not download checkpoints)")
-                sd = torch.load(model_path, map_location='cpu')
-            model = NativeDepthModel(sd, model_type, torch.device(device))
-        elif model_type in (1, 2):  # dpt_beit_large_512 / dpt_beit_large_384 (MiDaS 3.1)
-            name = {1: 'beitl16_512', 2: 'beitl16_384'}[model_type]
-            if self.weights_provider is not None:
-                sd = self.weights_provider(model_type)
-            else:
-                model_path = "./models/midas/" + {1: 'dpt_beit_large_512.pt', 2: 'dpt_beit_large_384.pt'}[model_type]
-                if not os.path.exists(model_path):
-                    raise FileNotFoundError(f"{model_path} not found (depthmap_b200 does not download checkpoints)")
-                sd = torch.load(model_path, map_location='cpu')
-                if "optimizer" in sd:       # dmidas/base_model.py:13: training checkpoints wrap the weights
-                    sd = sd["model"]
-            # BOOST feeds float crops through the op-level engine (estimatemidasBoost); plain forwards use the model-level handle
-            model = DptBeitEngine(sd, name, torch.device(device)) if boost else NativeDepthModel(sd, model_type, torch.device(device))
-        elif model_type == 0:  # res101 (LeReS)
-            if self.weights_provider is not None:
-                sd = self.weights_provider(model_type)
-            else:
-                model_path = "./models/leres/res101.pth"
-                if not os.path.exists(model_path):
-                    raise FileNotFoundError(f"{model_path} not found (depthmap_b200 does not download checkpoints)")
-                sd = torch.load(model_path, map_location='cpu')
-                if "depth_model" in sd:      # src/depthmap_generation.py:113-116: strip_prefix_if_present(checkpoint['depth_model'], "module.")
-                    sd = {(k[len("module."):] if k.startswith("module.") else k): v for k, v in sd["depth_model"].items()}
-            model = LeresEngine(sd, torch.device(device))
-        elif model_type == 3:  # dpt_large_384 (MiDaS 3.0)
-            if self.weights_provider is not None:
-                sd = self.weights_provider(model_type)
-            else:
-                model_path = "./models/midas/dpt_large-midas-2f21e586.pt"
-                if not os.path.exists(model_path):
-                    raise FileNotFoundError(f"{model_path} not found (depthmap_b200 does not download checkpoints)")
-                sd = torch.load(model_path, map_location='cpu')
-                if "optimizer" in sd:
-                    sd = sd["model"]
-            model = DptVitEngine(sd, 'vitl16_384', torch.device(device)) if boost else NativeDepthModel(sd, model_type, torch.device(device))
-        elif model_type == 9:  # zoedepth_nk (src/depthmap_generation.py:221-226: ZoeD_M12_NK.pt)
-            if self.weights_provider is not None:
-                sd = self.weights_provider(model_type)
-            else:
-                model_path = "./models/zoedepth/ZoeD_M12_NK.pt"
-                if not os.path.exists(model_path):
-                    raise FileNotFoundError(f"{model_path} not found (depthmap_b200 does not download checkpoints)")
-                sd = torch.load(model_path, map_location='cpu')
-                if "model" in sd:           # dzoedepth/models/model_io.py:52-53
-                    sd = sd["model"]
-            model = ZoeDepthNKEngine(sd, torch.device(device))
-        elif model_type in (7, 8):  # zoedepth_n (indoor) / zoedepth_k (outdoor) (src/depthmap_generation.py:196-204)
-            variant = {7: 'n', 8: 'k'}[model_type]
-            if self.weights_provider is not None:
-                sd = self.weights_provider(model_type)
-            else:
-                model_path = "./models/zoedepth/" + ZOE_SINGLE_VARIANTS[variant]['checkpoint']
-                if not os.path.exists(model_path):
-                    raise FileNotFoundError(f"{model_path} not found (depthmap_b200 does not download checkpoints)")
-                sd = torch.load(model_path, map_location='cpu')
-            if "model" in sd:               # dzoedepth/models/model_io.py:52-53
-                sd = sd["model"]
-            model = ZoeDepthEngine(sd, torch.device(device), variant)
-        else:
+        if model_type not in CHECKPOINTS:
             raise NotImplementedError(f"model_type {model_type} is not implemented in depthmap_b200 yet "
                                       f"(implemented: 0 = LeReS res101; 1, 2 = DPT-BEiT-L 512/384; 3 = DPT-Large 384; 7 = ZoeDepth-N; "
                                       f"8 = ZoeDepth-K; 9 = ZoeDepth-NK; 12, 13, 14 = Depth-Anything-V2 S/B/L)")
+        dev = torch.device(device)
+        path, unwrap, make = CHECKPOINTS[model_type]
+        model = make(self._load_checkpoint(model_type, path, unwrap), model_type, dev, boost)
         if boost:      # reference :284-299: the pix2pix merge network ('latest_net_G.pth', netG = unet_1024, norm none)
             from .boost import BoostPipeline, UnetMergeEngine
-            if self.weights_provider is not None:
-                psd = self.weights_provider("pix2pix")
-            else:
-                p2p_path = "./models/pix2pix/latest_net_G.pth"
-                if not os.path.exists(p2p_path):
-                    raise FileNotFoundError(f"{p2p_path} not found (depthmap_b200 does not download checkpoints)")
-                psd = torch.load(p2p_path, map_location='cpu')
-            self.pix2pix_model = BoostPipeline(model, UnetMergeEngine(psd, torch.device(device)), torch.device(device), model_type)
+            self.pix2pix_model = BoostPipeline(model, UnetMergeEngine(self._load_checkpoint("pix2pix", PIX2PIX_CHECKPOINT), dev), dev, model_type)
         self.depth_model = model
         self.depth_model_type = model_type
         self.resize_mode = "minimal"
         self.normalization = None
         self.tiling_mode = tiling_mode
         self.device = device
+
+    def _load_checkpoint(self, key, path, unwrap=_flat):
+        """weights_provider(key), or torch.load of the default path; unwrapped to the flat state dict"""
+        import torch
+        if self.weights_provider is not None:
+            sd = self.weights_provider(key)
+        else:
+            if not os.path.exists(path):
+                raise FileNotFoundError(f"{path} not found (depthmap_b200 does not download checkpoints)")
+            sd = torch.load(path, map_location='cpu')
+        return unwrap(sd)
 
     @staticmethod
     def get_default_net_size(model_type):

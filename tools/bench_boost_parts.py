@@ -50,7 +50,7 @@ def main():
     timeit("cubic resize 3 x 2048^2 -> 3 x 3136^2", lambda: pipe._cubic(img.data_ptr(), 2048, 2048, 2048, 3136, 3136, planes=3, src_plane=2048 * 2048))
     # eager (no graph) for comparison
     unet2 = UnetMergeEngine(synth_weights.make_pix2pix_state_dict(seed=1), dev)
-    unet2._use_graph = False
+    unet2._graphs.enabled = False
     timeit("merge U-Net forward, eager launches", lambda: unet2.forward(x2), n=5)
 
 
