@@ -117,7 +117,7 @@ class Dav2Stereo(_NetWorkload):
     FLOP_PER_IMAGE = 1304.2e9  # SURVEY §8d, cross-checked there against FlopCounterMode on the reference module
     MODEL_TYPE = 14
     ATTN_KERNEL = "attention_wgmma_kernel<0> (fused softmax(QK^T)V, wgmma, N = 1370, 16 heads x 64)"
-    FC1_KERNEL = "gemm_wgmma_kernel<128> (128x128 tiles; block-0 MLP fc1: M=B*1370, N=4096, K=1024, GELU epilogue)"
+    FC1_KERNEL = "gemm_wgmma_kernel<64, 256> (persistent ping-pong, 64x256 tile per warpgroup; block-0 MLP fc1: M=B*1370, N=4096, K=1024, GELU epilogue)"
 
     def _state_dict(self):
         from oracle import synth_weights  # synthetic checkpoint-layout weights (data generation, not compute)
@@ -210,7 +210,7 @@ class DepthBeit512(_NetWorkload):
     MODEL_TYPE = 1
     output_names = ("depth",)
     ATTN_KERNEL = "attention_wgmma_kernel<2> (fused softmax(QK^T + rel-pos bias)V, wgmma, N = 1025, 16 heads x 64)"
-    FC1_KERNEL = "gemm_wgmma_kernel<128> (128x128 tiles; block-0 MLP fc1: M=B*1025, N=4096, K=1024, GELU epilogue)"
+    FC1_KERNEL = "gemm_wgmma_kernel<64, 256> (persistent ping-pong, 64x256 tile per warpgroup; block-0 MLP fc1: M=B*1025, N=4096, K=1024, GELU epilogue)"
 
     def _state_dict(self):
         from oracle import synth_weights  # synthetic checkpoint-layout weights (data generation, not compute)
@@ -294,7 +294,7 @@ class ZoeAnaglyph(_NetWorkload):
     FLOP_PER_IMAGE = 2 * 962.7e9 + 2 * 10e9      # SURVEY 8d: two core forwards at 512x512 + the metric head (~1%)
     output_names = ("depth", "anaglyph")
     ATTN_KERNEL = "attention_wgmma_kernel<2> (fused softmax(QK^T + rel-pos bias)V of the BEiT-L-384 core at a 32x32 window, 64 forwards)"
-    FC1_KERNEL = "gemm_wgmma_kernel<128> (block MLP fc1: M=64*1025, N=4096, K=1024, GELU epilogue)"
+    FC1_KERNEL = "gemm_wgmma_kernel<64, 256> (persistent ping-pong, 64x256 tile per warpgroup; block MLP fc1: M=64*1025, N=4096, K=1024, GELU epilogue)"
 
     def _state_dict(self):
         from oracle import beit_dpt, synth_weights

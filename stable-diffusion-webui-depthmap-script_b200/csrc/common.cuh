@@ -39,6 +39,23 @@ struct PerDeviceFlag {
     }
 };
 
+// a device attribute read once per device ordinal (0 = not read yet; every attribute cached this way is positive)
+struct PerDeviceAttr {
+    int value[64] = {};
+    cudaDeviceAttr attr;
+    explicit PerDeviceAttr(cudaDeviceAttr a) : attr(a) {}
+    int get() {
+        int d = 0;
+        cudaGetDevice(&d);
+        int v = __atomic_load_n(&value[d & 63], __ATOMIC_ACQUIRE);
+        if (v == 0) {
+            cudaDeviceGetAttribute(&v, attr, d);
+            __atomic_store_n(&value[d & 63], v, __ATOMIC_RELEASE);
+        }
+        return v;
+    }
+};
+
 // order-preserving float <-> uint32 maps so min/max reductions can use integer atomics
 __device__ __forceinline__ uint32_t f32_to_ordered(float f) {
     uint32_t u = __float_as_uint(f);

@@ -5,15 +5,23 @@
 // the 3x3 stride-1 pad-1 convolutions of the DPT decoder (reference: dmidas/blocks.py, depth_anything_v2/util/blocks.py)
 // as implicit GEMM over NHWC activations: the 9 taps are 9 shifted TMA boxes, zero padding = TMA out-of-bounds fill.
 //
-// Structure (one 128 x BN output tile per CTA, three warpgroups):
-//   warpgroup 0   : TMA producer — one thread issues cp.async.bulk.tensor into a STAGES-deep ring of 128B-swizzled smem
-//                   tiles (mbarrier tx); the rest of the warpgroup exits the role branch at once
-//   warpgroups 1-2: consumers — each owns 64 of the 128 rows: wgmma.mma_async m64nBNk16 (fp16 operands from shared memory,
-//                   fp32 accumulators in registers), one commit group per k-block, the previous k-block's ring slot is
-//                   released once its group has retired; then the epilogue on the accumulator fragment: bias / GELU / ReLU /
-//                   LayerScale+residual / pixel-shuffle / fused 1x1 head, 8-byte (fp32) or 4-byte (fp16) accesses in which
-//                   the four lanes of a quad cover one 32- or 16-byte run of a row
-// Tiles of up to 64 columns keep two CTAs resident per SM, so one tile's epilogue overlaps another's main loop.
+// Structure (persistent, warp-specialised, ping-pong; one CTA of three warpgroups per SM):
+//   the grid is min(tiles, SMs); CTA b walks tiles b, b + grid, ... of one static order (launch_gemm: groups of m-tiles,
+//   n fastest inside a group, so the weight panels stay in L2 and each activation panel is read from HBM once)
+//   warpgroup 0   : TMA producer — drops to 40 registers (setmaxnreg); one thread issues cp.async.bulk.tensor for every
+//                   k-block of every tile of the CTA, in order, into one STAGES-deep ring of 128B-swizzled smem tiles
+//                   (mbarrier tx), running ahead across tile boundaries
+//   warpgroups 1-2: consumers — limit raised to 232 registers (the kernel builds in 168); each owns a whole BM x BN output tile and the two take alternate
+//                   tiles of the CTA's sequence (so alternate runs of the ring).  wgmma.mma_async m64nBNk16, BM / 64 per
+//                   16-wide k-slice (fp16 operands from shared memory, fp32 accumulators in registers), one commit group per
+//                   k-block, the previous k-block's ring slot released once its group has retired.  A pair of named
+//                   barriers makes the two main loops alternate: a warpgroup hands the tensor cores over as soon as its
+//                   last MMA is issued and runs its epilogue under the other's main loop.  The epilogue works on the
+//                   accumulator fragment: bias / GELU / ReLU / LayerScale+residual / pixel-shuffle / fused 1x1 head,
+//                   8-byte (fp32) or 4-byte (fp16) accesses in which the four lanes of a quad cover one 32- or 16-byte run
+//                   of a row
+// Every output element sums the same k-blocks and 16-wide k-slices in the same order whatever the tile shape or schedule,
+// so the results do not depend on either.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <math.h>
@@ -49,16 +57,20 @@ struct GemmParams {
     int ps_s, ps_cout, ps_h, ps_w;
     // implicit conv geometry (CONV): activations [B, H, W, Cin]; tile = hbox x wbox pixels
     int cB, cH, cW, cCin, hbox, wbox, tiles_x, tiles_y;
+    // static tile schedule (launch_gemm)
+    int m_tiles, n_tiles, group_m;
 };
 
-template <int BN>
+// BM x BN = the output tile of ONE consumer warpgroup.  The ring takes what the 227 KB of shared memory allows, up to 8
+// stages: 6 x 32 KB for 128 x 128, 5 x 40 KB for 64 x 256.
+template <int BM, int BN>
 struct GemmCfg {
-    static constexpr int BM = 128, BK = 64;
-    static constexpr int STAGES = 4;
+    static constexpr int BK = 64;
+    static constexpr int WM = BM / 64;                  // m64nBNk16 per k-slice
     static constexpr int A_BYTES = BM * BK * 2, B_BYTES = BN * BK * 2;
     static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+    static constexpr int STAGES = (220 * 1024) / STAGE_BYTES < 8 ? (220 * 1024) / STAGE_BYTES : 8;
     static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 256 /*barriers*/;   // base is __align__(1024)
-    static constexpr int CTAS_PER_SM = BN <= 64 ? 2 : 1;
 };
 constexpr int GEMM_THREADS = 384;
 
@@ -82,58 +94,82 @@ __device__ __forceinline__ float gelu_erf(float x) {
 }
 
 // Epilogue of one consumer thread: its accumulator fragment holds rows r0 = 16 * warp + lane / 4 and r0 + 8 of the
-// warpgroup's 64, and for every 8-column group j the columns 8j + 2 (lane % 4), +1 (tc_common.cuh).
-template <int BN>
+// warpgroup's 64, and for every 8-column group j the columns 8j + 2 (lane % 4), +1 (tc_common.cuh).  EPI = p.epi, fixed at
+// compile time so that a tile's epilogue is only the code of its own mode: the fully unrolled epilogue of all modes is
+// larger than the instruction cache and would otherwise be streamed through it under the other warpgroup's main loop.
+template <int BN, int EPI>
 __device__ __forceinline__ void epilogue_fragment(const GemmParams &p, const float (&acc)[BN / 2], const long long (&m)[2], const bool (&row_ok)[2],
                                                   int n_base, int lane) {
+    // Column groups are taken JC at a time: every operand load of a chunk is issued before its first store, so the loads
+    // of a chunk are in flight together instead of each waiting behind the previous group's store (X is read and written).
+    constexpr int JC = 2;
     const int t = lane & 3;
     float head_acc[2] = {0.f, 0.f};
 #pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-        const int n = n_base + 8 * j + 2 * t;
-        if (n >= p.N) continue;
-        float2 b2 = make_float2(0.f, 0.f);
-        if (p.bias) b2 = __ldg(reinterpret_cast<const float2 *>(p.bias + n));
+    for (int j0 = 0; j0 < BN / 8; j0 += JC) {
+        float2 b2[JC], g2[JC], x[JC][2];
+        __half2 rv[JC][2], rv2[JC][2];
 #pragma unroll
-        for (int r = 0; r < 2; ++r) {
-            if (!row_ok[r]) continue;
-            float v0 = acc[4 * j + 2 * r] + b2.x, v1 = acc[4 * j + 2 * r + 1] + b2.y;
-            if (p.epi == EPI_RESID_F32) {
-                float2 *xp = reinterpret_cast<float2 *>(p.X + m[r] * p.ldx + n);
-                const float2 g2 = __ldg(reinterpret_cast<const float2 *>(p.gamma + n));
-                float2 x = *xp;
-                x.x = fmaf(g2.x, v0, x.x); x.y = fmaf(g2.y, v1, x.y);
-                *xp = x;
-                continue;
+        for (int jj = 0; jj < JC; ++jj) {
+            const int n = n_base + 8 * (j0 + jj) + 2 * t;
+            b2[jj] = make_float2(0.f, 0.f);
+            g2[jj] = make_float2(0.f, 0.f);
+            if (n >= p.N) continue;
+            if (p.bias) b2[jj] = __ldg(reinterpret_cast<const float2 *>(p.bias + n));
+            if (EPI == EPI_RESID_F32 || EPI == EPI_HEAD) g2[jj] = __ldg(reinterpret_cast<const float2 *>(p.gamma + n));
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                if (!row_ok[r]) continue;
+                if (EPI == EPI_RESID_F32) x[jj][r] = *reinterpret_cast<const float2 *>(p.X + m[r] * p.ldx + n);
+                if (EPI == EPI_STORE_F16 || EPI == EPI_PIXSHUF) {
+                    if (p.R) rv[jj][r] = __ldg(reinterpret_cast<const __half2 *>(p.R + m[r] * p.ldr + n));
+                    if (p.R2) rv2[jj][r] = __ldg(reinterpret_cast<const __half2 *>(p.R2 + m[r] * p.ldr2 + n));
+                }
             }
-            if (p.epi == EPI_STORE_F32) {
-                *reinterpret_cast<float2 *>(p.X + m[r] * p.ldx + n) = make_float2(v0, v1);
-                continue;
-            }
-            if (p.act == ACT_GELU) { v0 = gelu_erf(v0); v1 = gelu_erf(v1); }
-            else if (p.act == ACT_RELU) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-            if (p.epi == EPI_HEAD) {
-                const float2 w2 = __ldg(reinterpret_cast<const float2 *>(p.gamma + n));
-                head_acc[r] = fmaf(v1, w2.y, fmaf(v0, w2.x, head_acc[r]));
-                continue;
-            }
-            if (p.R) { const float2 f = __half22float2(__ldg(reinterpret_cast<const __half2 *>(p.R + m[r] * p.ldr + n))); v0 += f.x; v1 += f.y; }
-            if (p.R2) { const float2 f = __half22float2(__ldg(reinterpret_cast<const __half2 *>(p.R2 + m[r] * p.ldr2 + n))); v0 += f.x; v1 += f.y; }
-            const __half2 h2 = __floats2half2_rn(v0, v1);
-            if (p.epi == EPI_PIXSHUF) {
-                const int s = p.ps_s, ij = n / p.ps_cout, co = n % p.ps_cout;
-                const int i = ij / s, jx = ij % s;
-                const long long bb = m[r] / ((long long)p.ps_h * p.ps_w);
-                const int rem = (int)(m[r] % ((long long)p.ps_h * p.ps_w));
-                const int y = rem / p.ps_w, x = rem % p.ps_w;
-                *reinterpret_cast<__half2 *>(p.C + (((bb * (p.ps_h * s) + (y * s + i)) * (long long)(p.ps_w * s)) + (x * s + jx)) * p.ps_cout + co) = h2;
-            } else {
-                *reinterpret_cast<__half2 *>(p.C + m[r] * p.ldc + n) = h2;
-                if (p.C2) *reinterpret_cast<__half2 *>(p.C2 + m[r] * p.ldc + n) = __hmax2(h2, __float2half2_rn(0.f));
+        }
+#pragma unroll
+        for (int jj = 0; jj < JC; ++jj) {
+            const int j = j0 + jj;
+            const int n = n_base + 8 * j + 2 * t;
+            if (n >= p.N) continue;
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                if (!row_ok[r]) continue;
+                float v0 = acc[4 * j + 2 * r] + b2[jj].x, v1 = acc[4 * j + 2 * r + 1] + b2[jj].y;
+                if (EPI == EPI_RESID_F32) {
+                    float2 xv = x[jj][r];
+                    xv.x = fmaf(g2[jj].x, v0, xv.x); xv.y = fmaf(g2[jj].y, v1, xv.y);
+                    *reinterpret_cast<float2 *>(p.X + m[r] * p.ldx + n) = xv;
+                    continue;
+                }
+                if (EPI == EPI_STORE_F32) {
+                    *reinterpret_cast<float2 *>(p.X + m[r] * p.ldx + n) = make_float2(v0, v1);
+                    continue;
+                }
+                if (p.act == ACT_GELU) { v0 = gelu_erf(v0); v1 = gelu_erf(v1); }
+                else if (p.act == ACT_RELU) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+                if (EPI == EPI_HEAD) {
+                    head_acc[r] = fmaf(v1, g2[jj].y, fmaf(v0, g2[jj].x, head_acc[r]));
+                    continue;
+                }
+                if (p.R) { const float2 f = __half22float2(rv[jj][r]); v0 += f.x; v1 += f.y; }
+                if (p.R2) { const float2 f = __half22float2(rv2[jj][r]); v0 += f.x; v1 += f.y; }
+                const __half2 h2 = __floats2half2_rn(v0, v1);
+                if (EPI == EPI_PIXSHUF) {
+                    const int s = p.ps_s, ij = n / p.ps_cout, co = n % p.ps_cout;
+                    const int i = ij / s, jx = ij % s;
+                    const long long bb = m[r] / ((long long)p.ps_h * p.ps_w);
+                    const int rem = (int)(m[r] % ((long long)p.ps_h * p.ps_w));
+                    const int y = rem / p.ps_w, xx = rem % p.ps_w;
+                    *reinterpret_cast<__half2 *>(p.C + (((bb * (p.ps_h * s) + (y * s + i)) * (long long)(p.ps_w * s)) + (xx * s + jx)) * p.ps_cout + co) = h2;
+                } else {
+                    *reinterpret_cast<__half2 *>(p.C + m[r] * p.ldc + n) = h2;
+                    if (p.C2) *reinterpret_cast<__half2 *>(p.C2 + m[r] * p.ldc + n) = __hmax2(h2, __float2half2_rn(0.f));
+                }
             }
         }
     }
-    if (p.epi == EPI_HEAD) {
+    if (EPI == EPI_HEAD) {
 #pragma unroll
         for (int r = 0; r < 2; ++r) {
             float s = head_acc[r];
@@ -144,97 +180,135 @@ __device__ __forceinline__ void epilogue_fragment(const GemmParams &p, const flo
     }
 }
 
-template <int BN, bool CONV>
-__global__ void __launch_bounds__(GEMM_THREADS, GemmCfg<BN>::CTAS_PER_SM) gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA,
-                                                                                          const __grid_constant__ CUtensorMap tmB, GemmParams p) {
-    using Cfg = GemmCfg<BN>;
+// tile t of the static schedule -> (m tile, n tile): groups of group_m m-tiles, n fastest inside a group (see launch_gemm)
+__device__ __forceinline__ void tile_coords(const GemmParams &p, int t, int &m_blk, int &n_blk) {
+    const int per_group = p.group_m * p.n_tiles;
+    const int g = t / per_group, r = t - g * per_group;
+    m_blk = g * p.group_m + r / p.n_tiles;
+    n_blk = r % p.n_tiles;
+}
+
+// implicit conv: m tile -> (image, top row, left column) of its hbox x wbox pixel box
+__device__ __forceinline__ void conv_origin(const GemmParams &p, int m_blk, int &cb, int &cy0, int &cx0) {
+    const int tiles_per_img = p.tiles_x * p.tiles_y;
+    cb = m_blk / tiles_per_img;
+    const int t = m_blk % tiles_per_img;
+    cy0 = (t / p.tiles_x) * p.hbox;
+    cx0 = (t % p.tiles_x) * p.wbox;
+}
+
+template <int BM, int BN, bool CONV>
+__global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA,
+                                                                     const __grid_constant__ CUtensorMap tmB, GemmParams p) {
+    using Cfg = GemmCfg<BM, BN>;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t *smem = smem_raw;
     uint64_t *full = reinterpret_cast<uint64_t *>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
     uint64_t *empty = full + Cfg::STAGES;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int m_blk = blockIdx.x, n_blk = blockIdx.y;
     const int num_kb = CONV ? 9 * (p.cCin / Cfg::BK) : p.K / Cfg::BK;
+    const int my_tiles = (p.m_tiles * p.n_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;   // grid <= tiles: >= 1
 
     if (threadIdx.x == 0) {
         prefetch_tmap(&tmA);
         prefetch_tmap(&tmB);
-        for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }   // 8 consumer warps
+        for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 4); }   // the 4 warps of one consumer
         fence_barrier_init();
     }
     __syncthreads();
 
-    // conv tile coordinates
-    int cb = 0, cy0 = 0, cx0 = 0;
-    if (CONV) {
-        const int tiles_per_img = p.tiles_x * p.tiles_y;
-        cb = m_blk / tiles_per_img;
-        const int t = m_blk % tiles_per_img;
-        cy0 = (t / p.tiles_x) * p.hbox;
-        cx0 = (t % p.tiles_x) * p.wbox;
-    }
-
     if (warp < 4) {
+        setmaxnreg_dec<40>();
         if (threadIdx.x == 0) {
+            // one ring across the CTA's whole tile sequence: tile i's k-blocks follow tile i-1's
             int stage = 0, phase = 0;
-            for (int kb = 0; kb < num_kb; ++kb) {
-                mbar_wait(&empty[stage], phase ^ 1);
-                uint8_t *sa = smem + stage * Cfg::STAGE_BYTES, *sb = sa + Cfg::A_BYTES;
-                mbar_arrive_expect_tx(&full[stage], Cfg::STAGE_BYTES);
-                if (CONV) {
-                    const int cblks = p.cCin / Cfg::BK;
-                    const int tap = kb / cblks, cblk = kb % cblks;
-                    const int dy = tap / 3 - 1, dx = tap % 3 - 1;
-                    tma_load_4d(sa, &tmA, &full[stage], cblk * Cfg::BK, cx0 + dx, cy0 + dy, cb);
-                } else {
-                    tma_load_2d(sa, &tmA, &full[stage], kb * Cfg::BK, m_blk * Cfg::BM);
+            for (int i = 0; i < my_tiles; ++i) {
+                int m_blk, n_blk, cb = 0, cy0 = 0, cx0 = 0;
+                tile_coords(p, blockIdx.x + i * gridDim.x, m_blk, n_blk);
+                if (CONV) conv_origin(p, m_blk, cb, cy0, cx0);
+                for (int kb = 0; kb < num_kb; ++kb) {
+                    mbar_wait(&empty[stage], phase ^ 1);
+                    uint8_t *sa = smem + stage * Cfg::STAGE_BYTES, *sb = sa + Cfg::A_BYTES;
+                    mbar_arrive_expect_tx(&full[stage], Cfg::STAGE_BYTES);
+                    if (CONV) {
+                        const int cblks = p.cCin / Cfg::BK;
+                        const int tap = kb / cblks, cblk = kb % cblks;
+                        const int dy = tap / 3 - 1, dx = tap % 3 - 1;
+                        tma_load_4d(sa, &tmA, &full[stage], cblk * Cfg::BK, cx0 + dx, cy0 + dy, cb);
+                    } else {
+                        tma_load_2d(sa, &tmA, &full[stage], kb * Cfg::BK, m_blk * BM);
+                    }
+                    tma_load_2d(sb, &tmB, &full[stage], kb * Cfg::BK, n_blk * BN);
+                    if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
                 }
-                tma_load_2d(sb, &tmB, &full[stage], kb * Cfg::BK, n_blk * BN);
-                if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
             }
         }
         return;
     }
 
-    // ===== consumers: warpgroup wg owns rows [64 wg, 64 wg + 64) of the tile =====
+    // ===== consumers: warpgroup wg takes tiles wg, wg + 2, ... of the CTA's sequence, each a whole BM x BN tile =====
+    setmaxnreg_inc<232>();
     const int wg = (warp >> 2) - 1;
-    float acc[BN / 2];
+    float acc[Cfg::WM][BN / 2];
+    for (int i = wg; i < my_tiles; i += 2) {
+        int m_blk, n_blk, cb = 0, cy0 = 0, cx0 = 0;
+        tile_coords(p, blockIdx.x + i * gridDim.x, m_blk, n_blk);
+        if (CONV) conv_origin(p, m_blk, cb, cy0, cx0);
+        const long long q0 = (long long)i * num_kb;              // ring position of the tile's first k-block
+        int stage = (int)(q0 % Cfg::STAGES), phase = (int)((q0 / Cfg::STAGES) & 1), prev = 0;
+        // ping-pong: the main loops of the two warpgroups alternate, so one's epilogue runs under the other's MMAs.  The
+        // alternation is also what makes the parity waits below sound: every ring position before q0 has already been
+        // waited for, so no full barrier is more than one phase behind this warpgroup's wait.
+        if (i > 0) named_bar_sync(1 + wg, 256);
+        for (int kb = 0; kb < num_kb; ++kb) {
+            mbar_wait(&full[stage], phase);
+            const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES), sb = sa + Cfg::A_BYTES;
+            const uint64_t bdesc = make_desc_kmajor_sw128(sb);
+            wgmma_fence();
 #pragma unroll
-    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-    int stage = 0, phase = 0, prev = 0;
-    for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full[stage], phase);
-        const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES) + wg * (64 * 128), sb = smem_u32(smem + stage * Cfg::STAGE_BYTES) + Cfg::A_BYTES;
-        const uint64_t adesc = make_desc_kmajor_sw128(sa), bdesc = make_desc_kmajor_sw128(sb);
-        wgmma_fence();
+            for (int k = 0; k < Cfg::BK / 16; ++k) {
 #pragma unroll
-        for (int k = 0; k < Cfg::BK / 16; ++k) wgmma_ss<BN>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (kb | k) != 0);
-        wgmma_commit();
-        if (kb > 0) {                       // the previous k-block's MMAs have retired: hand its slot back to the producer
-            wgmma_wait<1>();
-            if (lane == 0) mbar_arrive(&empty[prev]);
+                for (int h = 0; h < Cfg::WM; ++h)
+                    wgmma_ss<BN>(acc[h], make_desc_kmajor_sw128(sa + h * (64 * 128)) + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (kb | k) != 0);
+            }
+            wgmma_commit();
+            if (kb > 0) {                       // the previous k-block's MMAs have retired: hand its slot back to the producer
+                wgmma_wait<1>();
+                if (lane == 0) mbar_arrive(&empty[prev]);
+            }
+            prev = stage;
+            if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
         }
-        prev = stage;
-        if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
-    }
-    wgmma_wait<0>();
+        if (i + 1 < my_tiles) named_bar_arrive(2 - wg, 256);   // all MMAs issued: the other warpgroup's main loop may start
+        wgmma_wait<0>();
+        if (lane == 0) mbar_arrive(&empty[prev]);
 
-    long long m[2];
-    bool row_ok[2];
 #pragma unroll
-    for (int r = 0; r < 2; ++r) {
-        const int row = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * r;
-        if (CONV) {
-            const int y = cy0 + row / p.wbox, x = cx0 + row % p.wbox;
-            row_ok[r] = (y < p.cH) && (x < p.cW);
-            m[r] = ((long long)cb * p.cH + y) * p.cW + x;
-        } else {
-            m[r] = (long long)m_blk * Cfg::BM + row;
-            row_ok[r] = m[r] < p.M;
+        for (int h = 0; h < Cfg::WM; ++h) {
+            long long m[2];
+            bool row_ok[2];
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                const int row = h * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * r;
+                if (CONV) {
+                    const int y = cy0 + row / p.wbox, x = cx0 + row % p.wbox;
+                    row_ok[r] = (y < p.cH) && (x < p.cW);
+                    m[r] = ((long long)cb * p.cH + y) * p.cW + x;
+                } else {
+                    m[r] = (long long)m_blk * BM + row;
+                    row_ok[r] = m[r] < p.M;
+                }
+            }
+            switch (p.epi) {
+                case EPI_STORE_F16: epilogue_fragment<BN, EPI_STORE_F16>(p, acc[h], m, row_ok, n_blk * BN, lane); break;
+                case EPI_RESID_F32: epilogue_fragment<BN, EPI_RESID_F32>(p, acc[h], m, row_ok, n_blk * BN, lane); break;
+                case EPI_PIXSHUF: epilogue_fragment<BN, EPI_PIXSHUF>(p, acc[h], m, row_ok, n_blk * BN, lane); break;
+                case EPI_HEAD: epilogue_fragment<BN, EPI_HEAD>(p, acc[h], m, row_ok, n_blk * BN, lane); break;
+                case EPI_STORE_F32: epilogue_fragment<BN, EPI_STORE_F32>(p, acc[h], m, row_ok, n_blk * BN, lane); break;
+            }
         }
     }
-    epilogue_fragment<BN>(p, acc, m, row_ok, n_blk * BN, lane);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -283,14 +357,26 @@ int make_tmap_nhwc(CUtensorMap *tm, const void *ptr, uint64_t B, uint64_t H, uin
     return DM_OK;
 }
 
-template <int BN, bool CONV>
-static int launch_gemm(const CUtensorMap &tmA, const CUtensorMap &tmB, const GemmParams &p, int m_tiles, cudaStream_t stream) {
-    using Cfg = GemmCfg<BN>;
+// Tile order.  The CTAs running together cover about SMs consecutive tiles of the order.  With n fastest inside a group of
+// group_m m-tiles, those tiles share a few activation panels (A, 32-268 MB at the trunk's shapes) and sweep the weight matrix
+// (2-8 MB) across n; an activation panel is therefore read from HBM once and used for every n-tile while it is still in the
+// 50 MB L2, and the weights stay L2-resident for the whole call.  group_m bounds the activation panels of a group plus the
+// whole weight matrix by about half the L2 (the m fastest order re-read all of A once per weight panel).
+template <int BM, int BN, bool CONV>
+static int launch_gemm(const CUtensorMap &tmA, const CUtensorMap &tmB, GemmParams p, int m_tiles, cudaStream_t stream) {
+    using Cfg = GemmCfg<BM, BN>;
     static PerDeviceFlag configured;
+    static PerDeviceAttr sms(cudaDevAttrMultiProcessorCount);
     if (!configured.test_and_set())
-        DM_CUDA_CHECK(cudaFuncSetAttribute(gemm_wgmma_kernel<BN, CONV>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-    dim3 grid(m_tiles, (p.N + BN - 1) / BN);      // m fastest: the CTAs running together share one weight panel in L2
-    gemm_wgmma_kernel<BN, CONV><<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, p);
+        DM_CUDA_CHECK(cudaFuncSetAttribute(gemm_wgmma_kernel<BM, BN, CONV>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    const long long l2_budget = 24ll << 20, w_bytes = 2ll * p.N * p.K, a_panel = 2ll * BM * p.K;   // conv: K = 9 Cin over-counts
+    const long long g = (l2_budget - w_bytes) / a_panel;
+    p.m_tiles = m_tiles;
+    p.n_tiles = (p.N + BN - 1) / BN;
+    p.group_m = (int)(g < 1 ? 1 : (g > m_tiles ? m_tiles : g));
+    const int tiles = m_tiles * p.n_tiles;
+    const int grid = tiles < sms.get() ? tiles : sms.get();   // persistent: one CTA per SM, never more CTAs than tiles
+    gemm_wgmma_kernel<BM, BN, CONV><<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, p);
     DM_LAUNCH_CHECK("gemm_wgmma_kernel");
     return DM_OK;
 }
@@ -314,8 +400,16 @@ static int check_epilogue_operands(const GemmParams &p, const char *who) {
     return DM_OK;
 }
 
-// the fused head keeps a whole output row in one tile (BN = N = 32)
-static int pick_bn(const GemmParams &p) { return p.epi == EPI_HEAD ? 32 : (p.N % 128 == 0 ? 128 : (p.N % 64 == 0 ? 64 : 32)); }
+// N tile of one consumer warpgroup; its M tile is tile_m(bn).  The fused head keeps a whole output row in one tile
+// (BN = N = 32).  N % 256 == 0 takes 64 x 256 (m64n256k16: B is read from shared memory once per 256 columns instead of
+// twice), the rest 128 x 128, 128 x 64 or 128 x 32.  The two shapes give bit-identical results.  Their speed was compared
+// (tools/bench_gemm_micro.py, H100) only on an earlier build whose epilogue overflowed the instruction cache: 64 x 256 was
+// up to 7 % faster on qkv, 128 x 128 up to 12 % faster on the decoder's 3x3 convolutions; not re-measured since.
+static int pick_bn(const GemmParams &p) {
+    if (p.epi == EPI_HEAD) return 32;
+    return p.N % 256 == 0 ? 256 : (p.N % 128 == 0 ? 128 : (p.N % 64 == 0 ? 64 : 32));
+}
+static int tile_m(int bn) { return bn == 256 ? 64 : 128; }
 
 // Plain GEMM: A fp16 [M, K] (pitch lda), W fp16 [N, K] (pitch ldw)
 int gemm_f16(const __half *A, int lda, const __half *W, int ldw, GemmParams p, cudaStream_t stream) {
@@ -323,17 +417,18 @@ int gemm_f16(const __half *A, int lda, const __half *W, int ldw, GemmParams p, c
     if (p.epi == EPI_HEAD && p.N != 32) { set_error("gemm_f16: the fused head needs N = 32 (N=%d)", p.N); return DM_E_UNSUPPORTED; }
     if (int rc0 = check_epilogue_operands(p, "gemm_f16")) return rc0;
     if ((lda % 8) || (ldw % 8)) { set_error("gemm_f16: row pitches must be multiples of 8 elements"); return DM_E_INVALID; }
-    const int m_tiles = (p.M + 127) / 128;
-    const int bn = pick_bn(p);
+    const int bn = pick_bn(p), bm = tile_m(bn);
+    const int m_tiles = (p.M + bm - 1) / bm;
     CUtensorMap tmA, tmB;
-    int rc = make_tmap_2d(&tmA, A, (uint64_t)p.M, (uint64_t)p.K, (uint64_t)lda, 128, 64);
+    int rc = make_tmap_2d(&tmA, A, (uint64_t)p.M, (uint64_t)p.K, (uint64_t)lda, (uint32_t)bm, 64);
     if (rc) return rc;
     rc = make_tmap_2d(&tmB, W, (uint64_t)p.N, (uint64_t)p.K, (uint64_t)ldw, (uint32_t)bn, 64);
     if (rc) return rc;
     switch (bn) {
-        case 128: return launch_gemm<128, false>(tmA, tmB, p, m_tiles, stream);
-        case 64: return launch_gemm<64, false>(tmA, tmB, p, m_tiles, stream);
-        case 32: return launch_gemm<32, false>(tmA, tmB, p, m_tiles, stream);
+        case 256: return launch_gemm<64, 256, false>(tmA, tmB, p, m_tiles, stream);
+        case 128: return launch_gemm<128, 128, false>(tmA, tmB, p, m_tiles, stream);
+        case 64: return launch_gemm<128, 64, false>(tmA, tmB, p, m_tiles, stream);
+        case 32: return launch_gemm<128, 32, false>(tmA, tmB, p, m_tiles, stream);
     }
     set_error("gemm_f16: unsupported N tile %d", bn);
     return DM_E_UNSUPPORTED;
@@ -344,28 +439,29 @@ int conv3x3_f16(const __half *act, int B, int H, int W, int Cin, const __half *W
     if (Cin % 64 != 0 || p.N % 32 != 0) { set_error("conv3x3_f16: Cin must be a multiple of 64 and Cout of 32"); return DM_E_INVALID; }
     if (p.epi == EPI_HEAD && p.N != 32) { set_error("conv3x3_f16: the fused head needs Cout = 32 (Cout=%d)", p.N); return DM_E_UNSUPPORTED; }
     if (int rc0 = check_epilogue_operands(p, "conv3x3_f16")) return rc0;
-    // tile = hbox x wbox pixels = 128 rows; choose the wbox in {128,64,32,16,8} with the least padding waste
-    int best_w = 128; double best_eff = -1;
-    for (int wb = 128; wb >= 8; wb >>= 1) {
-        const int hb = 128 / wb;
+    const int bn = pick_bn(p), bm = tile_m(bn);
+    // tile = hbox x wbox pixels = bm rows; choose the wbox in {bm, .., 16, 8} with the least padding waste
+    int best_w = bm; double best_eff = -1;
+    for (int wb = bm; wb >= 8; wb >>= 1) {
+        const int hb = bm / wb;
         const double eff = (double)(W * H) / ((double)((W + wb - 1) / wb * wb) * ((H + hb - 1) / hb * hb));
         if (eff > best_eff + 1e-9) { best_eff = eff; best_w = wb; }
     }
-    p.wbox = best_w; p.hbox = 128 / best_w;
+    p.wbox = best_w; p.hbox = bm / best_w;
     p.tiles_x = (W + p.wbox - 1) / p.wbox; p.tiles_y = (H + p.hbox - 1) / p.hbox;
     p.cB = B; p.cH = H; p.cW = W; p.cCin = Cin;
     p.M = B * H * W; p.K = 9 * Cin;
     const int m_tiles = B * p.tiles_x * p.tiles_y;
-    const int bn = pick_bn(p);
     CUtensorMap tmA, tmB;
     int rc = make_tmap_nhwc(&tmA, act, B, H, W, Cin, p.hbox, p.wbox);
     if (rc) return rc;
     rc = make_tmap_2d(&tmB, Wt, (uint64_t)p.N, (uint64_t)p.K, (uint64_t)p.K, (uint32_t)bn, 64);
     if (rc) return rc;
     switch (bn) {
-        case 128: return launch_gemm<128, true>(tmA, tmB, p, m_tiles, stream);
-        case 64: return launch_gemm<64, true>(tmA, tmB, p, m_tiles, stream);
-        case 32: return launch_gemm<32, true>(tmA, tmB, p, m_tiles, stream);
+        case 256: return launch_gemm<64, 256, true>(tmA, tmB, p, m_tiles, stream);
+        case 128: return launch_gemm<128, 128, true>(tmA, tmB, p, m_tiles, stream);
+        case 64: return launch_gemm<128, 64, true>(tmA, tmB, p, m_tiles, stream);
+        case 32: return launch_gemm<128, 32, true>(tmA, tmB, p, m_tiles, stream);
     }
     set_error("conv3x3_f16: unsupported N tile %d", bn);
     return DM_E_UNSUPPORTED;
