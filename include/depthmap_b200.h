@@ -144,6 +144,13 @@ int dm_gemm_ex(const void *A, int lda, const void *W, int ldw, const dm_gemm_des
 /* 3x3 stride-1 pad-1 conv as implicit GEMM: act NHWC fp16 [B,H,W,Cin], Wt fp16 [Cout, 9*Cin] ordered (ky,kx,cin);
  * desc->N = Cout; M and K are derived. */
 int dm_conv3x3_ex(const void *act, int B, int H, int W, int Cin, const void *Wt, const dm_gemm_desc *desc_host, void *stream);
+/* Tiling mode (nn.Conv2d(padding_mode='circular')).  halo[b, y, x, :] = act[b, (y-1) mod H, (x-1) mod W, :]: fp16 NHWC
+ * [B, H+2, W+2, C], C % 8 == 0, both 16-byte aligned. */
+int dm_circular_halo_f16(const void *act, int B, int H, int W, int C, void *halo, void *stream);
+/* dm_conv3x3_ex with circular padding: dm_circular_halo_f16 into the caller's scratch `halo` (B*(H+2)*(W+2)*Cin fp16), then
+ * the implicit GEMM over it.  Two kernels. */
+int dm_conv3x3_circular_ex(const void *act, void *halo, int B, int H, int W, int Cin, const void *Wt, const dm_gemm_desc *desc_host,
+                           void *stream);
 /* convenience wrappers used by the unit tests */
 int dm_gemm_f16(const void *A, int lda, const void *W, int ldw, const float *bias, void *C, int ldc, int M, int N, int K,
                 int act, int out_f32, void *stream);
@@ -180,6 +187,8 @@ int dm_resize_bilinear_nhwc_f16(const void *in, int B, int Hin, int Win, int C, 
 /* mode 0: bilinear align_corners=True; mode 1: bicubic align_corners=False */
 int dm_resize_f32(const float *in, int B, int Hin, int Win, float *out, int Hout, int Wout, int mode, void *stream);
 int dm_im2col_s2_f16(const void *in, int B, int H, int W, int C, void *out, void *stream);
+/* dm_im2col_s2_f16 with circular padding (tiling mode) */
+int dm_im2col_s2_circular_f16(const void *in, int B, int H, int W, int C, void *out, void *stream);
 /* MiDaS ProjectReadout input: out[b*(N-1)+p, :] = [x[b,1+p,:], x[b,0,:]] (fp32 -> fp16), x fp32 [B, N, C] */
 int dm_concat_readout_f16(const float *x, int B, int N, int C, void *out, void *stream);
 
@@ -306,6 +315,9 @@ int dm_depth_forward(dm_model_t *model, const uint8_t *rgb, int B, int H, int W,
  * stem convolution: fp16 [B*Ho*Wo, 192], taps ordered (ky, kx, c), columns 147..191 zero */
 int dm_leres_stem_im2col(const uint8_t *rgb, int B, int H, int W, int net_h, int net_w, const float *mean_host, const float *std_host, void *out,
                          void *stream);
+/* the same with the stem's padding circular in network-input coordinates (tiling mode); likewise the two _f32 variants below */
+int dm_leres_stem_im2col_circular(const uint8_t *rgb, int B, int H, int W, int net_h, int net_w, const float *mean_host, const float *std_host,
+                                  void *out, void *stream);
 int dm_maxpool3x3s2_nhwc_f16(const void *in, int B, int H, int W, int C, void *out, void *stream);   /* kernel 3, stride 2, padding 1 */
 int dm_subsample2_nhwc_f16(const void *in, int B, int H, int W, int C, void *out, void *stream);     /* x[:, ::2, ::2, :] */
 int dm_add_f16(const void *a, const void *b, void *out, long long n, void *stream);
@@ -352,6 +364,10 @@ int dm_leres_stem_im2col_f32(const float *img /*[3,Hi,Wi]*/, int Hi, int Wi, int
 /* B crops of one planar image in one launch (BOOST batches its patches); rects: DEVICE int32 [B][4] = x0, y0, w, h */
 int dm_leres_stem_im2col_f32_batch(const float *img, int Hi, int Wi, const int *rects_dev, int B, int net_h, int net_w, const float *mean,
                                    const float *std, void *out, void *stream);
+int dm_leres_stem_im2col_f32_circular(const float *img, int Hi, int Wi, int x0, int y0, int w, int h, int net_h, int net_w, const float *mean,
+                                      const float *std, void *out, void *stream);
+int dm_leres_stem_im2col_f32_batch_circular(const float *img, int Hi, int Wi, const int *rects_dev, int B, int net_h, int net_w, const float *mean,
+                                            const float *std, void *out, void *stream);
 
 #ifdef __cplusplus
 }

@@ -84,6 +84,8 @@ EXPORTS = [
     "dm_boost_partials", "dm_unet_first_cols", "dm_unet_down_cols", "dm_unet_up_cols", "dm_unet_interleave", "dm_unet_final", "dm_unet_first", "dm_unet_last", "dm_sum_chunks_f32", "dm_boost_minmax",
     "dm_boost_merge_input", "dm_boost_post", "dm_boost_fit_sums", "dm_boost_blend", "dm_boost_resize_cubic", "dm_boost_u8_to_planar",
     "dm_leres_stem_im2col_f32", "dm_leres_stem_im2col_f32_batch", "dm_boost_minmax_normalise",
+    "dm_circular_halo_f16", "dm_conv3x3_circular_ex", "dm_im2col_s2_circular_f16", "dm_leres_stem_im2col_circular",
+    "dm_leres_stem_im2col_f32_circular", "dm_leres_stem_im2col_f32_batch_circular",
 ]
 
 
@@ -152,6 +154,8 @@ def _bind_optional(L):
         L.dm_conv3x3_f16.argtypes = [vp, i32, i32, i32, i32, vp, vp, vp, i32, i32, vp]
         L.dm_gemm_ex.argtypes = [vp, i32, vp, i32, c.POINTER(GemmDesc), vp]
         L.dm_conv3x3_ex.argtypes = [vp, i32, i32, i32, i32, vp, c.POINTER(GemmDesc), vp]
+        L.dm_circular_halo_f16.argtypes = [vp, i32, i32, i32, i32, vp, vp]
+        L.dm_conv3x3_circular_ex.argtypes = [vp, vp, i32, i32, i32, i32, vp, c.POINTER(GemmDesc), vp]
     if hasattr(L, "dm_attention_f16"):
         L.dm_attention_f16.argtypes = [vp, i32, i32, i32, f32, vp, i32, vp, vp]
         L.dm_attention_relpos_f16.argtypes = [vp, i32, i32, i32, i32, f32, vp, i32, vp, vp]
@@ -165,9 +169,11 @@ def _bind_optional(L):
         L.dm_resize_bilinear_nhwc_f16.argtypes = [vp, i32, i32, i32, i32, vp, i32, i32, vp]
         L.dm_resize_f32.argtypes = [vp, i32, i32, i32, vp, i32, i32, i32, vp]
         L.dm_im2col_s2_f16.argtypes = [vp, i32, i32, i32, i32, vp, vp]
+        L.dm_im2col_s2_circular_f16.argtypes = [vp, i32, i32, i32, i32, vp, vp]
         L.dm_concat_readout_f16.argtypes = [vp, i32, i32, i32, vp, vp]
     if hasattr(L, "dm_leres_stem_im2col"):
         L.dm_leres_stem_im2col.argtypes = [vp, i32, i32, i32, i32, i32, c.POINTER(c.c_float), c.POINTER(c.c_float), vp, vp]
+        L.dm_leres_stem_im2col_circular.argtypes = L.dm_leres_stem_im2col.argtypes
         L.dm_maxpool3x3s2_nhwc_f16.argtypes = [vp, i32, i32, i32, i32, vp, vp]
         L.dm_subsample2_nhwc_f16.argtypes = [vp, i32, i32, i32, i32, vp, vp]
         L.dm_add_f16.argtypes = [vp, vp, vp, c.c_longlong, vp]
@@ -192,6 +198,8 @@ def _bind_optional(L):
         L.dm_boost_u8_to_planar.argtypes = [vp, i32, i32, vp, vp]
         L.dm_leres_stem_im2col_f32.argtypes = [vp, i32, i32, i32, i32, i32, i32, i32, i32, c.POINTER(c.c_float), c.POINTER(c.c_float), vp, vp]
         L.dm_leres_stem_im2col_f32_batch.argtypes = [vp, i32, i32, vp, i32, i32, i32, c.POINTER(c.c_float), c.POINTER(c.c_float), vp, vp]
+        L.dm_leres_stem_im2col_f32_circular.argtypes = L.dm_leres_stem_im2col_f32.argtypes
+        L.dm_leres_stem_im2col_f32_batch_circular.argtypes = L.dm_leres_stem_im2col_f32_batch.argtypes
     if hasattr(L, "dm_zoe_clb_final"):
         L.dm_zoe_preprocess_patchify.argtypes = [vp, i32, i32, i32, i32, i32, i32, i32, i32, vp, i32, vp]
         L.dm_layernorm_post_f16.argtypes = [vp, c.c_longlong, i32, vp, vp, f32, vp, vp]
@@ -266,9 +274,15 @@ class Ops:
         self.call("dm_gemm_ex", A, lda, W, ldw, ctypes.byref(d))
 
     def conv3x3(self, act_t, B, H, W_, Cin, Wt, Cout, epi=EPI_STORE_F16, act=ACT_NONE, bias=None, C=None, C2=None,
-                R=None, R2=None, X=None, gamma=None, head_b2=0.0, ldx=1):
+                R=None, R2=None, X=None, gamma=None, head_b2=0.0, ldx=1, halo=None):
+        """pad-1 3x3 convolution; with a `halo` scratch tensor (at least B*(H+2)*(W_+2)*Cin fp16) the padding is circular"""
         d = _gemm_desc(0, Cout, 0, epi, act, bias, C, Cout, C2, R, Cout, R2, Cout, X, ldx, gamma, head_b2)
-        self.call("dm_conv3x3_ex", act_t, B, H, W_, Cin, Wt, ctypes.byref(d))
+        if halo is None:
+            self.call("dm_conv3x3_ex", act_t, B, H, W_, Cin, Wt, ctypes.byref(d))
+        else:
+            if halo.numel() < B * (H + 2) * (W_ + 2) * Cin:
+                raise ValueError(f"conv3x3: halo scratch of {halo.numel()} elements is too small for [{B}, {H + 2}, {W_ + 2}, {Cin}]")
+            self.call("dm_conv3x3_circular_ex", act_t, halo, B, H, W_, Cin, Wt, ctypes.byref(d), launches=2)
 
 
 class GraphCache:

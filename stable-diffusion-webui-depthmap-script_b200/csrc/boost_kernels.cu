@@ -450,7 +450,9 @@ __device__ __forceinline__ void stem_flush_rows_f32(const __half *s_rows, __half
     for (int i = threadIdx.x; i < (int)rows * 24; i += 256) dst[i] = src[i];
 }
 
-// rows assembled in shared memory and written with 16-byte stores (see leres_kernels.cu)
+// rows assembled in shared memory and written with 16-byte stores (see leres_kernels.cu).  CIRCULAR: the padding wraps around the
+// network input before the resize (leres_kernels.cu)
+template <bool CIRCULAR>
 __global__ void __launch_bounds__(256) leres_stem_im2col_f32_kernel(StemF32Params p) {
     __shared__ __align__(16) __half s_rows[32 * 192];
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -469,9 +471,9 @@ __global__ void __launch_bounds__(256) leres_stem_im2col_f32_kernel(StemF32Param
         }
         const bool identity = p.nh == p.h && p.nw == p.w;
         const float sy = (float)p.h / (float)p.nh, sx = (float)p.w / (float)p.nw;
-        const int iy = oy * 2 - 3 + ky;
+        const int iy = CIRCULAR ? wrap_index(oy * 2 - 3 + ky, p.nh) : oy * 2 - 3 + ky;
         for (int kx = 0; kx < 7; ++kx) {
-            const int ix = ox * 2 - 3 + kx;
+            const int ix = CIRCULAR ? wrap_index(ox * 2 - 3 + kx, p.nw) : ox * 2 - 3 + kx;
             float v[3] = {0.f, 0.f, 0.f};
             if (iy >= 0 && iy < p.nh && ix >= 0 && ix < p.nw) {
                 int y0 = iy, y1 = iy, x0 = ix, x1 = ix; float fy = 0.f, fx = 0.f;
@@ -631,33 +633,56 @@ DM_EXPORT int dm_boost_u8_to_planar(const uint8_t *rgb, int H, int W, float *out
     return DM_OK;
 }
 
-DM_EXPORT int dm_leres_stem_im2col_f32(const float *img, int Hi, int Wi, int x0, int y0, int w, int h, int net_h, int net_w, const float *mean_host,
-                                       const float *std_host, void *out, void *stream_) {
+template <bool CIRCULAR>
+static int leres_stem_im2col_f32(const char *who, const float *img, int Hi, int Wi, int x0, int y0, int w, int h, int net_h, int net_w,
+                                 const float *mean_host, const float *std_host, void *out, void *stream_) {
     using namespace dm;
-    if (!img || !out || x0 < 0 || y0 < 0 || w <= 0 || h <= 0 || x0 + w > Wi || y0 + h > Hi) { set_error("dm_leres_stem_im2col_f32: crop outside the image"); return DM_E_INVALID; }
+    if (!img || !out || x0 < 0 || y0 < 0 || w <= 0 || h <= 0 || x0 + w > Wi || y0 + h > Hi) { set_error("%s: crop outside the image", who); return DM_E_INVALID; }
     StemF32Params p;
     p.rects = nullptr; p.B = 1;
     p.img = img; p.plane = (long long)Hi * Wi; p.pitch = Wi; p.x0 = x0; p.y0 = y0; p.w = w; p.h = h; p.nh = net_h; p.nw = net_w;
     p.Ho = (net_h + 6 - 7) / 2 + 1; p.Wo = (net_w + 6 - 7) / 2 + 1;
     for (int c = 0; c < 3; ++c) { p.mean[c] = mean_host[c]; p.inv_std[c] = 1.0f / std_host[c]; }
     p.out = (__half *)out;
-    leres_stem_im2col_f32_kernel<<<GRID((long long)p.Ho * p.Wo * 8), 256, 0, (cudaStream_t)stream_>>>(p);
+    leres_stem_im2col_f32_kernel<CIRCULAR><<<GRID((long long)p.Ho * p.Wo * 8), 256, 0, (cudaStream_t)stream_>>>(p);
     DM_LAUNCH_CHECK("leres_stem_im2col_f32_kernel");
     return DM_OK;
 }
 
+DM_EXPORT int dm_leres_stem_im2col_f32(const float *img, int Hi, int Wi, int x0, int y0, int w, int h, int net_h, int net_w, const float *mean_host,
+                                       const float *std_host, void *out, void *stream_) {
+    return leres_stem_im2col_f32<false>("dm_leres_stem_im2col_f32", img, Hi, Wi, x0, y0, w, h, net_h, net_w, mean_host, std_host, out, stream_);
+}
+
+DM_EXPORT int dm_leres_stem_im2col_f32_circular(const float *img, int Hi, int Wi, int x0, int y0, int w, int h, int net_h, int net_w,
+                                                const float *mean_host, const float *std_host, void *out, void *stream_) {
+    return leres_stem_im2col_f32<true>("dm_leres_stem_im2col_f32_circular", img, Hi, Wi, x0, y0, w, h, net_h, net_w, mean_host, std_host, out, stream_);
+}
+
 /* B crops of the same planar image in one launch; rects: device int32 [B][4] = x0, y0, w, h (validated by the caller) */
-DM_EXPORT int dm_leres_stem_im2col_f32_batch(const float *img, int Hi, int Wi, const int *rects_dev, int B, int net_h, int net_w, const float *mean_host,
-                                             const float *std_host, void *out, void *stream_) {
+template <bool CIRCULAR>
+static int leres_stem_im2col_f32_batch(const char *who, const float *img, int Hi, int Wi, const int *rects_dev, int B, int net_h, int net_w,
+                                       const float *mean_host, const float *std_host, void *out, void *stream_) {
     using namespace dm;
-    if (!img || !out || !rects_dev || B <= 0) { set_error("dm_leres_stem_im2col_f32_batch: bad arguments"); return DM_E_INVALID; }
+    if (!img || !out || !rects_dev || B <= 0) { set_error("%s: bad arguments", who); return DM_E_INVALID; }
     StemF32Params p;
     p.rects = rects_dev; p.B = B;
     p.img = img; p.plane = (long long)Hi * Wi; p.pitch = Wi; p.x0 = 0; p.y0 = 0; p.w = Wi; p.h = Hi; p.nh = net_h; p.nw = net_w;
     p.Ho = (net_h + 6 - 7) / 2 + 1; p.Wo = (net_w + 6 - 7) / 2 + 1;
     for (int c = 0; c < 3; ++c) { p.mean[c] = mean_host[c]; p.inv_std[c] = 1.0f / std_host[c]; }
     p.out = (__half *)out;
-    leres_stem_im2col_f32_kernel<<<GRID((long long)B * p.Ho * p.Wo * 8), 256, 0, (cudaStream_t)stream_>>>(p);
+    leres_stem_im2col_f32_kernel<CIRCULAR><<<GRID((long long)B * p.Ho * p.Wo * 8), 256, 0, (cudaStream_t)stream_>>>(p);
     DM_LAUNCH_CHECK("leres_stem_im2col_f32_kernel");
     return DM_OK;
+}
+
+DM_EXPORT int dm_leres_stem_im2col_f32_batch(const float *img, int Hi, int Wi, const int *rects_dev, int B, int net_h, int net_w, const float *mean_host,
+                                             const float *std_host, void *out, void *stream_) {
+    return leres_stem_im2col_f32_batch<false>("dm_leres_stem_im2col_f32_batch", img, Hi, Wi, rects_dev, B, net_h, net_w, mean_host, std_host, out, stream_);
+}
+
+DM_EXPORT int dm_leres_stem_im2col_f32_batch_circular(const float *img, int Hi, int Wi, const int *rects_dev, int B, int net_h, int net_w,
+                                                      const float *mean_host, const float *std_host, void *out, void *stream_) {
+    return leres_stem_im2col_f32_batch<true>("dm_leres_stem_im2col_f32_batch_circular", img, Hi, Wi, rects_dev, B, net_h, net_w, mean_host, std_host, out,
+                                             stream_);
 }

@@ -56,6 +56,12 @@ struct PerDeviceAttr {
     }
 };
 
+// i mod n in [0, n) for any integer i (circular padding, n > 0)
+__host__ __device__ __forceinline__ int wrap_index(int i, int n) {
+    const int r = i % n;
+    return r < 0 ? r + n : r;
+}
+
 // order-preserving float <-> uint32 maps so min/max reductions can use integer atomics
 __device__ __forceinline__ uint32_t f32_to_ordered(float f) {
     uint32_t u = __float_as_uint(f);

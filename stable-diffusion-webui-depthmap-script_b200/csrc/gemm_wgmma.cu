@@ -4,6 +4,7 @@
 // the patch embedding, the DPT 1x1 convs, ConvTranspose k=s layers (GEMM + pixel-shuffle store) and, with CONV=true,
 // the 3x3 stride-1 pad-1 convolutions of the DPT decoder (reference: dmidas/blocks.py, depth_anything_v2/util/blocks.py)
 // as implicit GEMM over NHWC activations: the 9 taps are 9 shifted TMA boxes, zero padding = TMA out-of-bounds fill.
+// Circular padding (tiling mode) reads a copy of the activations with a one-pixel wrapped border instead (conv_halo_circular).
 //
 // Structure (persistent, warp-specialised, ping-pong; one CTA of three warpgroups per SM):
 //   the grid is min(tiles, SMs); CTA b walks tiles b, b + grid, ... of one static order (launch_gemm: groups of m-tiles,
@@ -59,6 +60,9 @@ struct GemmParams {
     int cB, cH, cW, cCin, hbox, wbox, tiles_x, tiles_y;
     // static tile schedule (launch_gemm)
     int m_tiles, n_tiles, group_m;
+    // implicit conv: tap offset into the tensor map, 0 = the activations themselves, 1 = their [B, H+2, W+2, Cin] halo copy (circular
+    // padding).  Last, so that the other fields keep their offsets and the plain GEMM kernels their code
+    int corg;
 };
 
 // BM x BN = the output tile of ONE consumer warpgroup.  The ring takes what the 227 KB of shared memory allows, up to 8
@@ -235,7 +239,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
                         const int cblks = p.cCin / Cfg::BK;
                         const int tap = kb / cblks, cblk = kb % cblks;
                         const int dy = tap / 3 - 1, dx = tap % 3 - 1;
-                        tma_load_4d(sa, &tmA, &full[stage], cblk * Cfg::BK, cx0 + dx, cy0 + dy, cb);
+                        tma_load_4d(sa, &tmA, &full[stage], cblk * Cfg::BK, cx0 + dx + p.corg, cy0 + dy + p.corg, cb);
                     } else {
                         tma_load_2d(sa, &tmA, &full[stage], kb * Cfg::BK, m_blk * BM);
                     }
@@ -434,11 +438,9 @@ int gemm_f16(const __half *A, int lda, const __half *W, int ldw, GemmParams p, c
     return DM_E_UNSUPPORTED;
 }
 
-// 3x3 stride-1 pad-1 convolution, NHWC fp16 activations [B,H,W,Cin], weights fp16 [Cout, 9*Cin] ordered (ky, kx, cin)
-int conv3x3_f16(const __half *act, int B, int H, int W, int Cin, const __half *Wt, GemmParams p, cudaStream_t stream) {
-    if (Cin % 64 != 0 || p.N % 32 != 0) { set_error("conv3x3_f16: Cin must be a multiple of 64 and Cout of 32"); return DM_E_INVALID; }
-    if (p.epi == EPI_HEAD && p.N != 32) { set_error("conv3x3_f16: the fused head needs Cout = 32 (Cout=%d)", p.N); return DM_E_UNSUPPORTED; }
-    if (int rc0 = check_epilogue_operands(p, "conv3x3_f16")) return rc0;
+// 3x3 stride-1 convolution, NHWC fp16 activations [B,H,W,Cin], weights fp16 [Cout, 9*Cin] ordered (ky, kx, cin).  halo = 0: pad 1
+// with zeros, `src` is the activations; halo = 1: `src` is their [B, H+2, W+2, Cin] copy with the padding already in its border.
+static int conv3x3_launch(const __half *src, int halo, int B, int H, int W, int Cin, const __half *Wt, GemmParams p, cudaStream_t stream) {
     const int bn = pick_bn(p), bm = tile_m(bn);
     // tile = hbox x wbox pixels = bm rows; choose the wbox in {bm, .., 16, 8} with the least padding waste
     int best_w = bm; double best_eff = -1;
@@ -449,11 +451,11 @@ int conv3x3_f16(const __half *act, int B, int H, int W, int Cin, const __half *W
     }
     p.wbox = best_w; p.hbox = bm / best_w;
     p.tiles_x = (W + p.wbox - 1) / p.wbox; p.tiles_y = (H + p.hbox - 1) / p.hbox;
-    p.cB = B; p.cH = H; p.cW = W; p.cCin = Cin;
+    p.cB = B; p.cH = H; p.cW = W; p.cCin = Cin; p.corg = halo;
     p.M = B * H * W; p.K = 9 * Cin;
     const int m_tiles = B * p.tiles_x * p.tiles_y;
     CUtensorMap tmA, tmB;
-    int rc = make_tmap_nhwc(&tmA, act, B, H, W, Cin, p.hbox, p.wbox);
+    int rc = make_tmap_nhwc(&tmA, src, B, H + 2 * halo, W + 2 * halo, Cin, p.hbox, p.wbox);
     if (rc) return rc;
     rc = make_tmap_2d(&tmB, Wt, (uint64_t)p.N, (uint64_t)p.K, (uint64_t)p.K, (uint32_t)bn, 64);
     if (rc) return rc;
@@ -465,6 +467,52 @@ int conv3x3_f16(const __half *act, int B, int H, int W, int Cin, const __half *W
     }
     set_error("conv3x3_f16: unsupported N tile %d", bn);
     return DM_E_UNSUPPORTED;
+}
+
+static int check_conv3x3(const GemmParams &p, int Cin, const char *who) {
+    if (Cin % 64 != 0 || p.N % 32 != 0) { set_error("%s: Cin must be a multiple of 64 and Cout of 32", who); return DM_E_INVALID; }
+    if (p.epi == EPI_HEAD && p.N != 32) { set_error("%s: the fused head needs Cout = 32 (Cout=%d)", who, p.N); return DM_E_UNSUPPORTED; }
+    return check_epilogue_operands(p, who);
+}
+
+int conv3x3_f16(const __half *act, int B, int H, int W, int Cin, const __half *Wt, GemmParams p, cudaStream_t stream) {
+    if (int rc = check_conv3x3(p, Cin, "conv3x3_f16")) return rc;
+    return conv3x3_launch(act, 0, B, H, W, Cin, Wt, p, stream);
+}
+
+// halo[b, y, x, :] = act[b, (y - 1) mod H, (x - 1) mod W, :] for y < H + 2, x < W + 2: what F.pad(mode='circular') gives a 3x3
+// pad-1 convolution.  One thread per 8 channels of a halo pixel; C % 8 == 0.
+__global__ void __launch_bounds__(256) conv_halo_circular_kernel(const __half *__restrict__ act, int B, int H, int W, int C, __half *__restrict__ halo) {
+    const int c8 = C / 8;
+    const long long total = (long long)B * (H + 2) * (W + 2) * c8;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        const int c = (int)(i % c8) * 8;
+        long long r = i / c8;
+        const int x = (int)(r % (W + 2));
+        r /= W + 2;
+        const int y = (int)(r % (H + 2));
+        const long long b = r / (H + 2);
+        const int sy = wrap_index(y - 1, H), sx = wrap_index(x - 1, W);
+        reinterpret_cast<uint4 *>(halo)[i] = __ldg(reinterpret_cast<const uint4 *>(act + ((b * H + sy) * W + sx) * C + c));
+    }
+}
+
+int conv_halo_circular(const __half *act, int B, int H, int W, int C, __half *halo, cudaStream_t stream) {
+    if (!act || !halo || B <= 0 || H <= 0 || W <= 0 || C <= 0 || C % 8) { set_error("dm_circular_halo_f16: bad arguments (C must be a positive multiple of 8)"); return DM_E_INVALID; }
+    if ((reinterpret_cast<uintptr_t>(act) | reinterpret_cast<uintptr_t>(halo)) % 16) { set_error("dm_circular_halo_f16: tensors must be 16-byte aligned"); return DM_E_INVALID; }
+    static PerDeviceAttr sms(cudaDevAttrMultiProcessorCount);
+    const long long total = (long long)B * (H + 2) * (W + 2) * (C / 8);
+    const long long blocks = (total + 255) / 256, cap = 16ll * sms.get();
+    conv_halo_circular_kernel<<<(unsigned)(blocks < cap ? blocks : cap), 256, 0, stream>>>(act, B, H, W, C, halo);
+    DM_LAUNCH_CHECK("conv_halo_circular_kernel");
+    return DM_OK;
+}
+
+// 3x3 stride-1 convolution with circular padding (nn.Conv2d(padding_mode='circular')): the halo copy, then the implicit GEMM on it
+int conv3x3_circular_f16(const __half *act, __half *halo, int B, int H, int W, int Cin, const __half *Wt, GemmParams p, cudaStream_t stream) {
+    if (int rc = check_conv3x3(p, Cin, "conv3x3_circular")) return rc;
+    if (int rc = conv_halo_circular(act, B, H, W, Cin, halo, stream)) return rc;
+    return conv3x3_launch(halo, 1, B, H, W, Cin, Wt, p, stream);
 }
 
 }  // namespace dm
@@ -511,5 +559,17 @@ extern "C" __attribute__((visibility("default"))) int dm_conv3x3_ex(const void *
     dm::GemmParams p;
     desc_to_params(d, p);
     return dm::conv3x3_f16((const __half *)act, B, H, W, Cin, (const __half *)Wt, p, (cudaStream_t)stream);
+}
+
+extern "C" __attribute__((visibility("default"))) int dm_circular_halo_f16(const void *act, int B, int H, int W, int C, void *halo, void *stream) {
+    return dm::conv_halo_circular((const __half *)act, B, H, W, C, (__half *)halo, (cudaStream_t)stream);
+}
+
+extern "C" __attribute__((visibility("default"))) int dm_conv3x3_circular_ex(const void *act, void *halo, int B, int H, int W, int Cin, const void *Wt,
+                                                                          const dm_gemm_desc *d, void *stream) {
+    if (!act || !halo || !Wt || !d) { dm::set_error("dm_conv3x3_circular_ex: null argument"); return DM_E_INVALID; }
+    dm::GemmParams p;
+    desc_to_params(d, p);
+    return dm::conv3x3_circular_f16((const __half *)act, (__half *)halo, B, H, W, Cin, (const __half *)Wt, p, (cudaStream_t)stream);
 }
 

@@ -42,6 +42,9 @@ __device__ __forceinline__ void stem_flush_rows(const __half *s_rows, __half *ou
     for (int i = threadIdx.x; i < (int)rows * 24; i += 256) dst[i] = src[i];
 }
 
+// CIRCULAR: the stem convolution's padding wraps around the network input (nn.Conv2d(padding_mode='circular')): a tap outside the
+// net_h x net_w image samples the pixel net_h (net_w) rows (columns) away, before the resize maps it to the source
+template <bool CIRCULAR>
 __global__ void __launch_bounds__(256) leres_stem_im2col_kernel(StemParams p) {
     // one thread per (output pixel, ky): 7 kx taps x 3 channels = 21 values; thread ky == 7 zero-fills the 45 padding columns
     __shared__ __align__(16) __half s_rows[32 * 192];
@@ -58,9 +61,9 @@ __global__ void __launch_bounds__(256) leres_stem_im2col_kernel(StemParams p) {
         const uint8_t *img = p.rgb + (long long)b * p.H * p.W * 3;
         const bool identity = p.nh == p.H && p.nw == p.W;           // cv2.resize to the same size is a copy
         const float sy = (float)p.H / (float)p.nh, sx = (float)p.W / (float)p.nw;
-        const int iy = oy * 2 - 3 + ky;
+        const int iy = CIRCULAR ? wrap_index(oy * 2 - 3 + ky, p.nh) : oy * 2 - 3 + ky;
         for (int kx = 0; kx < 7; ++kx) {
-            const int ix = ox * 2 - 3 + kx;
+            const int ix = CIRCULAR ? wrap_index(ox * 2 - 3 + kx, p.nw) : ox * 2 - 3 + kx;
             float v[3] = {0.f, 0.f, 0.f};
             if (iy >= 0 && iy < p.nh && ix >= 0 && ix < p.nw) {
                 if (identity) {
@@ -144,19 +147,30 @@ __global__ void __launch_bounds__(256) add_f16_kernel(const __half *__restrict__
 
 #define DM_EXPORT extern "C" __attribute__((visibility("default")))
 
-DM_EXPORT int dm_leres_stem_im2col(const uint8_t *rgb, int B, int H, int W, int net_h, int net_w, const float *mean_host, const float *std_host,
-                                   void *out, void *stream_) {
+template <bool CIRCULAR>
+static int leres_stem_im2col(const char *who, const uint8_t *rgb, int B, int H, int W, int net_h, int net_w, const float *mean_host,
+                             const float *std_host, void *out, void *stream_) {
     using namespace dm;
-    if (!rgb || !out || B <= 0 || net_h <= 0 || net_w <= 0) { set_error("dm_leres_stem_im2col: bad arguments"); return DM_E_INVALID; }
+    if (!rgb || !out || B <= 0 || net_h <= 0 || net_w <= 0) { set_error("%s: bad arguments", who); return DM_E_INVALID; }
     StemParams p;
     p.rgb = rgb; p.B = B; p.H = H; p.W = W; p.nh = net_h; p.nw = net_w;
     p.Ho = (net_h + 6 - 7) / 2 + 1; p.Wo = (net_w + 6 - 7) / 2 + 1;
     for (int c = 0; c < 3; ++c) { p.mean[c] = mean_host[c]; p.inv_std[c] = 1.0f / std_host[c]; }
     p.out = (__half *)out;
     const long long total = (long long)B * p.Ho * p.Wo * 8;
-    leres_stem_im2col_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream_>>>(p);
+    leres_stem_im2col_kernel<CIRCULAR><<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream_>>>(p);
     DM_LAUNCH_CHECK("leres_stem_im2col_kernel");
     return DM_OK;
+}
+
+DM_EXPORT int dm_leres_stem_im2col(const uint8_t *rgb, int B, int H, int W, int net_h, int net_w, const float *mean_host, const float *std_host,
+                                   void *out, void *stream_) {
+    return leres_stem_im2col<false>("dm_leres_stem_im2col", rgb, B, H, W, net_h, net_w, mean_host, std_host, out, stream_);
+}
+
+DM_EXPORT int dm_leres_stem_im2col_circular(const uint8_t *rgb, int B, int H, int W, int net_h, int net_w, const float *mean_host,
+                                            const float *std_host, void *out, void *stream_) {
+    return leres_stem_im2col<true>("dm_leres_stem_im2col_circular", rgb, B, H, W, net_h, net_w, mean_host, std_host, out, stream_);
 }
 
 DM_EXPORT int dm_maxpool3x3s2_nhwc_f16(const void *in, int B, int H, int W, int C, void *out, void *stream_) {

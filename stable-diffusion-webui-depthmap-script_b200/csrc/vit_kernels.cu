@@ -289,7 +289,9 @@ __global__ void __launch_bounds__(256) resize_f32_kernel(const float *__restrict
     }
 }
 
-// im2col for a 3x3 stride-2 pad-1 convolution on NHWC fp16: out [B*Ho*Wo, 9*C] ordered (ky, kx, c)
+// im2col for a 3x3 stride-2 pad-1 convolution on NHWC fp16: out [B*Ho*Wo, 9*C] ordered (ky, kx, c).  CIRCULAR: the padding
+// wraps around (nn.Conv2d(padding_mode='circular')) instead of being zeros
+template <bool CIRCULAR>
 __global__ void __launch_bounds__(256) im2col_s2_kernel(const __half *__restrict__ in, int B, int H, int W, int C, __half *__restrict__ out, int Ho, int Wo) {
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     const int c8 = C / 8;
@@ -303,7 +305,8 @@ __global__ void __launch_bounds__(256) im2col_s2_kernel(const __half *__restrict
     r /= Wo;
     const int yo = (int)(r % Ho);
     const int b = (int)(r / Ho);
-    const int y = yo * 2 - 1 + tap / 3, x = xo * 2 - 1 + tap % 3;
+    int y = yo * 2 - 1 + tap / 3, x = xo * 2 - 1 + tap % 3;
+    if (CIRCULAR) { y = wrap_index(y, H); x = wrap_index(x, W); }
     uint4 v = make_uint4(0, 0, 0, 0);
     if (y >= 0 && y < H && x >= 0 && x < W) v = __ldg(reinterpret_cast<const uint4 *>(in + (((long long)b * H + y) * W + x) * C + c));
     *reinterpret_cast<uint4 *>(out + ((((long long)b * Ho + yo) * Wo + xo) * 9 + tap) * C + c) = v;
@@ -441,7 +444,17 @@ DM_EXPORT int dm_im2col_s2_f16(const void *in, int B, int H, int W, int C, void 
     if (C % 8) { set_error("dm_im2col_s2_f16: C must be a multiple of 8"); return DM_E_INVALID; }
     const int Ho = (H + 2 - 3) / 2 + 1, Wo = (W + 2 - 3) / 2 + 1;
     const long long total = (long long)B * Ho * Wo * 9 * (C / 8);
-    im2col_s2_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream_>>>((const __half *)in, B, H, W, C, (__half *)out, Ho, Wo);
+    im2col_s2_kernel<false><<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream_>>>((const __half *)in, B, H, W, C, (__half *)out, Ho, Wo);
+    DM_LAUNCH_CHECK("im2col_s2_kernel");
+    return DM_OK;
+}
+
+DM_EXPORT int dm_im2col_s2_circular_f16(const void *in, int B, int H, int W, int C, void *out, void *stream_) {
+    using namespace dm;
+    if (!in || !out || B <= 0 || H <= 0 || W <= 0 || C <= 0 || C % 8) { set_error("dm_im2col_s2_circular_f16: bad arguments (C must be a positive multiple of 8)"); return DM_E_INVALID; }
+    const int Ho = (H + 2 - 3) / 2 + 1, Wo = (W + 2 - 3) / 2 + 1;
+    const long long total = (long long)B * Ho * Wo * 9 * (C / 8);
+    im2col_s2_kernel<true><<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream_>>>((const __half *)in, B, H, W, C, (__half *)out, Ho, Wo);
     DM_LAUNCH_CHECK("im2col_s2_kernel");
     return DM_OK;
 }

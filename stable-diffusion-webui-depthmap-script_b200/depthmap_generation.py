@@ -11,6 +11,8 @@ Implemented model types: 0 (LeReS res101), 1, 2 (MiDaS 3.1 DPT-BEiT-L 512 / 384)
 (ZoeDepth-N, -K, -NK) and 12, 13, 14 (Depth-Anything-V2 S/B/L).  Others raise NotImplementedError naming the type.
 Weights: a state_dict in the upstream checkpoint layout (``depth_anything_v2_vit{s,b,l}.pth``), packed once at load
 into the kernels' layout (fp16 GEMM operands, (ky,kx,cin)-ordered conv filters, ConvTranspose as GEMM + pixel shuffle).
+Tiling mode (``tiling_mode``, src/depthmap_generation.py:251-260) makes every padded Conv2d of the depth network pad
+circularly: the engines' ``circular=True`` runs those convolutions through the circular conv / im2col / stem entry points.
 """
 from __future__ import annotations
 
@@ -77,7 +79,9 @@ class DepthAnythingV2Engine:
     Mirrors DepthAnythingV2.forward / DPTHead.forward / DINOv2.get_intermediate_layers of the reference
     (ddepth_anything_v2/depth_anything_v2/dpt.py:117-184, dinov2.py:297-321) plus image2tensor (dpt.py:196-221) and the
     final resize of estimatedepthanything_v2 (src/depthmap_generation.py:548-559).  Also the base of DptBeitEngine: the
-    two families share the ViT block sequence and the whole DPT decoder and differ only in the hooks below."""
+    two families share the ViT block sequence and the whole DPT decoder and differ only in the hooks below.
+    circular=True: tiling mode, every padded convolution (the decoder's 3x3 convs and the reassemble stage's stride-2 one) pads
+    circularly."""
 
     PATCH = 14
     MEAN = (0.485, 0.456, 0.406)
@@ -88,11 +92,12 @@ class DepthAnythingV2Engine:
     FINAL_RESIZE_MODE = 0  # bilinear, align_corners=True (src/depthmap_generation.py:558)
     CONFIGS = DAV2_CONFIGS
 
-    def __init__(self, state_dict, encoder, device):
+    def __init__(self, state_dict, encoder, device, circular=False):
         import torch
         self.cfg = self.CONFIGS[encoder]
         self.encoder = encoder
         self.device = device
+        self.circular = circular
         self.ops = _lib.Ops()
         self._buf_key = None
         self._bufs = {}
@@ -227,6 +232,9 @@ class DepthAnythingV2Engine:
         b['oc1'] = h16(B, up[3][0], up[3][1], self.F2p)
         b['oc1u'] = h16(B, nh, nw, self.F2p)
         b['d'] = torch.empty(B, nh, nw, dtype=torch.float32, device=dev)
+        # circular padding: the halo copy of a 3x3 convolution's input, sized for the largest one
+        convs = [(s, c) for s, c in zip(sizes, self.ocp)] + [(s, Fp) for s in sizes] + [(up[3], Fp), ((nh, nw), self.F2p)]
+        b['halo'] = h16(max(B * (h + 2) * (w + 2) * c for (h, w), c in convs)) if self.circular else None
         self._bufs, self._buf_key = b, key
         return b
 
@@ -287,18 +295,18 @@ class DepthAnythingV2Engine:
         ops.gemm(b['p'][1], self.ocp[1], w['up1_w'], self.ocp[1], B * Np, 4 * self.ocp[1], self.ocp[1], epi=_lib.EPI_PIXSHUF, bias=w['up1_b'],
                  C=b['r'][1], ps=(2, self.ocp[1], gh, gw))
         r2 = b['p'][2]
-        ops.call("dm_im2col_s2_f16", b['p'][3], B, gh, gw, self.ocp[3], b['cols3'])
+        ops.call("dm_im2col_s2_circular_f16" if self.circular else "dm_im2col_s2_f16", b['p'][3], B, gh, gw, self.ocp[3], b['cols3'])
         ops.gemm(b['cols3'], 9 * self.ocp[3], w['down3_w'], 9 * self.ocp[3], B * sizes[3][0] * sizes[3][1], self.ocp[3], 9 * self.ocp[3],
                  bias=w['down3_b'], C=b['r'][3], ldc=self.ocp[3])
         rs = [b['r'][0], b['r'][1], r2, b['r'][3]]
         for i in range(4):  # layer{i}_rn (no bias) -> l_i and relu(l_i)
-            ops.conv3x3(rs[i], B, sizes[i][0], sizes[i][1], self.ocp[i], w[f'rn{i}_w'], Fp, C=b['l'][i], C2=b['lr'][i])
+            ops.conv3x3(rs[i], B, sizes[i][0], sizes[i][1], self.ocp[i], w[f'rn{i}_w'], Fp, C=b['l'][i], C2=b['lr'][i], halo=b['halo'])
         # refinenet4: resConfUnit2(l4) -> resize -> out_conv.  The 1x1 out_conv (+ bias) commutes with the bilinear
         # interpolation (a per-pixel channel mix against per-channel spatial weights that sum to one), so it runs BEFORE the
         # up-sample: a quarter of the MACs and no full-resolution intermediate (dmidas/blocks.py:425-437 has it after).
         s3 = sizes[3]
-        ops.conv3x3(b['lr'][3], B, s3[0], s3[1], Fp, w['rf4_u2c1_w'], Fp, act=_lib.ACT_RELU, bias=w['rf4_u2c1_b'], C=b['t3'])
-        ops.conv3x3(b['t3'], B, s3[0], s3[1], Fp, w['rf4_u2c2_w'], Fp, bias=w['rf4_u2c2_b'], C=b['u3'], R=b['l'][3])
+        ops.conv3x3(b['lr'][3], B, s3[0], s3[1], Fp, w['rf4_u2c1_w'], Fp, act=_lib.ACT_RELU, bias=w['rf4_u2c1_b'], C=b['t3'], halo=b['halo'])
+        ops.conv3x3(b['t3'], B, s3[0], s3[1], Fp, w['rf4_u2c2_w'], Fp, bias=w['rf4_u2c2_b'], C=b['u3'], R=b['l'][3], halo=b['halo'])
         up = b['up_sizes']
         ops.gemm(b['u3'], Fp, w['rf4_out_w'], Fp, B * s3[0] * s3[1], Fp, Fp, bias=w['rf4_out_b'], C=b['v'][0], ldc=Fp)
         ops.call("dm_resize_bilinear_nhwc_f16", b['v'][0], B, s3[0], s3[1], Fp, b['path'][0], up[0][0], up[0][1])
@@ -306,11 +314,13 @@ class DepthAnythingV2Engine:
         for step, (li, rf) in enumerate(((2, 3), (1, 2), (0, 1))):
             s = sizes[li]
             path = b['path'][step]
-            ops.conv3x3(b['lr'][li], B, s[0], s[1], Fp, w[f'rf{rf}_u1c1_w'], Fp, act=_lib.ACT_RELU, bias=w[f'rf{rf}_u1c1_b'], C=b[f't{li}'])
+            ops.conv3x3(b['lr'][li], B, s[0], s[1], Fp, w[f'rf{rf}_u1c1_w'], Fp, act=_lib.ACT_RELU, bias=w[f'rf{rf}_u1c1_b'], C=b[f't{li}'],
+                        halo=b['halo'])
             ops.conv3x3(b[f't{li}'], B, s[0], s[1], Fp, w[f'rf{rf}_u1c2_w'], Fp, bias=w[f'rf{rf}_u1c2_b'], C=b[f'o{li}'], C2=b[f'or{li}'],
-                        R=b['l'][li], R2=path)
-            ops.conv3x3(b[f'or{li}'], B, s[0], s[1], Fp, w[f'rf{rf}_u2c1_w'], Fp, act=_lib.ACT_RELU, bias=w[f'rf{rf}_u2c1_b'], C=b[f't{li}'])
-            ops.conv3x3(b[f't{li}'], B, s[0], s[1], Fp, w[f'rf{rf}_u2c2_w'], Fp, bias=w[f'rf{rf}_u2c2_b'], C=b[f'u{li}'], R=b[f'o{li}'])
+                        R=b['l'][li], R2=path, halo=b['halo'])
+            ops.conv3x3(b[f'or{li}'], B, s[0], s[1], Fp, w[f'rf{rf}_u2c1_w'], Fp, act=_lib.ACT_RELU, bias=w[f'rf{rf}_u2c1_b'], C=b[f't{li}'],
+                        halo=b['halo'])
+            ops.conv3x3(b[f't{li}'], B, s[0], s[1], Fp, w[f'rf{rf}_u2c2_w'], Fp, bias=w[f'rf{rf}_u2c2_b'], C=b[f'u{li}'], R=b[f'o{li}'], halo=b['halo'])
             t = up[step + 1]
             ops.gemm(b[f'u{li}'], Fp, w[f'rf{rf}_out_w'], Fp, B * s[0] * s[1], Fp, Fp, bias=w[f'rf{rf}_out_b'], C=b['v'][step + 1], ldc=Fp)
             ops.call("dm_resize_bilinear_nhwc_f16", b['v'][step + 1], B, s[0], s[1], Fp, b['path'][step + 1], t[0], t[1])
@@ -322,11 +332,11 @@ class DepthAnythingV2Engine:
         ops, w = self.ops, self.w
         Fp = self.Fp
         t = b['up_sizes'][3]
-        ops.conv3x3(b['path'][3], B, t[0], t[1], Fp, w['oc1_w'], self.F2p, bias=w['oc1_b'], C=b['oc1'])
+        ops.conv3x3(b['path'][3], B, t[0], t[1], Fp, w['oc1_w'], self.F2p, bias=w['oc1_b'], C=b['oc1'], halo=b['halo'])
         ops.call("dm_resize_bilinear_nhwc_f16", b['oc1'], B, t[0], t[1], self.F2p, b['oc1u'], nh, nw)
         # conv3x3 -> ReLU -> conv1x1 -> ReLU (+ the outer F.relu, idempotent) fused into one epilogue
         ops.conv3x3(b['oc1u'], B, nh, nw, self.F2p, w['oc2_w'], 32, epi=_lib.EPI_HEAD, act=_lib.ACT_RELU, bias=w['oc2_b'], X=b['d'],
-                    gamma=w['oc3_w'], head_b2=self.oc3_b)
+                    gamma=w['oc3_w'], head_b2=self.oc3_b, halo=b['halo'])
         if not resize:
             return b['d']
         oh, ow = out_hw if out_hw is not None else (H, W)
@@ -565,7 +575,8 @@ class LeresEngine:
     NHWC fp16 activations, fp32 accumulation.  1x1 convolutions are GEMMs, 3x3 ones the implicit-GEMM conv; the 32-group 3x3
     convolutions use block-diagonal dense filters (exact: the extra products are zeros), the three stride-2 ones go through the
     strided im2col; BatchNorm (running statistics, eps 1e-5) is folded into filters and biases when the checkpoint is packed; the
-    bottleneck's `relu(out + identity)` and FTB's `relu(x + branch)` come out of the GEMM epilogue's relu copy (C2)."""
+    bottleneck's `relu(out + identity)` and FTB's `relu(x + branch)` come out of the GEMM epilogue's relu copy (C2).
+    circular=True: tiling mode, the stem, every 3x3 convolution of the encoder and the decoder pad circularly."""
 
     LAYERS = (3, 4, 23, 3)
     GROUPS = 32
@@ -574,8 +585,10 @@ class LeresEngine:
     MEAN = (0.485, 0.456, 0.406)
     STD = (0.229, 0.224, 0.225)
 
-    def __init__(self, state_dict, device):
+    def __init__(self, state_dict, device, circular=False):
         self.device = device
+        self.circular = circular
+        self._cv = "_circular" if circular else ""      # entry-point suffix of the circular stem / im2col
         self.ops = _lib.Ops()
         self._bufs = {}
         # from the second call on at a given (B, net size) the ~500 launches of the network replay from a CUDA graph
@@ -705,9 +718,9 @@ class LeresEngine:
         m = (ctypes.c_float * 3)(*self.MEAN)
         s = (ctypes.c_float * 3)(*self.STD)
         if planar is None:
-            self.ops.call("dm_leres_stem_im2col", rgb, B, H, W, net_h, net_w, m, s, cols)
+            self.ops.call("dm_leres_stem_im2col" + self._cv, rgb, B, H, W, net_h, net_w, m, s, cols)
         else:
-            self.ops.call("dm_leres_stem_im2col_f32", pl_img, pl_hi, pl_wi, rect[0], rect[1], rect[2], rect[3], net_h, net_w, m, s, cols)
+            self.ops.call("dm_leres_stem_im2col_f32" + self._cv, pl_img, pl_hi, pl_wi, rect[0], rect[1], rect[2], rect[3], net_h, net_w, m, s, cols)
         dn = self._network(B, net_h, net_w, cols)
         hh, ww = net_h // 2, net_w // 2
         oh, ow = out_hw if out_hw is not None else (H, W)
@@ -736,13 +749,16 @@ class LeresEngine:
         cols = self._buf('stem_cols', (B * h1 * h1, 192))
         m = (ctypes.c_float * 3)(*self.MEAN)
         sdev = (ctypes.c_float * 3)(*self.STD)
-        self.ops.call("dm_leres_stem_im2col_f32_batch", planar, hi, wi, r, B, net, net, m, sdev, cols)
+        self.ops.call("dm_leres_stem_im2col_f32_batch" + self._cv, planar, hi, wi, r, B, net, net, m, sdev, cols)
         return self._network(B, net, net, cols)
 
     def _network_eager(self, B, net_h, net_w, cols):
         import torch
         ops, w = self.ops, self.w
         h1, w1 = (net_h + 6 - 7) // 2 + 1, (net_w + 6 - 7) // 2 + 1
+        # circular padding: the halo copy of a 3x3 convolution's input, sized for the largest one (adapt_conv.0's 256 channels at
+        # half the net size)
+        halo = self._buf('halo', (B * (net_h // 2 + 2) * (net_w // 2 + 2) * 256,)) if self.circular else None
         x = self._buf('stem', (B, h1, w1, 64))
         ops.gemm(cols, 192, w['stem'][0], 192, B * h1 * w1, 64, 192, act=_lib.ACT_RELU, bias=w['stem'][1], C=x, ldc=64)
         h, wd = (h1 + 2 - 3) // 2 + 1, (w1 + 2 - 3) // 2 + 1
@@ -762,11 +778,11 @@ class LeresEngine:
                 if stride == 1:
                     ho, wo = h, wd
                     t2 = self._buf(tag + '_t2', (B, ho, wo, width))
-                    ops.conv3x3(t1, B, h, wd, width, blk['c2'][0], width, act=_lib.ACT_RELU, bias=blk['c2'][1], C=t2)
+                    ops.conv3x3(t1, B, h, wd, width, blk['c2'][0], width, act=_lib.ACT_RELU, bias=blk['c2'][1], C=t2, halo=halo)
                 else:
                     ho, wo = (h + 2 - 3) // 2 + 1, (wd + 2 - 3) // 2 + 1
                     c2 = self._buf(tag + '_cols', (B * ho * wo, 9 * width))
-                    ops.call("dm_im2col_s2_f16", t1, B, h, wd, width, c2)
+                    ops.call("dm_im2col_s2_circular_f16" if self.circular else "dm_im2col_s2_f16", t1, B, h, wd, width, c2)
                     t2 = self._buf(tag + '_t2', (B, ho, wo, width))
                     ops.gemm(c2, 9 * width, blk['c2'][0], 9 * width, B * ho * wo, width, 9 * width, act=_lib.ACT_RELU, bias=blk['c2'][1], C=t2, ldc=width)
                 Mo = B * ho * wo
@@ -790,7 +806,7 @@ class LeresEngine:
         def conv(name, xin, hh, ww, ci, wb, co, act=_lib.ACT_NONE, R=None, C2=False):
             outp = self._buf(name, (B, hh, ww, co))
             out2 = self._buf(name + '_r', (B, hh, ww, co)) if C2 else None
-            ops.conv3x3(xin, B, hh, ww, ci, wb[0], co, act=act, bias=wb[1], C=outp, C2=out2, R=R)
+            ops.conv3x3(xin, B, hh, ww, ci, wb[0], co, act=act, bias=wb[1], C=outp, C2=out2, R=R, halo=halo)
             return out2 if C2 else outp
 
         def ftb(name, xin, hh, ww, ci, f, cm):
@@ -819,7 +835,7 @@ class LeresEngine:
             hh, ww = 2 * hl, 2 * wl
         x = conv('ao0', x, hh, ww, 256, w['ao0'], 128, act=_lib.ACT_RELU)
         d32 = self._buf('ao3', (B * hh * ww, 32), torch.float32)
-        ops.conv3x3(x, B, hh, ww, 128, w['ao3'][0], 32, epi=_lib.EPI_STORE_F32, bias=w['ao3'][1], X=d32, ldx=32)
+        ops.conv3x3(x, B, hh, ww, 128, w['ao3'][0], 32, epi=_lib.EPI_STORE_F32, bias=w['ao3'][1], X=d32, ldx=32, halo=halo)
         dn = self._buf('dnet', (B, 2 * hh, 2 * ww), torch.float32)
         ops.call("dm_resize_f32_ld", d32, 32, B, hh, ww, dn, 2 * hh, 2 * ww, 0)
         assert (2 * hh, 2 * ww) == (net_h, net_w)
@@ -952,9 +968,9 @@ class _ZoeDepthBase(DptBeitEngine):
 
     PROJ = ATT_HID = ATT_OUT = None     # hidden width of the projectors, of the attractor MLPs, and the attractor MLPs' output
 
-    def __init__(self, state_dict, device, core_name='beitl16_384'):
+    def __init__(self, state_dict, device, core_name='beitl16_384', circular=False):
         core_sd = {k[len("core.core."):]: v for k, v in state_dict.items() if k.startswith("core.core.")}
-        super().__init__(core_sd, core_name, device)
+        super().__init__(core_sd, core_name, device, circular)
         self._pack_head({k: v for k, v in state_dict.items() if not k.startswith("core.")})
         # output_conv.2, whose 32-channel ReLU output MidasCore hooks, stored as its own activation
         self.z['oc2_w'] = _conv_w(self._oc2_weight.to(device), self.F2p, 32)
@@ -1018,9 +1034,9 @@ class _ZoeDepthBase(DptBeitEngine):
         Fp = self.Fp
         # out_conv activation (MidasCore hooks output_conv[3], the 32-channel ReLU)
         t = b['up_sizes'][3]
-        ops.conv3x3(b['path'][3], F, t[0], t[1], Fp, self.w['oc1_w'], self.F2p, bias=self.w['oc1_b'], C=b['oc1'])
+        ops.conv3x3(b['path'][3], F, t[0], t[1], Fp, self.w['oc1_w'], self.F2p, bias=self.w['oc1_b'], C=b['oc1'], halo=b['halo'])
         ops.call("dm_resize_bilinear_nhwc_f16", b['oc1'], F, t[0], t[1], self.F2p, b['oc1u'], nh, nw)
-        ops.conv3x3(b['oc1u'], F, nh, nw, self.F2p, z['oc2_w'], 32, act=RELU, bias=z['oc2_b'], C=zb['o32'])
+        ops.conv3x3(b['oc1u'], F, nh, nw, self.F2p, z['oc2_w'], 32, act=RELU, bias=z['oc2_b'], C=zb['o32'], halo=b['halo'])
         n0 = zb['n0']
         # x = conv2(bottleneck); seed bins; seed embedding
         self.lin(b['l'][3], Fp, z['conv2'], F * n0, Fp, Fp, out=zb['x16'])
@@ -1179,12 +1195,12 @@ class ZoeDepthEngine(_ZoeDepthBase):
 
     PROJ, ATT_HID, ATT_OUT = 128, 128, 32
 
-    def __init__(self, state_dict, device, variant, core_name='beitl16_384'):
+    def __init__(self, state_dict, device, variant, core_name='beitl16_384', circular=False):
         if variant not in ZOE_SINGLE_VARIANTS:
             raise ValueError(f"ZoeDepthEngine: variant must be 'n' or 'k', not {variant!r}")
         self.variant = variant
         self.normed = ZOE_SINGLE_VARIANTS[variant]['bin_centers_type'] == 'normed'
-        super().__init__(state_dict, device, core_name)
+        super().__init__(state_dict, device, core_name, circular)
 
     def _pack_head(self, sd):
         import torch
@@ -1258,23 +1274,28 @@ def _unwrap_leres(sd):
 _flat = lambda sd: sd
 _midas = _unwrap_key("model", "optimizer")      # dmidas/base_model.py:13
 _zoe = _unwrap_key("model", "model")            # dzoedepth/models/model_io.py:52-53
-_native = lambda sd, t, dev, boost: NativeDepthModel(sd, t, dev)
-# model type -> (default checkpoint path, unwrap, engine(state_dict, model type, device, boost)).  The MiDaS DPT
-# models run through the op-level engine under BOOST (float crops, estimatemidasBoost) and through the model-level handle otherwise.
+
+
+def _op_or_native(cls, name):
+    """the model-level handle (zero padding only), or the op-level engine under BOOST (float crops) or tiling (circular padding)"""
+    return lambda sd, t, dev, boost, tiling: cls(sd, name, dev, tiling) if boost or tiling else NativeDepthModel(sd, t, dev)
+
+
+# model type -> (default checkpoint path, unwrap, engine(state_dict, model type, device, boost, tiling)).  The MiDaS DPT and
+# Depth-Anything-V2 models run through the model-level handle unless BOOST or tiling mode needs the op-level engine.
 CHECKPOINTS = {
-    0: ("./models/leres/res101.pth", _unwrap_leres, lambda sd, t, dev, boost: LeresEngine(sd, dev)),
-    1: ("./models/midas/dpt_beit_large_512.pt", _midas,
-        lambda sd, t, dev, boost: DptBeitEngine(sd, 'beitl16_512', dev) if boost else NativeDepthModel(sd, t, dev)),
-    2: ("./models/midas/dpt_beit_large_384.pt", _midas,
-        lambda sd, t, dev, boost: DptBeitEngine(sd, 'beitl16_384', dev) if boost else NativeDepthModel(sd, t, dev)),
-    3: ("./models/midas/dpt_large-midas-2f21e586.pt", _midas,
-        lambda sd, t, dev, boost: DptVitEngine(sd, 'vitl16_384', dev) if boost else NativeDepthModel(sd, t, dev)),
-    7: ("./models/zoedepth/" + ZOE_SINGLE_VARIANTS['n']['checkpoint'], _zoe, lambda sd, t, dev, boost: ZoeDepthEngine(sd, dev, 'n')),
-    8: ("./models/zoedepth/" + ZOE_SINGLE_VARIANTS['k']['checkpoint'], _zoe, lambda sd, t, dev, boost: ZoeDepthEngine(sd, dev, 'k')),
-    9: ("./models/zoedepth/ZoeD_M12_NK.pt", _zoe, lambda sd, t, dev, boost: ZoeDepthNKEngine(sd, dev)),
-    12: ("./models/depth_anything_v2/depth_anything_v2_vits.pth", _flat, _native),
-    13: ("./models/depth_anything_v2/depth_anything_v2_vitb.pth", _flat, _native),
-    14: ("./models/depth_anything_v2/depth_anything_v2_vitl.pth", _flat, _native),
+    0: ("./models/leres/res101.pth", _unwrap_leres, lambda sd, t, dev, boost, tiling: LeresEngine(sd, dev, tiling)),
+    1: ("./models/midas/dpt_beit_large_512.pt", _midas, _op_or_native(DptBeitEngine, 'beitl16_512')),
+    2: ("./models/midas/dpt_beit_large_384.pt", _midas, _op_or_native(DptBeitEngine, 'beitl16_384')),
+    3: ("./models/midas/dpt_large-midas-2f21e586.pt", _midas, _op_or_native(DptVitEngine, 'vitl16_384')),
+    7: ("./models/zoedepth/" + ZOE_SINGLE_VARIANTS['n']['checkpoint'], _zoe,
+        lambda sd, t, dev, boost, tiling: ZoeDepthEngine(sd, dev, 'n', circular=tiling)),
+    8: ("./models/zoedepth/" + ZOE_SINGLE_VARIANTS['k']['checkpoint'], _zoe,
+        lambda sd, t, dev, boost, tiling: ZoeDepthEngine(sd, dev, 'k', circular=tiling)),
+    9: ("./models/zoedepth/ZoeD_M12_NK.pt", _zoe, lambda sd, t, dev, boost, tiling: ZoeDepthNKEngine(sd, dev, circular=tiling)),
+    12: ("./models/depth_anything_v2/depth_anything_v2_vits.pth", _flat, _op_or_native(DepthAnythingV2Engine, 'vits')),
+    13: ("./models/depth_anything_v2/depth_anything_v2_vitb.pth", _flat, _op_or_native(DepthAnythingV2Engine, 'vitb')),
+    14: ("./models/depth_anything_v2/depth_anything_v2_vitl.pth", _flat, _op_or_native(DepthAnythingV2Engine, 'vitl')),
 }
 PIX2PIX_CHECKPOINT = "./models/pix2pix/latest_net_G.pth"
 
@@ -1319,8 +1340,6 @@ class ModelHolder:
         if boost and model_type not in BASE_NETWORKS:
             raise NotImplementedError(f"BOOST is implemented in depthmap_b200 for the base networks LeReS res101 (model type 0), "
                                       f"DPT-BEiT-L 512 / 384 (1, 2) and DPT-Large 384 (3), not for model type {model_type}")
-        if tiling_mode:
-            raise NotImplementedError("tiling_mode (circular conv padding) is not implemented in depthmap_b200 yet")
         if getattr(self, "no_half", False):
             # reference: `no_half` keeps the network in fp32 (src/depthmap_generation.py:268-275).  The H100 path feeds the tensor
             # cores fp16 operands (fp32 accumulation, fp32 residual stream) and has no fp32-operand variant: say so instead of
@@ -1333,7 +1352,7 @@ class ModelHolder:
                                       f"8 = ZoeDepth-K; 9 = ZoeDepth-NK; 12, 13, 14 = Depth-Anything-V2 S/B/L)")
         dev = torch.device(device)
         path, unwrap, make = CHECKPOINTS[model_type]
-        model = make(self._load_checkpoint(model_type, path, unwrap), model_type, dev, boost)
+        model = make(self._load_checkpoint(model_type, path, unwrap), model_type, dev, boost, bool(tiling_mode))
         if boost:      # reference :284-299: the pix2pix merge network ('latest_net_G.pth', netG = unet_1024, norm none)
             from .boost import BoostPipeline, UnetMergeEngine
             self.pix2pix_model = BoostPipeline(model, UnetMergeEngine(self._load_checkpoint("pix2pix", PIX2PIX_CHECKPOINT), dev), dev, model_type)
