@@ -207,7 +207,8 @@ int dm_zoe_preprocess_patchify(const uint8_t *rgb, int B, int H, int W, int pad_
                                int kpad, void *stream);
 /* x = LayerNorm(x) in place (fp32 [rows, 128]) + fp16 copy: post-norm nn.TransformerEncoderLayer of the router */
 int dm_layernorm_post_f16(float *x, long long rows, int C, const float *gamma, const float *beta, float eps, void *out, void *stream);
-/* self-attention of the router: qkv fp16 [F*S, 3*heads*32] (q | k | v) -> out fp16 [F*S, heads*32] */
+/* self-attention of the router: qkv fp16 [F*S, 3*heads*32] (q | k | v) -> out fp16 [F*S, heads*32]; any S >= 1 (K / V are
+ * streamed through shared memory in tiles) */
 int dm_attention_small_f16(const void *qkv, int F, int S, int heads, float scale, void *out, void *stream);
 int dm_cast_f32_f16(const float *x, long long n, void *out, void *stream);
 /* out[r, 0..63] = softplus(seed[r, head*64 .. head*64+63]) for the routed head of row r's forward */

@@ -6,7 +6,7 @@
 //   zoe_preprocess_patchify  ToTensor -> reflect pad -> (flip) -> bilinear align_corners=True to the net size -> (x-.5)/.5
 //                            -> fp16 patch matrix; forward 2b is image b, forward 2b+1 its horizontal flip (TTA)
 //   layernorm_post           post-norm transformer layer of the router: x = LN(x) in place (fp32) + fp16 copy
-//   attention_small          router self-attention (4 heads x 32 dims, 257 tokens), SIMT
+//   attention_small          router self-attention (4 heads x 32 dims, one token per 1/32 grid cell + 1), SIMT, K / V tiled
 //   select_softplus          seed bin centres of the routed head: softplus(seed[:, head*64 : head*64+64])
 //   resize_add_nhwc          x = b_emb + bilinear(prev_b_embedding)            (attractor.py:173-177)
 //   attractor                b_new = b + mean_i inv_attractor(A_i - b), b = bilinear(b_prev)   (attractor.py:178-208)
@@ -104,45 +104,96 @@ __global__ void __launch_bounds__(256) layernorm_post_kernel(float *__restrict__
     reinterpret_cast<uint2 *>(out + row * 128)[lane] = u;
 }
 
-// router attention: qkv fp16 [F*S, 3*E] (q | k | v, head h at columns h*32), out fp16 [F*S, E]; grid (F, heads)
-constexpr int RA_HD = 32, RA_PITCH = 33;
+// router attention: qkv fp16 [F*S, 3*E] (q | k | v, head h at columns h*32), out fp16 [F*S, E]; grid (F, heads, ceil(S / RA_ROWS)).
+// K and V stream through shared memory in tiles of RA_TILE tokens, so shared memory does not grow with S.  A block owns RA_ROWS
+// query rows; warp w carries rows w, w + 8, ... (RA_R of them) through every tile with an online softmax: running max, per-lane
+// partial sums and the output accumulator (lane = output dim), the last two scaled by exp(old max - new max) when a tile raises
+// the max.  The row sums are reduced across the warp once, after the last tile.
+constexpr int RA_HD = 32, RA_PITCH = 33, RA_TILE = 64, RA_R = 4, RA_ROWS = 8 * RA_R;
 __global__ void __launch_bounds__(256) attention_small_kernel(const __half *__restrict__ qkv, int S, int E, float scale, __half *__restrict__ out) {
-    extern __shared__ float ra_smem[];
-    float *sk = ra_smem, *sv = sk + (size_t)S * RA_PITCH, *sp = sv + (size_t)S * RA_PITCH;   // sp: [8 warps][S]
+    __shared__ float sk[RA_TILE * RA_PITCH], sv[RA_TILE * RA_PITCH];
+    __shared__ __align__(16) float sq[8][RA_R][RA_HD];      // the warp's scaled query rows, read as broadcasts
+    __shared__ float sp[8][RA_R][RA_TILE];                  // the warp's probabilities of the current tile
     const int f = blockIdx.x, h = blockIdx.y;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const __half *base = qkv + (size_t)f * S * 3 * E + h * RA_HD;
-    for (int i = threadIdx.x; i < S * RA_HD; i += 256) {
-        const int t = i >> 5, d = i & 31;
-        sk[t * RA_PITCH + d] = __half2float(base[(size_t)t * 3 * E + E + d]);
-        sv[t * RA_PITCH + d] = __half2float(base[(size_t)t * 3 * E + 2 * E + d]);
-    }
-    __syncthreads();
-    float *pw = sp + (size_t)warp * S;
-    const int rows_per = (S + gridDim.z - 1) / gridDim.z, t_beg = blockIdx.z * rows_per, t_end = min(S, t_beg + rows_per);
-    for (int t = t_beg + warp; t < t_end; t += 8) {
-        const float qd = __half2float(base[(size_t)t * 3 * E + lane]) * scale;
-        float mx = -INFINITY;
-        for (int j0 = 0; j0 < S; j0 += 32) {                 // uniform trip count: the shuffles need every lane
-            const int j = j0 + lane;
-            const float *kr = sk + (size_t)min(j, S - 1) * RA_PITCH;
-            float s = 0.f;
+    const int t0 = blockIdx.z * RA_ROWS + warp;
+    float mx[RA_R], sum[RA_R], acc[RA_R];
 #pragma unroll
-            for (int d = 0; d < RA_HD; ++d) s = fmaf(__shfl_sync(0xffffffffu, qd, d), kr[d], s);
-            if (j < S) { pw[j] = s; mx = fmaxf(mx, s); }
+    for (int r = 0; r < RA_R; ++r) {
+        const int t = min(t0 + 8 * r, S - 1);                // rows past S compute a copy of the last row and are not stored
+        sq[warp][r][lane] = __half2float(base[(size_t)t * 3 * E + lane]) * scale;
+        mx[r] = -INFINITY; sum[r] = 0.f; acc[r] = 0.f;
+    }
+    for (int j0 = 0; j0 < S; j0 += RA_TILE) {
+        const int n = min(RA_TILE, S - j0);
+        __syncthreads();                                     // the previous tile is consumed (and sq is written, first time)
+        for (int i = threadIdx.x; i < RA_TILE * RA_HD; i += 256) {
+            const int t = i >> 5, d = i & 31;
+            float kv = 0.f, vv = 0.f;                        // zeros past S: their probability is 0, and 0 * 0 stays finite
+            if (t < n) {
+                const __half *row = base + (size_t)(j0 + t) * 3 * E;
+                kv = __half2float(row[E + d]);
+                vv = __half2float(row[2 * E + d]);
+            }
+            sk[t * RA_PITCH + d] = kv;
+            sv[t * RA_PITCH + d] = vv;
+        }
+        __syncthreads();
+        float s[RA_R][RA_TILE / 32];                         // lane = key token c * 32 + lane of the tile
+#pragma unroll
+        for (int c = 0; c < RA_TILE / 32; ++c) {
+            const float *kr = sk + (c * 32 + lane) * RA_PITCH;
+#pragma unroll
+            for (int r = 0; r < RA_R; ++r) s[r][c] = 0.f;
+#pragma unroll
+            for (int d = 0; d < RA_HD; d += 4) {
+                const float k0 = kr[d], k1 = kr[d + 1], k2 = kr[d + 2], k3 = kr[d + 3];
+#pragma unroll
+                for (int r = 0; r < RA_R; ++r) {
+                    const float4 q = *reinterpret_cast<const float4 *>(&sq[warp][r][d]);
+                    s[r][c] = fmaf(q.w, k3, fmaf(q.z, k2, fmaf(q.y, k1, fmaf(q.x, k0, s[r][c]))));
+                }
+            }
+            if (c * 32 + lane >= n) {
+#pragma unroll
+                for (int r = 0; r < RA_R; ++r) s[r][c] = -INFINITY;
+            }
+        }
+#pragma unroll
+        for (int r = 0; r < RA_R; ++r) {
+            float tm = s[r][0];
+#pragma unroll
+            for (int c = 1; c < RA_TILE / 32; ++c) tm = fmaxf(tm, s[r][c]);
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) tm = fmaxf(tm, __shfl_xor_sync(0xffffffffu, tm, o));
+            const float nm = fmaxf(mx[r], tm);               // finite: every tile holds at least one token
+            const float corr = __expf(mx[r] - nm);           // 0 on the first tile (mx = -inf)
+            mx[r] = nm;
+            float ps = 0.f;
+#pragma unroll
+            for (int c = 0; c < RA_TILE / 32; ++c) {
+                const float p = __expf(s[r][c] - nm);
+                sp[warp][r][c * 32 + lane] = p;
+                ps += p;
+            }
+            sum[r] = sum[r] * corr + ps;
+            acc[r] *= corr;
         }
         __syncwarp();
+        for (int j = 0; j < n; ++j) {
+            const float v = sv[j * RA_PITCH + lane];
 #pragma unroll
-        for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-        float sum = 0.f;
-        for (int j = lane; j < S; j += 32) { const float e = __expf(pw[j] - mx); pw[j] = e; sum += e; }
+            for (int r = 0; r < RA_R; ++r) acc[r] = fmaf(sp[warp][r][j], v, acc[r]);
+        }
+    }
 #pragma unroll
-        for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-        __syncwarp();
-        float acc = 0.f;                                    // lane = output dim
-        for (int j = 0; j < S; ++j) acc = fmaf(pw[j], sv[j * RA_PITCH + lane], acc);
-        out[((size_t)f * S + t) * E + h * RA_HD + lane] = __float2half_rn(acc / sum);
-        __syncwarp();
+    for (int r = 0; r < RA_R; ++r) {
+        float tot = sum[r];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) tot += __shfl_xor_sync(0xffffffffu, tot, o);
+        const int t = t0 + 8 * r;
+        if (t < S) out[((size_t)f * S + t) * E + h * RA_HD + lane] = __float2half_rn(acc[r] / tot);
     }
 }
 
@@ -605,14 +656,12 @@ DM_EXPORT int dm_layernorm_post_f16(float *x, long long rows, int C, const float
 
 DM_EXPORT int dm_attention_small_f16(const void *qkv, int F, int S, int heads, float scale, void *out, void *stream_) {
     using namespace dm;
-    const size_t smem = ((size_t)2 * S * RA_PITCH + (size_t)8 * S) * sizeof(float);
-    if (smem > 200 * 1024) { set_error("dm_attention_small_f16: %d tokens do not fit in shared memory", S); return DM_E_UNSUPPORTED; }
-    if (smem > 48 * 1024) {
-        static PerDeviceFlag configured;
-        if (!configured.test_and_set())
-            DM_CUDA_CHECK(cudaFuncSetAttribute(attention_small_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    if (!qkv || !out || F < 1 || S < 1 || heads < 1 || heads > 65535 || (S + RA_ROWS - 1) / RA_ROWS > 65535) {
+        set_error("dm_attention_small_f16: bad arguments (F, S, heads >= 1; heads and S / %d within the grid's 65535)", RA_ROWS);
+        return DM_E_INVALID;
     }
-    attention_small_kernel<<<dim3(F, heads, 4), 256, smem, (cudaStream_t)stream_>>>((const __half *)qkv, S, heads * RA_HD, scale, (__half *)out);   // 4 query-row blocks per (forward, head)
+    const dim3 grid((unsigned)F, (unsigned)heads, (unsigned)((S + RA_ROWS - 1) / RA_ROWS));
+    attention_small_kernel<<<grid, 256, 0, (cudaStream_t)stream_>>>((const __half *)qkv, S, heads * RA_HD, scale, (__half *)out);
     DM_LAUNCH_CHECK("attention_small_kernel");
     return DM_OK;
 }
