@@ -326,6 +326,28 @@ int dm_add_f16(const void *a, const void *b, void *out, long long n, void *strea
 int dm_resize_f32_ld(const float *in, int ld, int B, int Hin, int Win, float *out, int Hout, int Wout, int mode, void *stream);
 
 
+
+/* ---------------------------------------------------------------------------------------------------------------
+ * MiDaS v2.1 (MidasNet: ResNeXt-101 32x8d + RefineNet decoder, model type 5), csrc/midas_kernels.cu.  The encoder runs on the
+ *   LeReS entry points above; these replace the rest of estimatemidas (src/depthmap_generation.py:455-499, dmidas/midas_net.py).
+ * ------------------------------------------------------------------------------------------------------------- */
+/* uint8 RGB [B,H,W,3] -> cv2.resize(INTER_CUBIC) to net_h x net_w (a copy when the sizes match) -> x/255 -> (x - mean) / std, network
+ * channel c reading source channel chan_map_host[c] -> im2col of the 7x7 stride-2 pad-3 stem convolution: fp16 [B*Ho*Wo, 192], the
+ * layout of dm_leres_stem_im2col (taps ordered (ky, kx, c), columns 147..191 zero) */
+int dm_midas_stem_im2col(const uint8_t *rgb, int B, int H, int W, int net_h, int net_w, const float *mean_host, const float *std_host,
+                         const int *chan_map_host, void *out, void *stream);
+/* the same for B crops of one planar fp32 image [3, Hi, Wi] (values used as they are, no /255; BOOST's estimatemidasBoost):
+ * rects_dev: DEVICE int32 [B][4] = x0, y0, w, h inside the image (validated by the caller), 16-byte aligned */
+int dm_midas_stem_im2col_f32_crops(const float *img, int Hi, int Wi, const int *rects_dev, int B, int net_h, int net_w, const float *mean_host,
+                                   const float *std_host, const int *chan_map_host, void *out, void *stream);
+/* the two above with the stem's padding circular in network-input coordinates (tiling mode) */
+int dm_midas_stem_im2col_circular(const uint8_t *rgb, int B, int H, int W, int net_h, int net_w, const float *mean_host, const float *std_host,
+                                  const int *chan_map_host, void *out, void *stream);
+int dm_midas_stem_im2col_f32_crops_circular(const float *img, int Hi, int Wi, const int *rects_dev, int B, int net_h, int net_w,
+                                            const float *mean_host, const float *std_host, const int *chan_map_host, void *out, void *stream);
+/* fp16 NHWC bilinear resize, align_corners=False (half-pixel centres, source coordinate clamped at 0): F.interpolate(mode='bilinear') */
+int dm_resize_bilinear_half_nhwc_f16(const void *in, int B, int Hin, int Win, int C, void *out, int Hout, int Wout, void *stream);
+
 /* ---------------------------------------------------------------------------------------------------------------
  * D9 — BOOST (csrc/boost_kernels.cu): the device side of estimateboost / doubleestimate
  * (src/depthmap_generation.py:774-941, :1028-1050) and of the pix2pix merge U-Net (pix2pix/models/networks.py:444-543,

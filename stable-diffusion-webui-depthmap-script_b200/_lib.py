@@ -86,6 +86,8 @@ EXPORTS = [
     "dm_leres_stem_im2col_f32", "dm_leres_stem_im2col_f32_batch", "dm_boost_minmax_normalise",
     "dm_circular_halo_f16", "dm_conv3x3_circular_ex", "dm_im2col_s2_circular_f16", "dm_leres_stem_im2col_circular",
     "dm_leres_stem_im2col_f32_circular", "dm_leres_stem_im2col_f32_batch_circular",
+    "dm_midas_stem_im2col", "dm_midas_stem_im2col_circular", "dm_midas_stem_im2col_f32_crops", "dm_midas_stem_im2col_f32_crops_circular",
+    "dm_resize_bilinear_half_nhwc_f16",
 ]
 
 
@@ -178,6 +180,13 @@ def _bind_optional(L):
         L.dm_subsample2_nhwc_f16.argtypes = [vp, i32, i32, i32, i32, vp, vp]
         L.dm_add_f16.argtypes = [vp, vp, vp, c.c_longlong, vp]
         L.dm_resize_f32_ld.argtypes = [vp, i32, i32, i32, i32, vp, i32, i32, i32, vp]
+    if hasattr(L, "dm_midas_stem_im2col"):
+        fp, ip = c.POINTER(c.c_float), c.POINTER(c.c_int)
+        L.dm_midas_stem_im2col.argtypes = [vp, i32, i32, i32, i32, i32, fp, fp, ip, vp, vp]
+        L.dm_midas_stem_im2col_circular.argtypes = L.dm_midas_stem_im2col.argtypes
+        L.dm_midas_stem_im2col_f32_crops.argtypes = [vp, i32, i32, vp, i32, i32, i32, fp, fp, ip, vp, vp]
+        L.dm_midas_stem_im2col_f32_crops_circular.argtypes = L.dm_midas_stem_im2col_f32_crops.argtypes
+        L.dm_resize_bilinear_half_nhwc_f16.argtypes = [vp, i32, i32, i32, i32, vp, i32, i32, vp]
     if hasattr(L, "dm_unet_first_cols"):
         ll = c.c_longlong
         L.dm_unet_first_cols.argtypes = [vp, i32, i32, vp, i32, vp]

@@ -9,8 +9,8 @@ Split of work.  The CONTROL PLANE stays on the host exactly as in the reference,
 move: the R_x resolution search and the patch selection look only at the RGB image (Sobel gradients, thresholds, an integral
 image) and run through the same cv2 calls.  Every PIXEL of the depth result is produced on the GPU: the float image and its two
 cubic resizes, the base-network forwards on crops (LeReS, model type 0: csrc/boost_kernels.cu leres_stem_im2col_f32; the MiDaS DPT
-models 1-3 through estimatemidasBoost, :1180-1220: csrc/vit_kernels.cu preprocess_patchify_f32_crops, then the per-call min-max
-normalisation at crop size), the cubic resizes to and from the
+models 1-3 and MiDaS v2.1 (5) through estimatemidasBoost, :1180-1220: csrc/vit_kernels.cu preprocess_patchify_f32_crops or
+csrc/midas_kernels.cu midas_stem_im2col_f32_crops, then the per-call min-max normalisation at crop size), the cubic resizes to and from the
 1024^2 merge resolution, the merge U-Net (split-operand fp32-class GEMMs), min-max normalisations, the degree-1 least-squares fit
 (fp64 sums) and the Gaussian-mask blend; one device->host copy at the end.
 
@@ -322,7 +322,7 @@ class UnetMergeEngine:
 # ---------------------------------------------------------------------------------------------------------------------
 # data plane
 # ---------------------------------------------------------------------------------------------------------------------
-BASE_NETWORKS = (0, 1, 2, 3)      # LeReS res101; DPT-BEiT-L 512, DPT-BEiT-L 384, DPT-Large 384 (singleestimate, :1053-1066)
+BASE_NETWORKS = (0, 1, 2, 3, 5)   # LeReS res101; DPT-BEiT-L 512, DPT-BEiT-L 384, DPT-Large 384; MiDaS v2.1 (singleestimate, :1053-1066)
 
 
 class BoostPipeline:
@@ -331,7 +331,7 @@ class BoostPipeline:
     def __init__(self, depth_engine, merge_engine, device, model_type=0):
         import torch
         if model_type not in BASE_NETWORKS:
-            raise NotImplementedError(f"boost is built for the base networks LeReS res101 (model type 0) and the MiDaS DPT models (1, 2, 3), "
+            raise NotImplementedError(f"boost is built for the base networks LeReS res101 (model type 0) and the MiDaS models (1, 2, 3, 5), "
                                       f"not model type {model_type}")
         self.depth, self.merge, self.device, self.model_type = depth_engine, merge_engine, device, model_type
         self.midas = model_type != 0      # estimatemidasBoost: crop-size min-max normalisation of every estimate

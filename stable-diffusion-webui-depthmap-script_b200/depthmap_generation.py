@@ -7,8 +7,8 @@
 the bench.  The network forward is a sequence of C-ABI calls (wgmma GEMM / implicit-GEMM conv / fused attention /
 LayerNorm / resize kernels, include/depthmap_b200.h); PyTorch only owns device memory and the stream.
 
-Implemented model types: 0 (LeReS res101), 1, 2 (MiDaS 3.1 DPT-BEiT-L 512 / 384), 3 (MiDaS 3.0 DPT-Large 384), 7, 8, 9
-(ZoeDepth-N, -K, -NK) and 12, 13, 14 (Depth-Anything-V2 S/B/L).  Others raise NotImplementedError naming the type.
+Implemented model types: 0 (LeReS res101), 1, 2 (MiDaS 3.1 DPT-BEiT-L 512 / 384), 3 (MiDaS 3.0 DPT-Large 384), 5 (MiDaS v2.1,
+ResNeXt-101 MidasNet), 7, 8, 9 (ZoeDepth-N, -K, -NK) and 12, 13, 14 (Depth-Anything-V2 S/B/L).  Others raise NotImplementedError naming the type.
 Weights: a state_dict in the upstream checkpoint layout (``depth_anything_v2_vit{s,b,l}.pth``), packed once at load
 into the kernels' layout (fp16 GEMM operands, (ky,kx,cin)-ordered conv filters, ConvTranspose as GEMM + pixel shuffle).
 Tiling mode (``tiling_mode``, src/depthmap_generation.py:251-260) makes every padded Conv2d of the depth network pad
@@ -367,17 +367,41 @@ def midas_net_size(width, height, net_w, net_h, multiple_of=32):
     return _constrain_to_multiple_of(sw * width, multiple_of), _constrain_to_multiple_of(sh * height, multiple_of)
 
 
-def midas_boost_net_size(width, height, msize, multiple_of=32):
-    """Resize(msize, msize, keep_aspect_ratio, 'upper_bound', multiple of 32) of estimatemidasBoost (src/depthmap_generation.py:1183-1192,
-    dmidas/transforms.py:94-160): the largest net inside msize x msize with the crop's aspect; a side that rounds past msize is
-    floored instead."""
-    sh, sw = msize / height, msize / width
+def midas_upper_bound_net_size(width, height, net_w, net_h, multiple_of=32):
+    """Resize(net_w, net_h, keep_aspect_ratio, 'upper_bound', multiple of 32) (dmidas/transforms.py:94-160): scale by the smaller of
+    the two ratios, so the net fits inside net_w x net_h with the image's aspect; a side that rounds past its bound is floored
+    instead, and may become 0 for a very elongated image."""
+    sh, sw = net_h / height, net_w / width
     if sw < sh:
         sh = sw
     else:
         sw = sh
-    return (_constrain_to_multiple_of(sw * width, multiple_of, max_val=msize),
-            _constrain_to_multiple_of(sh * height, multiple_of, max_val=msize))
+    return (_constrain_to_multiple_of(sw * width, multiple_of, max_val=net_w),
+            _constrain_to_multiple_of(sh * height, multiple_of, max_val=net_h))
+
+
+def midas_boost_net_size(width, height, msize, multiple_of=32):
+    """Resize(msize, msize, keep_aspect_ratio, 'upper_bound', multiple of 32) of estimatemidasBoost (src/depthmap_generation.py:1183-1192):
+    the largest net inside msize x msize with the crop's aspect."""
+    return midas_upper_bound_net_size(width, height, msize, msize, multiple_of)
+
+
+def _midas_crop_groups(planar, rects, msize):
+    """estimatemidasBoost's crops (x0, y0, w, h) of one planar fp32 image [3, Hi, Wi] -> (Hi, Wi, {(nh, nw): [crop indices]}): each
+    crop at its upper-bound net size for msize.  Crops clipped at the image border are not square, hence the grouping."""
+    import torch
+    hi, wi = int(planar.shape[1]), int(planar.shape[2])
+    if planar.dtype != torch.float32 or planar.dim() != 3 or planar.shape[0] != 3 or not planar.is_contiguous():
+        raise ValueError("planar must be a contiguous float32 tensor [3, H, W]")
+    groups = {}
+    for k, (x0, y0, w, h) in enumerate(rects):
+        if x0 < 0 or y0 < 0 or w <= 0 or h <= 0 or x0 + w > wi or y0 + h > hi:
+            raise ValueError(f"crop {(x0, y0, w, h)} outside the {wi}x{hi} image")
+        nw, nh = midas_boost_net_size(w, h, msize)
+        if nw <= 0 or nh <= 0:
+            raise ValueError(f"crop {w}x{h} is too elongated for a net of at most {msize} px")
+        groups.setdefault((nh, nw), []).append(k)
+    return hi, wi, groups
 
 
 class DptBeitEngine(DepthAnythingV2Engine):
@@ -501,17 +525,7 @@ class DptBeitEngine(DepthAnythingV2Engine):
         upper-bound net size for msize, then cv2-cubic back to the crop.  Crops clipped at the image border are not square, so the
         crops are grouped by net shape, one batched forward per shape."""
         import torch
-        hi, wi = int(planar.shape[1]), int(planar.shape[2])
-        if planar.dtype != torch.float32 or planar.dim() != 3 or planar.shape[0] != 3 or not planar.is_contiguous():
-            raise ValueError("planar must be a contiguous float32 tensor [3, H, W]")
-        groups = {}
-        for k, (x0, y0, w, h) in enumerate(rects):
-            if x0 < 0 or y0 < 0 or w <= 0 or h <= 0 or x0 + w > wi or y0 + h > hi:
-                raise ValueError(f"crop {(x0, y0, w, h)} outside the {wi}x{hi} image")
-            nw, nh = midas_boost_net_size(w, h, msize)
-            if nw <= 0 or nh <= 0:
-                raise ValueError(f"crop {w}x{h} is too elongated for a net of at most {msize} px")
-            groups.setdefault((nh, nw), []).append(k)
+        hi, wi, groups = _midas_crop_groups(planar, rects, msize)
         m, sd, cm = (ctypes.c_float * 3)(*self.BOOST_MEAN), (ctypes.c_float * 3)(*self.BOOST_STD), (ctypes.c_int * 3)(*self.CHAN_MAP)
         out = [None] * len(rects)
         for (nh, nw), ks in groups.items():
@@ -569,21 +583,20 @@ class DptVitEngine(DptBeitEngine):
     attention = DepthAnythingV2Engine.attention     # plain attention, no relative-position bias
 
 
-class LeresEngine:
-    """LeReS / res101 (model type 0) on the sm_90a kernels: estimateleres (src/depthmap_generation.py:406-440) around
-    RelDepthModel('resnext101') (lib/multi_depth_model_woauxi.py:6-32, lib/Resnext_torch.py:60-220, lib/network_auxi.py:15-215).
+class _ResNeXtEngine:
+    """The ResNeXt-101 32x8d encoder LeReS and MiDaS v2.1 share (torchvision's ResNet(Bottleneck, [3, 4, 23, 3], groups=32,
+    width_per_group=8); lib/Resnext_torch.py:60-220), with the buffer pool and CUDA-graph cache of their op-level engines.
     NHWC fp16 activations, fp32 accumulation.  1x1 convolutions are GEMMs, 3x3 ones the implicit-GEMM conv; the 32-group 3x3
     convolutions use block-diagonal dense filters (exact: the extra products are zeros), the three stride-2 ones go through the
     strided im2col; BatchNorm (running statistics, eps 1e-5) is folded into filters and biases when the checkpoint is packed; the
-    bottleneck's `relu(out + identity)` and FTB's `relu(x + branch)` come out of the GEMM epilogue's relu copy (C2).
-    circular=True: tiling mode, the stem, every 3x3 convolution of the encoder and the decoder pad circularly."""
+    bottleneck's `relu(out + identity)` comes out of the GEMM epilogue's relu copy (C2).  circular=True: tiling mode, the stem and
+    every 3x3 convolution pad circularly (the max-pool keeps its padding)."""
 
     LAYERS = (3, 4, 23, 3)
     GROUPS = 32
-    ENC = "depth_model.encoder_modules.encoder."
-    DEC = "depth_model.decoder_modules."
     MEAN = (0.485, 0.456, 0.406)
     STD = (0.229, 0.224, 0.225)
+    GRAPH_ENV, NAME = None, None     # environment switch and name of the engine's CUDA-graph cache
 
     def __init__(self, state_dict, device, circular=False):
         self.device = device
@@ -592,7 +605,7 @@ class LeresEngine:
         self.ops = _lib.Ops()
         self._bufs = {}
         # from the second call on at a given (B, net size) the ~500 launches of the network replay from a CUDA graph
-        self._graphs = _lib.GraphCache(self.ops, "DEPTHMAP_B200_LERES_GRAPH", "LeReS")
+        self._graphs = _lib.GraphCache(self.ops, self.GRAPH_ENV, self.NAME)
         self._pooled_bytes, self._pool_limit = 0, None
         self._pack(state_dict)
 
@@ -634,16 +647,15 @@ class LeresEngine:
         bb[:co] = b
         return t.reshape(n, 9 * ci).to(self.device).contiguous(), bb.to(self.device).contiguous()
 
-    def _pack(self, sd):
-        import torch
-        E, D = self.ENC, self.DEC
-        w = {}
-        sw, sb = self._fold(sd, E + 'conv1', E + 'bn1')            # [64, 3, 7, 7] -> [64, (ky, kx, c)] padded to 192
-        w['stem'] = self._mat(sw.permute(0, 2, 3, 1).contiguous(), sb, kpad=192)
+    def _pack_encoder(self, sd, stem_conv, stem_bn, block):
+        """folded stem (fp16 [64, 192], K ordered (ky, kx, c)) and bottleneck weights; block(li, bi) is the checkpoint prefix of
+        bottleneck bi of stage li"""
+        sw, sb = self._fold(sd, stem_conv, stem_bn)               # [64, 3, 7, 7] -> [64, (ky, kx, c)] padded to 192
+        stem = self._mat(sw.permute(0, 2, 3, 1).contiguous(), sb, kpad=192)
         blocks = []
         for li, nb in enumerate(self.LAYERS, start=1):
             for bi in range(nb):
-                p = f"{E}layer{li}.{bi}"
+                p = block(li, bi)
                 blk = dict(stride=2 if (bi == 0 and li > 1) else 1)
                 blk['c1'] = self._mat(*self._fold(sd, p + '.conv1', p + '.bn1'))
                 blk['c2'] = self._conv3(*self._fold(sd, p + '.conv2', p + '.bn2'), groups=self.GROUPS)
@@ -651,20 +663,7 @@ class LeresEngine:
                 blk['down'] = self._mat(*self._fold(sd, p + '.downsample.0', p + '.downsample.1')) if bi == 0 else None
                 blk['width'], blk['cout'] = blk['c1'][0].shape[0], blk['c3'][0].shape[0]
                 blocks.append(blk)
-        w['blocks'] = blocks
-
-        def ftb(p):
-            return dict(c1=self._conv3(*self._fold(sd, p + '.conv1', None)),
-                        b1=self._conv3(*self._fold(sd, p + '.conv_branch.1', p + '.conv_branch.2')),
-                        b4=self._conv3(*self._fold(sd, p + '.conv_branch.4', None)))
-        w['conv'] = ftb(D + 'conv')
-        w['conv1'] = self._conv3(*self._fold(sd, D + 'conv1', None))
-        for k in ('ffm2', 'ffm1', 'ffm0'):
-            w[k] = (ftb(D + k + '.ftb1'), ftb(D + k + '.ftb2'))
-        a = D + 'outconv.adapt_conv'
-        w['ao0'] = self._conv3(*self._fold(sd, a + '.0', a + '.1'))
-        w['ao3'] = self._conv3(*self._fold(sd, a + '.3', None), npad=32)
-        self.w = w
+        return stem, blocks
 
     # ---- buffers: a simple keyed pool (every tensor of a forward has its own name) ---------------------------------
     def _buf(self, name, shape, dtype=None):
@@ -692,11 +691,95 @@ class LeresEngine:
             self._pooled_bytes = 0
             torch.cuda.empty_cache()
 
-    # ---- forward ---------------------------------------------------------------------------------------------------
     def _network(self, B, net_h, net_w, cols):
         """stem GEMM .. decoder output [B, net_h, net_w] fp32 (a pooled buffer)"""
         return self._graphs.run((B, net_h, net_w), lambda: self._network_eager(B, net_h, net_w, cols))
 
+    def _encoder(self, B, net_h, net_w, cols, halo):
+        """stem GEMM (folded BN + ReLU) on the stem's im2col `cols`, max-pool, the 33 bottlenecks -> [(feature, h, w, channels)] after
+        each stage (1/4 .. 1/32); `halo`: the circular-padding scratch, or None"""
+        ops, w = self.ops, self.w
+        h1, w1 = (net_h + 6 - 7) // 2 + 1, (net_w + 6 - 7) // 2 + 1
+        x = self._buf('stem', (B, h1, w1, 64))
+        ops.gemm(cols, 192, w['stem'][0], 192, B * h1 * w1, 64, 192, act=_lib.ACT_RELU, bias=w['stem'][1], C=x, ldc=64)
+        h, wd = (h1 + 2 - 3) // 2 + 1, (w1 + 2 - 3) // 2 + 1
+        xp = self._buf('pool', (B, h, wd, 64))
+        ops.call("dm_maxpool3x3s2_nhwc_f16", x, B, h1, w1, 64, xp)
+        x, cin = xp, 64
+        feats = []
+        bi_global = 0
+        for li, nb in enumerate(self.LAYERS, start=1):
+            for bi in range(nb):
+                blk = w['blocks'][bi_global]
+                tag = f"l{li}b{bi % 2}" if bi > 0 else f"l{li}first"
+                width, cout, stride = blk['width'], blk['cout'], blk['stride']
+                M = B * h * wd
+                t1 = self._buf(tag + '_t1', (B, h, wd, width))
+                ops.gemm(x, cin, blk['c1'][0], cin, M, width, cin, act=_lib.ACT_RELU, bias=blk['c1'][1], C=t1, ldc=width)
+                if stride == 1:
+                    ho, wo = h, wd
+                    t2 = self._buf(tag + '_t2', (B, ho, wo, width))
+                    ops.conv3x3(t1, B, h, wd, width, blk['c2'][0], width, act=_lib.ACT_RELU, bias=blk['c2'][1], C=t2, halo=halo)
+                else:
+                    ho, wo = (h + 2 - 3) // 2 + 1, (wd + 2 - 3) // 2 + 1
+                    c2 = self._buf(tag + '_cols', (B * ho * wo, 9 * width))
+                    ops.call("dm_im2col_s2_circular_f16" if self.circular else "dm_im2col_s2_f16", t1, B, h, wd, width, c2)
+                    t2 = self._buf(tag + '_t2', (B, ho, wo, width))
+                    ops.gemm(c2, 9 * width, blk['c2'][0], 9 * width, B * ho * wo, width, 9 * width, act=_lib.ACT_RELU, bias=blk['c2'][1], C=t2, ldc=width)
+                Mo = B * ho * wo
+                if blk['down'] is not None:
+                    xs = x
+                    if stride == 2:
+                        xs = self._buf(tag + '_xs', (B, ho, wo, cin))
+                        ops.call("dm_subsample2_nhwc_f16", x, B, h, wd, cin, xs)
+                    idn = self._buf(tag + '_idn', (B, ho, wo, cout))
+                    ops.gemm(xs, cin, blk['down'][0], cin, Mo, cout, cin, bias=blk['down'][1], C=idn, ldc=cout)
+                else:
+                    idn = x
+                pre = self._buf(tag + '_pre', (B, ho, wo, cout))
+                last = bi == nb - 1
+                out = self._buf(f"feat{li}" if last else tag + '_out', (B, ho, wo, cout))
+                ops.gemm(t2, width, blk['c3'][0], width, Mo, cout, width, bias=blk['c3'][1], C=pre, ldc=cout, C2=out, R=idn, ldr=cout)
+                x, cin, h, wd = out, cout, ho, wo
+                bi_global += 1
+            feats.append((x, h, wd, cin))
+        return feats
+
+    def to(self, device):
+        return self
+
+
+class LeresEngine(_ResNeXtEngine):
+    """LeReS / res101 (model type 0) on the sm_90a kernels: estimateleres (src/depthmap_generation.py:406-440) around
+    RelDepthModel('resnext101') (lib/multi_depth_model_woauxi.py:6-32, lib/Resnext_torch.py:60-220, lib/network_auxi.py:15-215).
+    The shared ResNeXt-101 encoder, then the FTB / FFM / AO decoder on the implicit-GEMM conv; FTB's `relu(x + branch)` comes out of
+    the epilogue's relu copy (C2).  circular=True: tiling mode, the stem, every 3x3 convolution of the encoder and the decoder pad
+    circularly."""
+
+    ENC = "depth_model.encoder_modules.encoder."
+    DEC = "depth_model.decoder_modules."
+    GRAPH_ENV, NAME = "DEPTHMAP_B200_LERES_GRAPH", "LeReS"
+
+    def _pack(self, sd):
+        import torch
+        E, D = self.ENC, self.DEC
+        w = {}
+        w['stem'], w['blocks'] = self._pack_encoder(sd, E + 'conv1', E + 'bn1', lambda li, bi: f"{E}layer{li}.{bi}")
+
+        def ftb(p):
+            return dict(c1=self._conv3(*self._fold(sd, p + '.conv1', None)),
+                        b1=self._conv3(*self._fold(sd, p + '.conv_branch.1', p + '.conv_branch.2')),
+                        b4=self._conv3(*self._fold(sd, p + '.conv_branch.4', None)))
+        w['conv'] = ftb(D + 'conv')
+        w['conv1'] = self._conv3(*self._fold(sd, D + 'conv1', None))
+        for k in ('ffm2', 'ffm1', 'ffm0'):
+            w[k] = (ftb(D + k + '.ftb1'), ftb(D + k + '.ftb2'))
+        a = D + 'outconv.adapt_conv'
+        w['ao0'] = self._conv3(*self._fold(sd, a + '.0', a + '.1'))
+        w['ao3'] = self._conv3(*self._fold(sd, a + '.3', None), npad=32)
+        self.w = w
+
+    # ---- forward ---------------------------------------------------------------------------------------------------
     def forward_batch(self, rgb, net_w, net_h=None, out_hw=None, planar=None):
         """rgb: uint8 CUDA [B,H,W,3] -> float32 CUDA [B,H,W] (what estimateleres returns; invert = True).
         planar = (fp32 CUDA [3,Hi,Wi] image in network channel order, (x0, y0, w, h)) instead of `rgb`: estimateleres on a float
@@ -755,53 +838,10 @@ class LeresEngine:
     def _network_eager(self, B, net_h, net_w, cols):
         import torch
         ops, w = self.ops, self.w
-        h1, w1 = (net_h + 6 - 7) // 2 + 1, (net_w + 6 - 7) // 2 + 1
         # circular padding: the halo copy of a 3x3 convolution's input, sized for the largest one (adapt_conv.0's 256 channels at
         # half the net size)
         halo = self._buf('halo', (B * (net_h // 2 + 2) * (net_w // 2 + 2) * 256,)) if self.circular else None
-        x = self._buf('stem', (B, h1, w1, 64))
-        ops.gemm(cols, 192, w['stem'][0], 192, B * h1 * w1, 64, 192, act=_lib.ACT_RELU, bias=w['stem'][1], C=x, ldc=64)
-        h, wd = (h1 + 2 - 3) // 2 + 1, (w1 + 2 - 3) // 2 + 1
-        xp = self._buf('pool', (B, h, wd, 64))
-        ops.call("dm_maxpool3x3s2_nhwc_f16", x, B, h1, w1, 64, xp)
-        x, cin = xp, 64
-        feats = []
-        bi_global = 0
-        for li, nb in enumerate(self.LAYERS, start=1):
-            for bi in range(nb):
-                blk = w['blocks'][bi_global]
-                tag = f"l{li}b{bi % 2}" if bi > 0 else f"l{li}first"
-                width, cout, stride = blk['width'], blk['cout'], blk['stride']
-                M = B * h * wd
-                t1 = self._buf(tag + '_t1', (B, h, wd, width))
-                ops.gemm(x, cin, blk['c1'][0], cin, M, width, cin, act=_lib.ACT_RELU, bias=blk['c1'][1], C=t1, ldc=width)
-                if stride == 1:
-                    ho, wo = h, wd
-                    t2 = self._buf(tag + '_t2', (B, ho, wo, width))
-                    ops.conv3x3(t1, B, h, wd, width, blk['c2'][0], width, act=_lib.ACT_RELU, bias=blk['c2'][1], C=t2, halo=halo)
-                else:
-                    ho, wo = (h + 2 - 3) // 2 + 1, (wd + 2 - 3) // 2 + 1
-                    c2 = self._buf(tag + '_cols', (B * ho * wo, 9 * width))
-                    ops.call("dm_im2col_s2_circular_f16" if self.circular else "dm_im2col_s2_f16", t1, B, h, wd, width, c2)
-                    t2 = self._buf(tag + '_t2', (B, ho, wo, width))
-                    ops.gemm(c2, 9 * width, blk['c2'][0], 9 * width, B * ho * wo, width, 9 * width, act=_lib.ACT_RELU, bias=blk['c2'][1], C=t2, ldc=width)
-                Mo = B * ho * wo
-                if blk['down'] is not None:
-                    xs = x
-                    if stride == 2:
-                        xs = self._buf(tag + '_xs', (B, ho, wo, cin))
-                        ops.call("dm_subsample2_nhwc_f16", x, B, h, wd, cin, xs)
-                    idn = self._buf(tag + '_idn', (B, ho, wo, cout))
-                    ops.gemm(xs, cin, blk['down'][0], cin, Mo, cout, cin, bias=blk['down'][1], C=idn, ldc=cout)
-                else:
-                    idn = x
-                pre = self._buf(tag + '_pre', (B, ho, wo, cout))
-                last = bi == nb - 1
-                out = self._buf(f"feat{li}" if last else tag + '_out', (B, ho, wo, cout))
-                ops.gemm(t2, width, blk['c3'][0], width, Mo, cout, width, bias=blk['c3'][1], C=pre, ldc=cout, C2=out, R=idn, ldr=cout)
-                x, cin, h, wd = out, cout, ho, wo
-                bi_global += 1
-            feats.append((x, h, wd, cin))
+        feats = self._encoder(B, net_h, net_w, cols, halo)
 
         def conv(name, xin, hh, ww, ci, wb, co, act=_lib.ACT_NONE, R=None, C2=False):
             outp = self._buf(name, (B, hh, ww, co))
@@ -841,8 +881,155 @@ class LeresEngine:
         assert (2 * hh, 2 * ww) == (net_h, net_w)
         return dn
 
-    def to(self, device):
-        return self
+
+class _RequiredKeys(dict):
+    """a state dict whose missing keys raise ValueError naming the key"""
+
+    def __init__(self, sd, what):
+        super().__init__(sd)
+        self.what = what
+
+    def __missing__(self, key):
+        raise ValueError(f"{self.what} checkpoint lacks {key!r}")
+
+
+class MidasV21Engine(_ResNeXtEngine):
+    """MiDaS v2.1 (midas_v21, model type 5) on the sm_90a kernels: estimatemidas (src/depthmap_generation.py:455-499) with the
+    'upper_bound' resize and ImageNet statistics, around MidasNet (dmidas/midas_net.py:12-76, dmidas/blocks.py:136-320).
+
+    The encoder is the ResNeXt-101 32x8d of LeReS (`pretrained.layer1` = conv1, bn1, relu, maxpool, layer1), its stem fed by a cv2
+    INTER_CUBIC pre-processing + im2col.  The decoder: layer{1..4}_rn (3x3, no bias, 256 channels), the four FeatureFusionBlocks and
+    the head, all on the implicit-GEMM conv.  ResidualConvUnit's ReLU is in place, so its skip operand is relu(x):
+    RCU(x) = conv2(relu(conv1(relu(x)))) + relu(x), and only relu(layer_rn) is ever read.  FeatureFusionBlock: relu(path + RCU1(l))
+    leaves conv2's epilogue as its relu copy (the sum itself is dead), RCU2, then a x2 bilinear up-sample with align_corners=True.
+    refinenet4 has one input, and its resConfUnit1 is never used.  Head: conv3x3 256 -> 128, x2 bilinear with align_corners=False,
+    then conv3x3 128 -> 32, ReLU, conv1x1 32 -> 1, ReLU fused into one epilogue.  The prediction goes back to the image size by
+    bicubic interpolation (align_corners=False).
+
+    BOOST (estimatemidasBoost, :1180-1220) calls forward_batch(None, msize, msize, planar=(img, rect)) and
+    forward_crops(img, rects, msize) on float crops of a planar fp32 image, as for the DPT engines.  circular=True: tiling mode,
+    every padded convolution (stem, encoder and decoder 3x3s, head) pads circularly."""
+
+    FEATURES = 256
+    CHAN_MAP = (2, 1, 0)     # the network sees the BGR-swapped image of get_raw_prediction (:381): channel c reads source channel 2-c
+    GRAPH_ENV, NAME = "DEPTHMAP_B200_MIDAS_GRAPH", "MiDaS v2.1"
+
+    @staticmethod
+    def _block(li, bi):
+        return f"pretrained.layer1.4.{bi}" if li == 1 else f"pretrained.layer{li}.{bi}"
+
+    def _pack(self, sd):
+        import torch
+        sd = _RequiredKeys(sd, "MiDaS v2.1")
+        w = {}
+        w['stem'], w['blocks'] = self._pack_encoder(sd, 'pretrained.layer1.0', 'pretrained.layer1.1', self._block)
+        def conv(key, bias=True):
+            if bias and key + '.bias' not in sd:       # _fold would take a missing bias for zeros
+                raise ValueError(f"MiDaS v2.1 checkpoint lacks {key + '.bias'!r}")
+            return self._conv3(*self._fold(sd, key, None))
+        w['rn'] = [conv(f'scratch.layer{i}_rn', bias=False) for i in range(1, 5)]
+        for i in range(1, 5):
+            for u in ((2,) if i == 4 else (1, 2)):
+                for c in (1, 2):
+                    w[f'rf{i}_u{u}c{c}'] = conv(f'scratch.refinenet{i}.resConfUnit{u}.conv{c}')
+        w['oc0'] = conv('scratch.output_conv.0')
+        w['oc2'] = conv('scratch.output_conv.2')
+        w['oc4_w'] = sd['scratch.output_conv.4.weight'].detach().to(self.device, torch.float32).reshape(32).contiguous()
+        self.oc4_b = float(sd['scratch.output_conv.4.bias'].detach().float().reshape(-1)[0])
+        self.w = w
+
+    def _consts(self):
+        return (ctypes.c_float * 3)(*self.MEAN), (ctypes.c_float * 3)(*self.STD), (ctypes.c_int * 3)(*self.CHAN_MAP)
+
+    def _stem_cols(self, B, nh, nw):
+        return self._buf('stem_cols', (B * ((nh + 6 - 7) // 2 + 1) * ((nw + 6 - 7) // 2 + 1), 192))
+
+    # ---- forward ---------------------------------------------------------------------------------------------------
+    def net_size(self, W, H, net_w, net_h):
+        nw, nh = midas_upper_bound_net_size(W, H, net_w, net_h)
+        if nw <= 0 or nh <= 0:
+            raise ValueError(f"a {W}x{H} image is too elongated for a net of at most {net_w}x{net_h} px")
+        return nw, nh
+
+    def forward_batch(self, rgb, net_w, net_h=None, out_hw=None, planar=None):
+        """rgb: uint8 CUDA [B,H,W,3] -> float32 CUDA [B,H,W] (what estimatemidas returns; invert = False).  planar = (fp32 CUDA [3,Hi,Wi]
+        image, (x0, y0, w, h)) instead of `rgb`: estimatemidasBoost's network and resize on that crop with msize = net_w -> [1, h, w]
+        (not normalised)."""
+        import torch
+        if planar is not None:
+            img, rect = planar
+            return self.forward_crops(img, [rect], net_w)[0].unsqueeze(0)
+        B, H, W, _ = rgb.shape
+        nw, nh = self.net_size(W, H, net_w, net_h if net_h is not None else net_w)
+        self._trim_pools()
+        cols = self._stem_cols(B, nh, nw)
+        self.ops.call("dm_midas_stem_im2col" + self._cv, rgb, B, H, W, nh, nw, *self._consts(), cols)
+        d = self._network(B, nh, nw, cols)
+        oh, ow = out_hw if out_hw is not None else (H, W)
+        out = torch.empty(B, oh, ow, dtype=torch.float32, device=self.device)
+        self.ops.call("dm_resize_f32", d, B, nh, nw, out, oh, ow, 1)     # F.interpolate(bicubic, align_corners=False)
+        return out
+
+    def forward_crops(self, planar, rects, msize):
+        """B crops (x0, y0, w, h) of one planar fp32 image [3, Hi, Wi] -> [fp32 CUDA [h, w]] in the order of `rects`: each crop at its
+        upper-bound net size for msize, then cv2-cubic back to the crop; one batched forward per net shape."""
+        import torch
+        hi, wi, groups = _midas_crop_groups(planar, rects, msize)
+        self._trim_pools()
+        out = [None] * len(rects)
+        for (nh, nw), ks in groups.items():
+            B = len(ks)
+            r = torch.tensor([[int(v) for v in rects[k]] for k in ks], dtype=torch.int32).to(self.device)
+            cols = self._stem_cols(B, nh, nw)
+            self.ops.call("dm_midas_stem_im2col_f32_crops" + self._cv, planar, hi, wi, r, B, nh, nw, *self._consts(), cols)
+            d = self._network(B, nh, nw, cols)
+            for i, k in enumerate(ks):
+                w, h = int(rects[k][2]), int(rects[k][3])
+                o = torch.empty(h, w, dtype=torch.float32, device=self.device)
+                self.ops.call("dm_boost_resize_cubic", d[i], nw, 0, nh, nw, o, w, 0, h, w, 1)
+                out[k] = o
+        return out
+
+    def _network_eager(self, B, net_h, net_w, cols):
+        """stem GEMM .. head: the depth at the net size, fp32 [B, net_h, net_w] (a pooled buffer)"""
+        import torch
+        ops, w, F = self.ops, self.w, self.FEATURES
+        # circular padding: the halo copy of a 3x3 convolution's input, sized for the largest one (the head's second conv: 128
+        # channels at the net size, or its first: 256 at half of it)
+        halo = self._buf('halo', (B * max((net_h + 2) * (net_w + 2) * 128, (net_h // 2 + 2) * (net_w // 2 + 2) * F),)) if self.circular else None
+        feats = self._encoder(B, net_h, net_w, cols, halo)
+
+        def conv(name, xin, hh, ww, ci, wb, co, act=_lib.ACT_NONE, R=None, R2=None, C2=False):
+            outp = self._buf(name, (B, hh, ww, co))
+            out2 = self._buf(name + '_r', (B, hh, ww, co)) if C2 else None
+            ops.conv3x3(xin, B, hh, ww, ci, wb[0], co, act=act, bias=wb[1], C=outp, C2=out2, R=R, R2=R2, halo=halo)
+            return out2 if C2 else outp
+
+        def up2(name, xin, hh, ww):
+            outp = self._buf(name, (B, 2 * hh, 2 * ww, F))
+            ops.call("dm_resize_bilinear_nhwc_f16", xin, B, hh, ww, F, outp, 2 * hh, 2 * ww)
+            return outp
+
+        # layer{i}_rn, followed by the in-place ReLU of the first RCU that reads it
+        lr = [conv(f'rn{i}', x, h, wd, c, w['rn'][i], F, act=_lib.ACT_RELU) for i, (x, h, wd, c) in enumerate(feats)]
+        _, h, wd, _ = feats[3]
+        t = conv('rf4_t', lr[3], h, wd, F, w['rf4_u2c1'], F, act=_lib.ACT_RELU)
+        path = up2('rf4_up', conv('rf4_o', t, h, wd, F, w['rf4_u2c2'], F, R=lr[3]), h, wd)
+        for i in (3, 2, 1):                                   # refinenet{i} reads layer{i}_rn = lr[i - 1]
+            _, h, wd, _ = feats[i - 1]
+            t = conv(f'rf{i}_t1', lr[i - 1], h, wd, F, w[f'rf{i}_u1c1'], F, act=_lib.ACT_RELU)
+            s = conv(f'rf{i}_s', t, h, wd, F, w[f'rf{i}_u1c2'], F, R=lr[i - 1], R2=path, C2=True)     # relu(path + RCU1(l))
+            t = conv(f'rf{i}_t2', s, h, wd, F, w[f'rf{i}_u2c1'], F, act=_lib.ACT_RELU)
+            path = up2(f'rf{i}_up', conv(f'rf{i}_o', t, h, wd, F, w[f'rf{i}_u2c2'], F, R=s), h, wd)
+        h, wd = 2 * h, 2 * wd
+        a = conv('oc0', path, h, wd, F, w['oc0'], 128)
+        au = self._buf('oc0_up', (B, net_h, net_w, 128))
+        ops.call("dm_resize_bilinear_half_nhwc_f16", a, B, h, wd, 128, au, net_h, net_w)
+        d = self._buf('dnet', (B, net_h, net_w), torch.float32)
+        ops.conv3x3(au, B, net_h, net_w, 128, w['oc2'][0], 32, epi=_lib.EPI_HEAD, act=_lib.ACT_RELU, bias=w['oc2'][1], X=d,
+                    gamma=w['oc4_w'], head_b2=self.oc4_b, halo=halo)
+        assert (2 * h, 2 * wd) == (net_h, net_w)
+        return d
 
 
 class NativeDepthModel:
@@ -1288,6 +1475,7 @@ CHECKPOINTS = {
     1: ("./models/midas/dpt_beit_large_512.pt", _midas, _op_or_native(DptBeitEngine, 'beitl16_512')),
     2: ("./models/midas/dpt_beit_large_384.pt", _midas, _op_or_native(DptBeitEngine, 'beitl16_384')),
     3: ("./models/midas/dpt_large-midas-2f21e586.pt", _midas, _op_or_native(DptVitEngine, 'vitl16_384')),
+    5: ("./models/midas/midas_v21-f6b98070.pt", _midas, lambda sd, t, dev, boost, tiling: MidasV21Engine(sd, dev, tiling)),
     7: ("./models/zoedepth/" + ZOE_SINGLE_VARIANTS['n']['checkpoint'], _zoe,
         lambda sd, t, dev, boost, tiling: ZoeDepthEngine(sd, dev, 'n', circular=tiling)),
     8: ("./models/zoedepth/" + ZOE_SINGLE_VARIANTS['k']['checkpoint'], _zoe,
@@ -1339,7 +1527,7 @@ class ModelHolder:
         from .boost import BASE_NETWORKS
         if boost and model_type not in BASE_NETWORKS:
             raise NotImplementedError(f"BOOST is implemented in depthmap_b200 for the base networks LeReS res101 (model type 0), "
-                                      f"DPT-BEiT-L 512 / 384 (1, 2) and DPT-Large 384 (3), not for model type {model_type}")
+                                      f"DPT-BEiT-L 512 / 384 (1, 2), DPT-Large 384 (3) and MiDaS v2.1 (5), not for model type {model_type}")
         if getattr(self, "no_half", False):
             # reference: `no_half` keeps the network in fp32 (src/depthmap_generation.py:268-275).  The H100 path feeds the tensor
             # cores fp16 operands (fp32 accumulation, fp32 residual stream) and has no fp32-operand variant: say so instead of
@@ -1348,7 +1536,7 @@ class ModelHolder:
                                       "with fp32 accumulation; unset the setting")
         if model_type not in CHECKPOINTS:
             raise NotImplementedError(f"model_type {model_type} is not implemented in depthmap_b200 yet "
-                                      f"(implemented: 0 = LeReS res101; 1, 2 = DPT-BEiT-L 512/384; 3 = DPT-Large 384; 7 = ZoeDepth-N; "
+                                      f"(implemented: 0 = LeReS res101; 1, 2 = DPT-BEiT-L 512/384; 3 = DPT-Large 384; 5 = MiDaS v2.1; 7 = ZoeDepth-N; "
                                       f"8 = ZoeDepth-K; 9 = ZoeDepth-NK; 12, 13, 14 = Depth-Anything-V2 S/B/L)")
         dev = torch.device(device)
         path, unwrap, make = CHECKPOINTS[model_type]
@@ -1358,7 +1546,7 @@ class ModelHolder:
             self.pix2pix_model = BoostPipeline(model, UnetMergeEngine(self._load_checkpoint("pix2pix", PIX2PIX_CHECKPOINT), dev), dev, model_type)
         self.depth_model = model
         self.depth_model_type = model_type
-        self.resize_mode = "minimal"
+        self.resize_mode = "upper_bound" if model_type == 5 else "minimal"
         self.normalization = None
         self.tiling_mode = tiling_mode
         self.device = device
@@ -1421,7 +1609,7 @@ class ModelHolder:
             import torch
             preds = [self.pix2pix_model.run(rgb[i].cpu().numpy(), self.boost_rmax, to_host=False) for i in range(rgb.shape[0])]
             return torch.stack(preds), self.depth_model_type in [0, 7, 8, 9, 10]
-        if self.depth_model_type in (0, 1, 2, 3, 7, 8, 9, 12, 13, 14):
+        if self.depth_model_type in (0, 1, 2, 3, 5, 7, 8, 9, 12, 13, 14):
             pred = self.depth_model.forward_batch(rgb, net_width, net_height)
         else:
             raise NotImplementedError(f"model_type {self.depth_model_type}")
