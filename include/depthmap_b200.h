@@ -151,6 +151,20 @@ int dm_circular_halo_f16(const void *act, int B, int H, int W, int C, void *halo
  * the implicit GEMM over it.  Two kernels. */
 int dm_conv3x3_circular_ex(const void *act, void *halo, int B, int H, int W, int Cin, const void *Wt, const dm_gemm_desc *desc_host,
                            void *stream);
+/* Split mode (fp32-class GEMM for no_half).  A split tensor stores an fp32 value v as fp16 hi = rn(v), lo = rn(v - hi), each
+ * row of logical width n as [hi | lo | hi] (3n halves; NHWC tensors per pixel).  Split weights [N, K] are the pre-scaled fp32
+ * weights w * 2^e[n] packed [w_hi | w_hi | w_lo] (a conv filter per tap), wscale[n] = 2^-e[n] (fp32, 8-byte aligned).
+ * dm_gemm_split_ex: A split [M, K/3 logical] with desc->K = the tripled depth (K % 64 == 0); the epilogue multiplies the
+ * accumulator by wscale, then applies the desc's epilogue.  STORE_F16 / PIXSHUF write split outputs (C rows of pitch
+ * ldc >= 3N: hi at column n, lo at N + n, hi at 2N + n; pixel shuffle: 3*ps_cout halves per output pixel), C2 the split relu
+ * copy, R / R2 are split residuals (pitches >= 3N); RESID_F32, STORE_F32 and HEAD write fp32 as in dm_gemm_ex.  The tensor
+ * core's truncating accumulator is added into an fp32 register sum every 4 k-blocks (gemm_wgmma.cu). */
+int dm_gemm_split_ex(const void *A, int lda, const void *W, int ldw, const float *wscale, const dm_gemm_desc *desc_host, void *stream);
+/* Split 3x3 pad-1 conv: act split NHWC [B, H, W, 3*Cin] (Cin logical, % 64 == 0), Wt split [Cout, 9*3*Cin] per tap; desc->ldc /
+ * ldr / ldr2 are the output / residual pixel pitches (>= 3 Cout).  halo: NULL = zero padding (one kernel), else circular
+ * padding through the halo scratch, B*(H+2)*(W+2)*3*Cin halves (two kernels). */
+int dm_conv3x3_split_ex(const void *act, void *halo, int B, int H, int W, int Cin, const void *Wt, const float *wscale,
+                        const dm_gemm_desc *desc_host, void *stream);
 /* convenience wrappers used by the unit tests */
 int dm_gemm_f16(const void *A, int lda, const void *W, int ldw, const float *bias, void *C, int ldc, int M, int N, int K,
                 int act, int out_f32, void *stream);
@@ -164,12 +178,18 @@ int dm_attention_f16(const void *qkv, int B, int N, int H, float scale, const vo
  * nrd = (2gh-1)(2gw-1)+3, N = gh*gw+1 tokens (class token first).  No [H,N,N] bias tensor is read by the kernel. */
 int dm_attention_relpos_f16(const void *qkv, int B, int gh, int gw, int H, float scale, const float *rel_table_log2e,
                             int nrd, void *out, void *stream);
+/* Split attention (no_half): softmax(scale * Q K^T) V, head_dim 64, any N >= 2, from the split qkv [B*N, 9*H*64] (rows
+ * [hi | lo | hi] of the 3*H*64 q, k, v) to the split output [B*N, 3*H*64]; fp32 softmax and running output. */
+int dm_attention_split(const void *qkv, int B, int N, int H, float scale, void *out, void *stream);
 /* Any window: per 128-key tile the kernel stages only the table rows the tile pair spans, read from L2 (the table is at most
  * ~160 KB per head at 100 x 100). */
 /* uint8 RGB [B,H,W,3] -> (cv2-style bicubic resize to net_h x net_w) -> (x/255 - mean)/std -> fp16 patch matrix
  * [B*(net_h/patch)*(net_w/patch), kpad], K ordered (c, ky, kx); network channel c reads source channel chan_map[c]. */
 int dm_preprocess_patchify(const uint8_t *rgb, int B, int H, int W, int net_h, int net_w, int patch, const float *mean_host,
                            const float *std_host, const int *chan_map_host, void *out, int kpad, void *stream);
+/* The same into a split patch matrix [B*(net_h/patch)*(net_w/patch), 3*kpad] (the normalised values are fp32 before the split) */
+int dm_preprocess_patchify_split(const uint8_t *rgb, int B, int H, int W, int net_h, int net_w, int patch, const float *mean_host,
+                                 const float *std_host, const int *chan_map_host, void *out, int kpad, void *stream);
 /* The same for B crops of one planar fp32 image [3, Hi, Wi] (values used as they are, no /255), all resized to net_h x net_w:
  * rects_dev: DEVICE int32 [B][4] = x0, y0, w, h inside the image (validated by the caller), 16-byte aligned (DM_E_INVALID
  * otherwise).  BOOST's estimatemidasBoost
@@ -180,10 +200,18 @@ int dm_preprocess_patchify_f32_crops(const float *img, int Hi, int Wi, const int
                                      void *stream);
 /* X[b,0,:] = cls + pos[0]; X[b,1+p,:] = pe[b*Np+p,:] + pos[1+p]  (pos may be NULL); X fp32 [B, Np+1, C] */
 int dm_assemble_tokens(const void *pe, const float *cls, const float *pos, float *X, int B, int Np, int C, void *stream);
+/* the same with an fp32 patch embedding pe [B*Np, C] */
+int dm_assemble_tokens_f32(const float *pe, const float *cls, const float *pos, float *X, int B, int Np, int C, void *stream);
 /* LayerNorm over the last dim of fp32 x [rows, C] -> fp16; drop_first != 0 skips token 0 of every image (tokens_per_img) */
 int dm_layernorm_f16(const float *x, long long rows, int C, const float *gamma, const float *beta, float eps, void *out,
                      int tokens_per_img, int drop_first, void *stream);
+/* the same with a split output [rows, 3C] (C = 384, 768 or 1024) */
+int dm_layernorm_split(const float *x, long long rows, int C, const float *gamma, const float *beta, float eps, void *out,
+                       int tokens_per_img, int drop_first, void *stream);
 int dm_resize_bilinear_nhwc_f16(const void *in, int B, int Hin, int Win, int C, void *out, int Hout, int Wout, void *stream);
+/* bilinear align_corners=True resize of a split NHWC tensor [B, Hin, Win, 3C] (C logical, % 4 == 0): hi + lo interpolated in
+ * fp32, re-split */
+int dm_resize_bilinear_nhwc_split(const void *in, int B, int Hin, int Win, int C, void *out, int Hout, int Wout, void *stream);
 /* mode 0: bilinear align_corners=True; mode 1: bicubic align_corners=False */
 int dm_resize_f32(const float *in, int B, int Hin, int Win, float *out, int Hout, int Wout, int mode, void *stream);
 int dm_im2col_s2_f16(const void *in, int B, int H, int W, int C, void *out, void *stream);

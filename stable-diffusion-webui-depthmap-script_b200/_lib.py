@@ -88,6 +88,8 @@ EXPORTS = [
     "dm_leres_stem_im2col_f32_circular", "dm_leres_stem_im2col_f32_batch_circular",
     "dm_midas_stem_im2col", "dm_midas_stem_im2col_circular", "dm_midas_stem_im2col_f32_crops", "dm_midas_stem_im2col_f32_crops_circular",
     "dm_resize_bilinear_half_nhwc_f16",
+    "dm_gemm_split_ex", "dm_conv3x3_split_ex", "dm_attention_split", "dm_preprocess_patchify_split", "dm_assemble_tokens_f32",
+    "dm_layernorm_split", "dm_resize_bilinear_nhwc_split",
 ]
 
 
@@ -158,9 +160,12 @@ def _bind_optional(L):
         L.dm_conv3x3_ex.argtypes = [vp, i32, i32, i32, i32, vp, c.POINTER(GemmDesc), vp]
         L.dm_circular_halo_f16.argtypes = [vp, i32, i32, i32, i32, vp, vp]
         L.dm_conv3x3_circular_ex.argtypes = [vp, vp, i32, i32, i32, i32, vp, c.POINTER(GemmDesc), vp]
+        L.dm_gemm_split_ex.argtypes = [vp, i32, vp, i32, vp, c.POINTER(GemmDesc), vp]
+        L.dm_conv3x3_split_ex.argtypes = [vp, vp, i32, i32, i32, i32, vp, vp, c.POINTER(GemmDesc), vp]
     if hasattr(L, "dm_attention_f16"):
         L.dm_attention_f16.argtypes = [vp, i32, i32, i32, f32, vp, i32, vp, vp]
         L.dm_attention_relpos_f16.argtypes = [vp, i32, i32, i32, i32, f32, vp, i32, vp, vp]
+        L.dm_attention_split.argtypes = [vp, i32, i32, i32, f32, vp, vp]
     if hasattr(L, "dm_layernorm_f16"):
         L.dm_preprocess_patchify.argtypes = [vp, i32, i32, i32, i32, i32, i32, c.POINTER(c.c_float), c.POINTER(c.c_float),
                                              c.POINTER(c.c_int), vp, i32, vp]
@@ -169,6 +174,10 @@ def _bind_optional(L):
         L.dm_assemble_tokens.argtypes = [vp, vp, vp, vp, i32, i32, i32, vp]
         L.dm_layernorm_f16.argtypes = [vp, c.c_longlong, i32, vp, vp, f32, vp, i32, i32, vp]
         L.dm_resize_bilinear_nhwc_f16.argtypes = [vp, i32, i32, i32, i32, vp, i32, i32, vp]
+        L.dm_preprocess_patchify_split.argtypes = L.dm_preprocess_patchify.argtypes
+        L.dm_assemble_tokens_f32.argtypes = L.dm_assemble_tokens.argtypes
+        L.dm_layernorm_split.argtypes = L.dm_layernorm_f16.argtypes
+        L.dm_resize_bilinear_nhwc_split.argtypes = L.dm_resize_bilinear_nhwc_f16.argtypes
         L.dm_resize_f32.argtypes = [vp, i32, i32, i32, vp, i32, i32, i32, vp]
         L.dm_im2col_s2_f16.argtypes = [vp, i32, i32, i32, i32, vp, vp]
         L.dm_im2col_s2_circular_f16.argtypes = [vp, i32, i32, i32, i32, vp, vp]
@@ -292,6 +301,23 @@ class Ops:
             if halo.numel() < B * (H + 2) * (W_ + 2) * Cin:
                 raise ValueError(f"conv3x3: halo scratch of {halo.numel()} elements is too small for [{B}, {H + 2}, {W_ + 2}, {Cin}]")
             self.call("dm_conv3x3_circular_ex", act_t, halo, B, H, W_, Cin, Wt, ctypes.byref(d), launches=2)
+
+
+    def gemm_split(self, A, lda, W, ldw, wscale, M, N, K, epi=EPI_STORE_F16, act=ACT_NONE, bias=None, C=None, ldc=0, C2=None,
+                   R=None, ldr=0, R2=None, ldr2=0, X=None, ldx=0, gamma=None, head_b2=0.0, ps=None):
+        """split-mode GEMM (dm_gemm_split_ex): A, W split operands of depth K (3x the logical one), wscale the weights' [N] factor;
+        ldc / ldr / ldr2 are the split rows' pitches (>= 3N)"""
+        d = _gemm_desc(M, N, K, epi, act, bias, C, ldc, C2, R, ldr, R2, ldr2, X, ldx, gamma, head_b2, ps)
+        self.call("dm_gemm_split_ex", A, lda, W, ldw, wscale, ctypes.byref(d))
+
+    def conv3x3_split(self, act_t, B, H, W_, Cin, Wt, wscale, Cout, epi=EPI_STORE_F16, act=ACT_NONE, bias=None, C=None, C2=None,
+                      R=None, R2=None, X=None, gamma=None, head_b2=0.0, ldx=1, halo=None):
+        """split-mode pad-1 3x3 convolution on split NHWC activations (Cin, Cout logical); circular padding with a `halo` scratch
+        of at least B*(H+2)*(W_+2)*3*Cin fp16"""
+        d = _gemm_desc(0, Cout, 0, epi, act, bias, C, 3 * Cout, C2, R, 3 * Cout, R2, 3 * Cout, X, ldx, gamma, head_b2)
+        if halo is not None and halo.numel() < B * (H + 2) * (W_ + 2) * 3 * Cin:
+            raise ValueError(f"conv3x3_split: halo scratch of {halo.numel()} elements is too small for [{B}, {H + 2}, {W_ + 2}, {3 * Cin}]")
+        self.call("dm_conv3x3_split_ex", act_t, halo, B, H, W_, Cin, Wt, wscale, ctypes.byref(d), launches=1 if halo is None else 2)
 
 
 class GraphCache:

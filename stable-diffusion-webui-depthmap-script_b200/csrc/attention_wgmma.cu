@@ -287,7 +287,192 @@ int attention_f16(const __half *qkv, AttnParams p, cudaStream_t stream, const fl
     return p.bias ? launch_attn<1>(tm, p, stream) : launch_attn<0>(tm, p, stream);
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Split attention (the fp32-class path of no_half, bias mode 0): qkv is a split tensor [B*N, 9C], each row [hi | lo | hi] of the
+// 3C-wide q, k, v; the output is split [B*N, 3C].  Same skeleton as above, with hi and lo tiles of Q, K and V in shared memory
+// (160 KB).  Per KV tile:
+//   S = Q_lo K_hi^T + Q_hi K_lo^T + Q_hi K_hi^T   twelve m64n128k16: the small cross terms go first, so the accumulator's
+//                                                 alignment truncation only acts at the magnitude of S for the last four
+//   fp32 online softmax; p = 2^(u - m) * 2^12 split into p_hi + p_lo (the 2^12 keeps p_lo out of the fp16 subnormals for
+//   p > 2^-15; it cancels against the row sum, which adds the same unsplit fp32 values)
+//   PV = P_lo V_hi + P_hi V_lo + P_hi V_hi     twenty-four m64n64k16 into a FRESH accumulator, then O = O * alpha + PV by FFMA,
+//                                              so the running O never sits in a truncating accumulator across KV tiles
+// ---------------------------------------------------------------------------------------------------------------------
+constexpr int AS_K_OFF = 2 * AT_Q_BYTES;                          // Q hi | Q lo, then per stage K hi | K lo, then V hi | V lo
+constexpr int AS_V_OFF = AS_K_OFF + AT_STAGES * 2 * AT_KV_BYTES;
+constexpr int AS_BAR_OFF = AS_V_OFF + AT_STAGES * 2 * AT_KV_BYTES;
+constexpr int AS_SMEM = AS_BAR_OFF + 64;
+
+__global__ void __launch_bounds__(AT_THREADS, 1) attention_split_kernel(const __grid_constant__ CUtensorMap tmQKV, AttnParams p) {
+    extern __shared__ __align__(1024) uint8_t smem_raw[];
+    uint8_t *sQ = smem_raw, *sK = smem_raw + AS_K_OFF, *sV = smem_raw + AS_V_OFF;
+    uint64_t *bars = reinterpret_cast<uint64_t *>(smem_raw + AS_BAR_OFF);
+    uint64_t *q_full = bars, *kv_full = bars + 1, *kv_empty = bars + 1 + AT_STAGES;
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int q0 = blockIdx.x * AT_BQ, h = blockIdx.y, b = blockIdx.z;
+    const int num_kv = (p.N + AT_BKV - 1) / AT_BKV;
+    const int row_base = b * p.N;
+    const int lo = 3 * p.C;                   // column offset of the lo halves in a qkv row
+
+    if (threadIdx.x == 0) {
+        prefetch_tmap(&tmQKV);
+        mbar_init(q_full, 1);
+        for (int s = 0; s < AT_STAGES; ++s) { mbar_init(&kv_full[s], 1); mbar_init(&kv_empty[s], 8); }
+        fence_barrier_init();
+    }
+    __syncthreads();
+
+    if (warp < 4) {
+        if (threadIdx.x == 0) {
+            mbar_arrive_expect_tx(q_full, 2 * AT_Q_BYTES);
+            tma_load_2d(sQ, &tmQKV, q_full, h * AT_D, row_base + q0);
+            tma_load_2d(sQ + AT_Q_BYTES, &tmQKV, q_full, lo + h * AT_D, row_base + q0);
+            for (int j = 0; j < num_kv; ++j) {
+                const int s = j % AT_STAGES, r = row_base + j * AT_BKV;
+                uint8_t *k = sK + s * 2 * AT_KV_BYTES, *v = sV + s * 2 * AT_KV_BYTES;
+                mbar_wait(&kv_empty[s], ((j / AT_STAGES) & 1) ^ 1);
+                mbar_arrive_expect_tx(&kv_full[s], 4 * AT_KV_BYTES);
+                tma_load_2d(k, &tmQKV, &kv_full[s], p.C + h * AT_D, r);
+                tma_load_2d(k + AT_KV_BYTES, &tmQKV, &kv_full[s], lo + p.C + h * AT_D, r);
+                tma_load_2d(v, &tmQKV, &kv_full[s], 2 * p.C + h * AT_D, r);
+                tma_load_2d(v + AT_KV_BYTES, &tmQKV, &kv_full[s], lo + 2 * p.C + h * AT_D, r);
+            }
+        }
+        return;
+    }
+
+    const int wg = (warp >> 2) - 1, t = lane & 3;
+    int qi[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) qi[r] = q0 + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * r;
+    float o[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[i] = 0.f;
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+    const uint64_t qh_desc = make_desc_kmajor_sw128(smem_u32(sQ) + wg * (64 * 128));
+    const uint64_t ql_desc = make_desc_kmajor_sw128(smem_u32(sQ + AT_Q_BYTES) + wg * (64 * 128));
+
+    mbar_wait(q_full, 0);
+    for (int j = 0; j < num_kv; ++j) {
+        const int s = j % AT_STAGES;
+        const int kbase = j * AT_BKV;
+        mbar_wait(&kv_full[s], (j / AT_STAGES) & 1);
+        float sc[64];
+        const uint32_t sk = smem_u32(sK + s * 2 * AT_KV_BYTES);
+        const uint64_t kh_desc = make_desc_kmajor_sw128(sk), kl_desc = make_desc_kmajor_sw128(sk + AT_KV_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < AT_D / 16; ++k) wgmma_ss<AT_BKV>(sc, ql_desc + (uint64_t)(2 * k), kh_desc + (uint64_t)(2 * k), k != 0);
+#pragma unroll
+        for (int k = 0; k < AT_D / 16; ++k) wgmma_ss<AT_BKV>(sc, qh_desc + (uint64_t)(2 * k), kl_desc + (uint64_t)(2 * k), 1);
+#pragma unroll
+        for (int k = 0; k < AT_D / 16; ++k) wgmma_ss<AT_BKV>(sc, qh_desc + (uint64_t)(2 * k), kh_desc + (uint64_t)(2 * k), 1);
+        wgmma_commit();
+        wgmma_wait<0>();
+        float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+        for (int c = 0; c < AT_BKV / 8; ++c) {
+            const int k0 = kbase + 8 * c + 2 * t;
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                float u0 = sc[4 * c + 2 * r] * p.scale_log2e, u1 = sc[4 * c + 2 * r + 1] * p.scale_log2e;
+                u0 = k0 < p.N ? u0 : -INFINITY;
+                u1 = k0 + 1 < p.N ? u1 : -INFINITY;
+                sc[4 * c + 2 * r] = u0; sc[4 * c + 2 * r + 1] = u1;
+                mx[r] = fmaxf(mx[r], fmaxf(u0, u1));
+            }
+        }
+        float alpha[2];
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+            mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+            const float m_new = fmaxf(m_run[r], mx[r]);
+            alpha[r] = ex2_approx(m_run[r] - m_new);
+            m_run[r] = m_new;
+        }
+        uint32_t ph[AT_BKV / 16][4], pl[AT_BKV / 16][4];
+        float ls[2] = {0.f, 0.f};
+#pragma unroll
+        for (int c = 0; c < AT_BKV / 8; ++c) {
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                const float e0 = ex2_approx(sc[4 * c + 2 * r] - m_run[r]) * 4096.f, e1 = ex2_approx(sc[4 * c + 2 * r + 1] - m_run[r]) * 4096.f;
+                ls[r] += e0 + e1;
+                const __half2 hi = __floats2half2_rn(e0, e1);
+                const float2 hf = __half22float2(hi);
+                const __half2 lo2 = __floats2half2_rn(e0 - hf.x, e1 - hf.y);
+                ph[c >> 1][(c & 1) * 2 + r] = *reinterpret_cast<const uint32_t *>(&hi);
+                pl[c >> 1][(c & 1) * 2 + r] = *reinterpret_cast<const uint32_t *>(&lo2);
+            }
+        }
+#pragma unroll
+        for (int r = 0; r < 2; ++r) l_run[r] = fmaf(l_run[r], alpha[r], ls[r]);
+        float pv[32];
+#pragma unroll
+        for (int i = 0; i < 32; ++i) pv[i] = 0.f;
+        const uint32_t sv = smem_u32(sV + s * 2 * AT_KV_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < AT_BKV / 16; ++k) wgmma_rs_n64_bt(pv, pl[k], make_desc_mnmajor_sw128(sv + k * 16 * 128));
+#pragma unroll
+        for (int k = 0; k < AT_BKV / 16; ++k) wgmma_rs_n64_bt(pv, ph[k], make_desc_mnmajor_sw128(sv + AT_KV_BYTES + k * 16 * 128));
+#pragma unroll
+        for (int k = 0; k < AT_BKV / 16; ++k) wgmma_rs_n64_bt(pv, ph[k], make_desc_mnmajor_sw128(sv + k * 16 * 128));
+        wgmma_commit();
+        wgmma_wait<0>();
+        if (lane == 0) mbar_arrive(&kv_empty[s]);
+#pragma unroll
+        for (int c = 0; c < AT_D / 8; ++c) {
+            o[4 * c] = fmaf(o[4 * c], alpha[0], pv[4 * c]); o[4 * c + 1] = fmaf(o[4 * c + 1], alpha[0], pv[4 * c + 1]);
+            o[4 * c + 2] = fmaf(o[4 * c + 2], alpha[1], pv[4 * c + 2]); o[4 * c + 3] = fmaf(o[4 * c + 3], alpha[1], pv[4 * c + 3]);
+        }
+    }
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+        float l = l_run[r];
+        l += __shfl_xor_sync(0xffffffffu, l, 1);
+        l += __shfl_xor_sync(0xffffffffu, l, 2);
+        if (qi[r] >= p.N) continue;
+        __half *dst = p.out + (size_t)(row_base + qi[r]) * (3 * p.C) + h * AT_D + 2 * t;
+#pragma unroll
+        for (int c = 0; c < AT_D / 8; ++c) {
+            const float v0 = o[4 * c + 2 * r] / l, v1 = o[4 * c + 2 * r + 1] / l;
+            const __half2 hi = __floats2half2_rn(v0, v1);
+            const float2 hf = __half22float2(hi);
+            *reinterpret_cast<__half2 *>(dst + 8 * c) = hi;
+            *reinterpret_cast<__half2 *>(dst + p.C + 8 * c) = __floats2half2_rn(v0 - hf.x, v1 - hf.y);
+            *reinterpret_cast<__half2 *>(dst + 2 * p.C + 8 * c) = hi;
+        }
+    }
+}
+
+int attention_split(const __half *qkv, AttnParams p, cudaStream_t stream) {
+    if (p.C != p.H * AT_D || p.H < 1) { set_error("dm_attention_split: head_dim must be 64"); return DM_E_UNSUPPORTED; }
+    if (p.N < 2 || p.B < 1 || !qkv || !p.out) { set_error("dm_attention_split: bad arguments (N >= 2 tokens, B >= 1)"); return DM_E_INVALID; }
+    CUtensorMap tm;
+    int rc = make_tmap_2d(&tm, qkv, (uint64_t)p.B * p.N, (uint64_t)9 * p.C, (uint64_t)9 * p.C, AT_BQ, AT_D);
+    if (rc) return rc;
+    static PerDeviceFlag configured;
+    if (!configured.test_and_set())
+        DM_CUDA_CHECK(cudaFuncSetAttribute(attention_split_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AS_SMEM));
+    dim3 grid((p.N + AT_BQ - 1) / AT_BQ, p.H, p.B);
+    attention_split_kernel<<<grid, AT_THREADS, AS_SMEM, stream>>>(tm, p);
+    DM_LAUNCH_CHECK("attention_split_kernel");
+    return DM_OK;
+}
+
 }  // namespace dm
+
+extern "C" __attribute__((visibility("default"))) int dm_attention_split(const void *qkv, int B, int N, int H, float scale, void *out, void *stream) {
+    dm::AttnParams p;
+    memset(&p, 0, sizeof(p));
+    p.B = B; p.N = N; p.H = H; p.C = H * 64;
+    p.scale_log2e = scale * 1.4426950408889634f;
+    p.out = (__half *)out;
+    return dm::attention_split((const __half *)qkv, p, (cudaStream_t)stream);
+}
 
 extern "C" __attribute__((visibility("default"))) int dm_attention_f16(const void *qkv, int B, int N, int H, float scale, const void *bias, int bias_ld,
                                                                     void *out, void *stream) {

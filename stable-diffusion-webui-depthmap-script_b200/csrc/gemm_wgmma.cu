@@ -23,6 +23,21 @@
 //                   of a row
 // Every output element sums the same k-blocks and 16-wide k-slices in the same order whatever the tile shape or schedule,
 // so the results do not depend on either.
+//
+// Split mode (gemm_split / conv3x3_split, the fp32-class path of no_half): an fp32 activation a is stored as fp16 a_hi =
+// rn(a), a_lo = rn(a - a_hi) in one tensor of 3x the width, each row [a_hi | a_lo | a_hi]; the weights are packed
+// [w_hi | w_hi | w_lo] after a per-output-channel power-of-two pre-scale (so the low halves stay normal), and the MMA over the
+// tripled depth forms a_hi w_hi + a_lo w_hi + a_hi w_lo.  The tensor core's fp32 accumulator aligns and truncates its partial
+// sums (tools/probe_tensor_core.py), a bias that grows with the number of k-steps accumulated in it, so the split mainloop
+// PROMOTES: every SPLIT_PROMOTE k-blocks it waits for its MMAs, adds the wgmma accumulator into a register-resident fp32 sum with
+// rounding FADDs and restarts the accumulator.  SPLIT_PROMOTE = 1 (64 of the tripled depth, four k-steps), chosen by measurement
+// (tools/probe_tensor_core.py's method, H100 SXM 80 GB at 700 W): with all-positive products the relative bias of the split GEMM
+// is -1.4e-7 at P = 1, -3.8e-7 at 2, -1.0e-6 at 4 and -5.3e-6 at 16 k-blocks, independent of K (fp32 torch.matmul: 1e-9); its
+// largest error on random-sign data is 2.6-4.6x fp32's at P = 1, 2.2-2.9x at P = 4 and up to 8.2x at P = 16 (K = 1024 to
+// 49152); and P = 1 was also the fastest in that one run (ViT-L batch-32 fc2 / fc1 / qkv: 423 / 299 / 322 TFLOP/s of MMA work,
+// against 369 / 293 / 306 at P = 4).  The extra fp32 sum doubles the accumulator registers, so split tiles are 128 x 64 (or
+// 128 x 32): 168 registers, no spills.
+// Split epilogues undo the pre-scale, apply bias / activation / residual in fp32 and store split outputs (or fp32 ones).
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <math.h>
@@ -63,6 +78,8 @@ struct GemmParams {
     // implicit conv: tap offset into the tensor map, 0 = the activations themselves, 1 = their [B, H+2, W+2, Cin] halo copy (circular
     // padding).  Last, so that the other fields keep their offsets and the plain GEMM kernels their code
     int corg;
+    // split mode: [N] fp32 factor undoing the weights' power-of-two pre-scale
+    const float *wscale;
 };
 
 // BM x BN = the output tile of ONE consumer warpgroup.  The ring takes what the 227 KB of shared memory allows, up to 8
@@ -77,6 +94,7 @@ struct GemmCfg {
     static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 256 /*barriers*/;   // base is __align__(1024)
 };
 constexpr int GEMM_THREADS = 384;
+constexpr int SPLIT_PROMOTE = 1;    // split mode: k-blocks per wgmma accumulator before it is added into the fp32 sum (header)
 
 // exact-erf GELU, one MUFU.  With u = min(|x|, 5.75):
 //     gelu(x) = max(x, 0) - u * 2^(-u Q(u) - 1),      Q(u) = -log2(erfc(u / sqrt 2)) / u
@@ -97,11 +115,24 @@ __device__ __forceinline__ float gelu_erf(float x) {
     return fmaf(-u, e, fmaxf(x, 0.f));
 }
 
+// (v0, v1) as split fp16 pairs: hi at dst, lo at dst + lo_off, hi again at dst + 2 lo_off
+__device__ __forceinline__ void split_store2(__half *dst, int lo_off, float v0, float v1) {
+    const __half2 hi = __floats2half2_rn(v0, v1);
+    const float2 hf = __half22float2(hi);
+    const __half2 lo = __floats2half2_rn(v0 - hf.x, v1 - hf.y);
+    *reinterpret_cast<__half2 *>(dst) = hi;
+    *reinterpret_cast<__half2 *>(dst + lo_off) = lo;
+    *reinterpret_cast<__half2 *>(dst + 2 * lo_off) = hi;
+}
+
 // Epilogue of one consumer thread: its accumulator fragment holds rows r0 = 16 * warp + lane / 4 and r0 + 8 of the
 // warpgroup's 64, and for every 8-column group j the columns 8j + 2 (lane % 4), +1 (tc_common.cuh).  EPI = p.epi, fixed at
 // compile time so that a tile's epilogue is only the code of its own mode: the fully unrolled epilogue of all modes is
 // larger than the instruction cache and would otherwise be streamed through it under the other warpgroup's main loop.
-template <int BN, int EPI>
+// SPLIT: the operands R / R2 are split tensors (lo halves p.N columns after the hi ones), the output is stored split (C,
+// C2: [hi | lo | hi] at column offsets 0, N, 2N; pixel shuffle: per output pixel, offsets 0, cout, 2 cout) and the
+// accumulator is multiplied by wscale[n] first.
+template <int BN, int EPI, bool SPLIT = false>
 __device__ __forceinline__ void epilogue_fragment(const GemmParams &p, const float (&acc)[BN / 2], const long long (&m)[2], const bool (&row_ok)[2],
                                                   int n_base, int lane) {
     // Column groups are taken JC at a time: every operand load of a chunk is issued before its first store, so the loads
@@ -111,8 +142,8 @@ __device__ __forceinline__ void epilogue_fragment(const GemmParams &p, const flo
     float head_acc[2] = {0.f, 0.f};
 #pragma unroll
     for (int j0 = 0; j0 < BN / 8; j0 += JC) {
-        float2 b2[JC], g2[JC], x[JC][2];
-        __half2 rv[JC][2], rv2[JC][2];
+        float2 b2[JC], g2[JC], x[JC][2], ws[JC];
+        __half2 rv[JC][2], rv2[JC][2], rl[JC][2], rl2[JC][2];
 #pragma unroll
         for (int jj = 0; jj < JC; ++jj) {
             const int n = n_base + 8 * (j0 + jj) + 2 * t;
@@ -120,6 +151,7 @@ __device__ __forceinline__ void epilogue_fragment(const GemmParams &p, const flo
             g2[jj] = make_float2(0.f, 0.f);
             if (n >= p.N) continue;
             if (p.bias) b2[jj] = __ldg(reinterpret_cast<const float2 *>(p.bias + n));
+            if (SPLIT) ws[jj] = __ldg(reinterpret_cast<const float2 *>(p.wscale + n));
             if (EPI == EPI_RESID_F32 || EPI == EPI_HEAD) g2[jj] = __ldg(reinterpret_cast<const float2 *>(p.gamma + n));
 #pragma unroll
             for (int r = 0; r < 2; ++r) {
@@ -128,6 +160,8 @@ __device__ __forceinline__ void epilogue_fragment(const GemmParams &p, const flo
                 if (EPI == EPI_STORE_F16 || EPI == EPI_PIXSHUF) {
                     if (p.R) rv[jj][r] = __ldg(reinterpret_cast<const __half2 *>(p.R + m[r] * p.ldr + n));
                     if (p.R2) rv2[jj][r] = __ldg(reinterpret_cast<const __half2 *>(p.R2 + m[r] * p.ldr2 + n));
+                    if (SPLIT && p.R) rl[jj][r] = __ldg(reinterpret_cast<const __half2 *>(p.R + m[r] * p.ldr + p.N + n));
+                    if (SPLIT && p.R2) rl2[jj][r] = __ldg(reinterpret_cast<const __half2 *>(p.R2 + m[r] * p.ldr2 + p.N + n));
                 }
             }
         }
@@ -139,7 +173,9 @@ __device__ __forceinline__ void epilogue_fragment(const GemmParams &p, const flo
 #pragma unroll
             for (int r = 0; r < 2; ++r) {
                 if (!row_ok[r]) continue;
-                float v0 = acc[4 * j + 2 * r] + b2[jj].x, v1 = acc[4 * j + 2 * r + 1] + b2[jj].y;
+                float v0, v1;
+                if (SPLIT) { v0 = fmaf(acc[4 * j + 2 * r], ws[jj].x, b2[jj].x); v1 = fmaf(acc[4 * j + 2 * r + 1], ws[jj].y, b2[jj].y); }
+                else { v0 = acc[4 * j + 2 * r] + b2[jj].x; v1 = acc[4 * j + 2 * r + 1] + b2[jj].y; }
                 if (EPI == EPI_RESID_F32) {
                     float2 xv = x[jj][r];
                     xv.x = fmaf(g2[jj].x, v0, xv.x); xv.y = fmaf(g2[jj].y, v1, xv.y);
@@ -154,6 +190,27 @@ __device__ __forceinline__ void epilogue_fragment(const GemmParams &p, const flo
                 else if (p.act == ACT_RELU) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
                 if (EPI == EPI_HEAD) {
                     head_acc[r] = fmaf(v1, g2[jj].y, fmaf(v0, g2[jj].x, head_acc[r]));
+                    continue;
+                }
+                if (SPLIT) {
+                    if (p.R) { const float2 f = __half22float2(rv[jj][r]), l = __half22float2(rl[jj][r]); v0 += f.x + l.x; v1 += f.y + l.y; }
+                    if (p.R2) { const float2 f = __half22float2(rv2[jj][r]), l = __half22float2(rl2[jj][r]); v0 += f.x + l.x; v1 += f.y + l.y; }
+                    __half *dst;
+                    int lo_off;
+                    if (EPI == EPI_PIXSHUF) {
+                        const int s = p.ps_s, ij = n / p.ps_cout, co = n % p.ps_cout;
+                        const int i = ij / s, jx = ij % s;
+                        const long long bb = m[r] / ((long long)p.ps_h * p.ps_w);
+                        const int rem = (int)(m[r] % ((long long)p.ps_h * p.ps_w));
+                        const int y = rem / p.ps_w, xx = rem % p.ps_w;
+                        dst = p.C + (((bb * (p.ps_h * s) + (y * s + i)) * (long long)(p.ps_w * s)) + (xx * s + jx)) * (3 * p.ps_cout) + co;
+                        lo_off = p.ps_cout;
+                    } else {
+                        dst = p.C + m[r] * p.ldc + n;
+                        lo_off = p.N;
+                    }
+                    split_store2(dst, lo_off, v0, v1);
+                    if (EPI != EPI_PIXSHUF && p.C2) split_store2(p.C2 + m[r] * p.ldc + n, lo_off, fmaxf(v0, 0.f), fmaxf(v1, 0.f));
                     continue;
                 }
                 if (p.R) { const float2 f = __half22float2(rv[jj][r]); v0 += f.x; v1 += f.y; }
@@ -201,9 +258,8 @@ __device__ __forceinline__ void conv_origin(const GemmParams &p, int m_blk, int 
     cx0 = (t % p.tiles_x) * p.wbox;
 }
 
-template <int BM, int BN, bool CONV>
-__global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA,
-                                                                     const __grid_constant__ CUtensorMap tmB, GemmParams p) {
+template <int BM, int BN, bool CONV, bool SPLIT>
+__device__ __forceinline__ void gemm_body(const CUtensorMap &tmA, const CUtensorMap &tmB, const GemmParams &p) {
     using Cfg = GemmCfg<BM, BN>;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t *smem = smem_raw;
@@ -255,6 +311,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
     setmaxnreg_inc<232>();
     const int wg = (warp >> 2) - 1;
     float acc[Cfg::WM][BN / 2];
+    float sum[Cfg::WM][BN / 2];      // split mode: the promoted fp32 sum (unused otherwise)
     for (int i = wg; i < my_tiles; i += 2) {
         int m_blk, n_blk, cb = 0, cy0 = 0, cx0 = 0;
         tile_coords(p, blockIdx.x + i * gridDim.x, m_blk, n_blk);
@@ -265,6 +322,12 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
         // alternation is also what makes the parity waits below sound: every ring position before q0 has already been
         // waited for, so no full barrier is more than one phase behind this warpgroup's wait.
         if (i > 0) named_bar_sync(1 + wg, 256);
+        if (SPLIT) {
+#pragma unroll
+            for (int h = 0; h < Cfg::WM; ++h)
+#pragma unroll
+                for (int e = 0; e < BN / 2; ++e) sum[h][e] = 0.f;
+        }
         for (int kb = 0; kb < num_kb; ++kb) {
             mbar_wait(&full[stage], phase);
             const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES), sb = sa + Cfg::A_BYTES;
@@ -274,12 +337,20 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
             for (int k = 0; k < Cfg::BK / 16; ++k) {
 #pragma unroll
                 for (int h = 0; h < Cfg::WM; ++h)
-                    wgmma_ss<BN>(acc[h], make_desc_kmajor_sw128(sa + h * (64 * 128)) + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (kb | k) != 0);
+                    wgmma_ss<BN>(acc[h], make_desc_kmajor_sw128(sa + h * (64 * 128)) + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k),
+                                 SPLIT ? ((kb % SPLIT_PROMOTE) | k) != 0 : (kb | k) != 0);
             }
             wgmma_commit();
             if (kb > 0) {                       // the previous k-block's MMAs have retired: hand its slot back to the producer
                 wgmma_wait<1>();
                 if (lane == 0) mbar_arrive(&empty[prev]);
+            }
+            if (SPLIT && ((kb + 1) % SPLIT_PROMOTE == 0 || kb + 1 == num_kb)) {   // promotion: fp32 sum += accumulator
+                wgmma_wait<0>();
+#pragma unroll
+                for (int h = 0; h < Cfg::WM; ++h)
+#pragma unroll
+                    for (int e = 0; e < BN / 2; ++e) sum[h][e] = __fadd_rn(sum[h][e], acc[h][e]);
             }
             prev = stage;
             if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
@@ -304,15 +375,29 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __gri
                     row_ok[r] = m[r] < p.M;
                 }
             }
+            const float (&res)[BN / 2] = SPLIT ? sum[h] : acc[h];
             switch (p.epi) {
-                case EPI_STORE_F16: epilogue_fragment<BN, EPI_STORE_F16>(p, acc[h], m, row_ok, n_blk * BN, lane); break;
-                case EPI_RESID_F32: epilogue_fragment<BN, EPI_RESID_F32>(p, acc[h], m, row_ok, n_blk * BN, lane); break;
-                case EPI_PIXSHUF: epilogue_fragment<BN, EPI_PIXSHUF>(p, acc[h], m, row_ok, n_blk * BN, lane); break;
-                case EPI_HEAD: epilogue_fragment<BN, EPI_HEAD>(p, acc[h], m, row_ok, n_blk * BN, lane); break;
-                case EPI_STORE_F32: epilogue_fragment<BN, EPI_STORE_F32>(p, acc[h], m, row_ok, n_blk * BN, lane); break;
+                case EPI_STORE_F16: epilogue_fragment<BN, EPI_STORE_F16, SPLIT>(p, res, m, row_ok, n_blk * BN, lane); break;
+                case EPI_RESID_F32: epilogue_fragment<BN, EPI_RESID_F32, SPLIT>(p, res, m, row_ok, n_blk * BN, lane); break;
+                case EPI_PIXSHUF: epilogue_fragment<BN, EPI_PIXSHUF, SPLIT>(p, res, m, row_ok, n_blk * BN, lane); break;
+                case EPI_HEAD: epilogue_fragment<BN, EPI_HEAD, SPLIT>(p, res, m, row_ok, n_blk * BN, lane); break;
+                case EPI_STORE_F32: epilogue_fragment<BN, EPI_STORE_F32, SPLIT>(p, res, m, row_ok, n_blk * BN, lane); break;
             }
         }
     }
+}
+
+template <int BM, int BN, bool CONV>
+__global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA,
+                                                                     const __grid_constant__ CUtensorMap tmB, GemmParams p) {
+    gemm_body<BM, BN, CONV, false>(tmA, tmB, p);
+}
+
+// split mode (header): promoted mainloop, split epilogues
+template <int BM, int BN, bool CONV>
+__global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_split_kernel(const __grid_constant__ CUtensorMap tmA,
+                                                                     const __grid_constant__ CUtensorMap tmB, GemmParams p) {
+    gemm_body<BM, BN, CONV, true>(tmA, tmB, p);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -366,13 +451,16 @@ int make_tmap_nhwc(CUtensorMap *tm, const void *ptr, uint64_t B, uint64_t H, uin
 // (2-8 MB) across n; an activation panel is therefore read from HBM once and used for every n-tile while it is still in the
 // 50 MB L2, and the weights stay L2-resident for the whole call.  group_m bounds the activation panels of a group plus the
 // whole weight matrix by about half the L2 (the m fastest order re-read all of A once per weight panel).
-template <int BM, int BN, bool CONV>
+template <int BM, int BN, bool CONV, bool SPLIT = false>
 static int launch_gemm(const CUtensorMap &tmA, const CUtensorMap &tmB, GemmParams p, int m_tiles, cudaStream_t stream) {
     using Cfg = GemmCfg<BM, BN>;
     static PerDeviceFlag configured;
     static PerDeviceAttr sms(cudaDevAttrMultiProcessorCount);
+    void (*kernel)(const CUtensorMap, const CUtensorMap, GemmParams);
+    if constexpr (SPLIT) kernel = gemm_split_kernel<BM, BN, CONV>;
+    else kernel = gemm_wgmma_kernel<BM, BN, CONV>;
     if (!configured.test_and_set())
-        DM_CUDA_CHECK(cudaFuncSetAttribute(gemm_wgmma_kernel<BM, BN, CONV>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+        DM_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
     const long long l2_budget = 24ll << 20, w_bytes = 2ll * p.N * p.K, a_panel = 2ll * BM * p.K;   // conv: K = 9 Cin over-counts
     const long long g = (l2_budget - w_bytes) / a_panel;
     p.m_tiles = m_tiles;
@@ -380,8 +468,8 @@ static int launch_gemm(const CUtensorMap &tmA, const CUtensorMap &tmB, GemmParam
     p.group_m = (int)(g < 1 ? 1 : (g > m_tiles ? m_tiles : g));
     const int tiles = m_tiles * p.n_tiles;
     const int grid = tiles < sms.get() ? tiles : sms.get();   // persistent: one CTA per SM, never more CTAs than tiles
-    gemm_wgmma_kernel<BM, BN, CONV><<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, p);
-    DM_LAUNCH_CHECK("gemm_wgmma_kernel");
+    kernel<<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, p);
+    DM_LAUNCH_CHECK(SPLIT ? "gemm_split_kernel" : "gemm_wgmma_kernel");
     return DM_OK;
 }
 
@@ -415,6 +503,18 @@ static int pick_bn(const GemmParams &p) {
 }
 static int tile_m(int bn) { return bn == 256 ? 64 : 128; }
 
+// split mode: the weight-scale vector, and output / residual rows wide enough for their [hi | lo | hi] thirds
+static int check_split(const GemmParams &p, const char *who) {
+    if (!p.wscale || reinterpret_cast<uintptr_t>(p.wscale) % 8) { set_error("%s: wscale missing or not 8-byte aligned", who); return DM_E_INVALID; }
+    const bool f16_out = p.epi == EPI_STORE_F16;
+    if ((f16_out && p.ldc < 3 * p.N) || (p.R && p.ldr < 3 * p.N) || (p.R2 && p.ldr2 < 3 * p.N)) {
+        set_error("%s: split rows need pitches of at least 3N (N=%d ldc=%d ldr=%d ldr2=%d)", who, p.N, p.ldc, p.ldr, p.ldr2);
+        return DM_E_INVALID;
+    }
+    return DM_OK;
+}
+static int split_bn(const GemmParams &p) { const int bn = pick_bn(p); return bn > 64 ? 64 : bn; }
+
 // Plain GEMM: A fp16 [M, K] (pitch lda), W fp16 [N, K] (pitch ldw)
 int gemm_f16(const __half *A, int lda, const __half *W, int ldw, GemmParams p, cudaStream_t stream) {
     if (p.K % 64 != 0 || p.N % 32 != 0) { set_error("gemm_f16: K must be a multiple of 64 and N of 32 (K=%d N=%d)", p.K, p.N); return DM_E_INVALID; }
@@ -438,10 +538,29 @@ int gemm_f16(const __half *A, int lda, const __half *W, int ldw, GemmParams p, c
     return DM_E_UNSUPPORTED;
 }
 
+// Split GEMM: A = split activations [M, K] (K = 3x the logical depth), W = split weights [N, K], p.wscale set
+int gemm_split(const __half *A, int lda, const __half *W, int ldw, GemmParams p, cudaStream_t stream) {
+    if (p.K % 64 != 0 || p.N % 32 != 0) { set_error("gemm_split: K must be a multiple of 64 and N of 32 (K=%d N=%d)", p.K, p.N); return DM_E_INVALID; }
+    if (p.epi == EPI_HEAD && p.N != 32) { set_error("gemm_split: the fused head needs N = 32 (N=%d)", p.N); return DM_E_UNSUPPORTED; }
+    if (int rc0 = check_epilogue_operands(p, "gemm_split")) return rc0;
+    if (int rc0 = check_split(p, "gemm_split")) return rc0;
+    if ((lda % 8) || (ldw % 8)) { set_error("gemm_split: row pitches must be multiples of 8 elements"); return DM_E_INVALID; }
+    const int bn = split_bn(p);
+    const int m_tiles = (p.M + 127) / 128;
+    CUtensorMap tmA, tmB;
+    int rc = make_tmap_2d(&tmA, A, (uint64_t)p.M, (uint64_t)p.K, (uint64_t)lda, 128, 64);
+    if (rc) return rc;
+    rc = make_tmap_2d(&tmB, W, (uint64_t)p.N, (uint64_t)p.K, (uint64_t)ldw, (uint32_t)bn, 64);
+    if (rc) return rc;
+    return bn == 64 ? launch_gemm<128, 64, false, true>(tmA, tmB, p, m_tiles, stream) : launch_gemm<128, 32, false, true>(tmA, tmB, p, m_tiles, stream);
+}
+
 // 3x3 stride-1 convolution, NHWC fp16 activations [B,H,W,Cin], weights fp16 [Cout, 9*Cin] ordered (ky, kx, cin).  halo = 0: pad 1
 // with zeros, `src` is the activations; halo = 1: `src` is their [B, H+2, W+2, Cin] copy with the padding already in its border.
-static int conv3x3_launch(const __half *src, int halo, int B, int H, int W, int Cin, const __half *Wt, GemmParams p, cudaStream_t stream) {
-    const int bn = pick_bn(p), bm = tile_m(bn);
+// split: the split kernel (Cin is then the stored channel count, 3x the logical one)
+static int conv3x3_launch(const __half *src, int halo, int B, int H, int W, int Cin, const __half *Wt, GemmParams p, cudaStream_t stream,
+                          bool split = false) {
+    const int bn = split ? split_bn(p) : pick_bn(p), bm = tile_m(bn);
     // tile = hbox x wbox pixels = bm rows; choose the wbox in {bm, .., 16, 8} with the least padding waste
     int best_w = bm; double best_eff = -1;
     for (int wb = bm; wb >= 8; wb >>= 1) {
@@ -459,6 +578,7 @@ static int conv3x3_launch(const __half *src, int halo, int B, int H, int W, int 
     if (rc) return rc;
     rc = make_tmap_2d(&tmB, Wt, (uint64_t)p.N, (uint64_t)p.K, (uint64_t)p.K, (uint32_t)bn, 64);
     if (rc) return rc;
+    if (split) return bn == 64 ? launch_gemm<128, 64, true, true>(tmA, tmB, p, m_tiles, stream) : launch_gemm<128, 32, true, true>(tmA, tmB, p, m_tiles, stream);
     switch (bn) {
         case 256: return launch_gemm<64, 256, true>(tmA, tmB, p, m_tiles, stream);
         case 128: return launch_gemm<128, 128, true>(tmA, tmB, p, m_tiles, stream);
@@ -513,6 +633,16 @@ int conv3x3_circular_f16(const __half *act, __half *halo, int B, int H, int W, i
     if (int rc = check_conv3x3(p, Cin, "conv3x3_circular")) return rc;
     if (int rc = conv_halo_circular(act, B, H, W, Cin, halo, stream)) return rc;
     return conv3x3_launch(halo, 1, B, H, W, Cin, Wt, p, stream);
+}
+
+// Split 3x3 convolution: act = split NHWC [B, H, W, 3 Cin]; Wt = split weights [Cout, 9 * 3 Cin], each tap's columns
+// [w_hi | w_hi | w_lo]; halo != NULL: circular padding through the halo copy (B*(H+2)*(W+2)*3*Cin fp16)
+int conv3x3_split(const __half *act, __half *halo, int B, int H, int W, int Cin, const __half *Wt, GemmParams p, cudaStream_t stream) {
+    if (int rc = check_conv3x3(p, Cin, "conv3x3_split")) return rc;
+    if (int rc = check_split(p, "conv3x3_split")) return rc;
+    if (!halo) return conv3x3_launch(act, 0, B, H, W, 3 * Cin, Wt, p, stream, true);
+    if (int rc = conv_halo_circular(act, B, H, W, 3 * Cin, halo, stream)) return rc;
+    return conv3x3_launch(halo, 1, B, H, W, 3 * Cin, Wt, p, stream, true);
 }
 
 }  // namespace dm
@@ -573,3 +703,20 @@ extern "C" __attribute__((visibility("default"))) int dm_conv3x3_circular_ex(con
     return dm::conv3x3_circular_f16((const __half *)act, (__half *)halo, B, H, W, Cin, (const __half *)Wt, p, (cudaStream_t)stream);
 }
 
+extern "C" __attribute__((visibility("default"))) int dm_gemm_split_ex(const void *A, int lda, const void *W, int ldw, const float *wscale,
+                                                                    const dm_gemm_desc *d, void *stream) {
+    if (!A || !W || !d) { dm::set_error("dm_gemm_split_ex: null argument"); return DM_E_INVALID; }
+    dm::GemmParams p;
+    desc_to_params(d, p);
+    p.wscale = wscale;
+    return dm::gemm_split((const __half *)A, lda, (const __half *)W, ldw, p, (cudaStream_t)stream);
+}
+
+extern "C" __attribute__((visibility("default"))) int dm_conv3x3_split_ex(const void *act, void *halo, int B, int H, int W, int Cin, const void *Wt,
+                                                                       const float *wscale, const dm_gemm_desc *d, void *stream) {
+    if (!act || !Wt || !d) { dm::set_error("dm_conv3x3_split_ex: null argument"); return DM_E_INVALID; }
+    dm::GemmParams p;
+    desc_to_params(d, p);
+    p.wscale = wscale;
+    return dm::conv3x3_split((const __half *)act, (__half *)halo, B, H, W, Cin, (const __half *)Wt, p, (cudaStream_t)stream);
+}

@@ -10,6 +10,9 @@
 //   resize_f32           final depth resize: bilinear align_corners=True (DA-v2, src/depthmap_generation.py:558) or
 //                        bicubic align_corners=False (MiDaS, :487-497)
 //   im2col_s2            3x3 stride-2 pad-1 gather for the one strided conv of the reassemble stage (dpt.py:75-80)
+// Split variants (the fp32-class path of no_half, gemm_wgmma.cu): the patch matrix, LayerNorm output and NHWC resize store an
+// fp32 value v as fp16 hi = rn(v), lo = rn(v - hi) in rows [hi | lo | hi] of 3x the width; the assembly reads an fp32 patch
+// embedding.
 #include <cuda_fp16.h>
 #include <math.h>
 
@@ -29,20 +32,28 @@ struct PreParams {
     int kpad;            // padded K (>= 3*patch*patch, multiple of 64)
     float mean[3], inv_std[3];
     int chan_map[3];     // network channel c reads source channel chan_map[c]
-    __half *out;         // [B*gh*gw, kpad]
+    __half *out;         // [B*gh*gw, kpad]; split: [B*gh*gw, 3*kpad], rows [hi | lo | hi]
 };
 
 // normalise network pixel (y, x) of image b and store it into its patch row, K ordered (c, ky, kx)
+template <bool SPLIT = false>
 __device__ __forceinline__ void store_patch_pixel(const PreParams &p, int b, int y, int x, const float (&v)[3], float value_scale) {
     const int py = y / p.patch, ky = y % p.patch, pxi = x / p.patch, kx = x % p.patch;
-    __half *row = p.out + ((long long)(b * p.gh + py) * p.gw + pxi) * p.kpad;
+    __half *row = p.out + ((long long)(b * p.gh + py) * p.gw + pxi) * (SPLIT ? 3 * p.kpad : p.kpad);
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
         const float val = (v[p.chan_map[c]] * value_scale - p.mean[c]) * p.inv_std[c];
-        row[(c * p.patch + ky) * p.patch + kx] = __float2half_rn(val);
+        const int k = (c * p.patch + ky) * p.patch + kx;
+        const __half hi = __float2half_rn(val);
+        row[k] = hi;
+        if (SPLIT) {
+            row[p.kpad + k] = __float2half_rn(val - __half2float(hi));
+            row[2 * p.kpad + k] = hi;
+        }
     }
 }
 
+template <bool SPLIT>
 __global__ void __launch_bounds__(256) preprocess_patchify_kernel(PreParams p) {
     // one thread per (network pixel, channel triple): thread -> (b, y, x) of the network input
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -54,7 +65,7 @@ __global__ void __launch_bounds__(256) preprocess_patchify_kernel(PreParams p) {
     const U8Source src{p.rgb + (long long)b * p.H * p.W * 3, p.H, p.W};
     float v[3];
     cubic_sample(src, p.nh, p.nw, y, x, v);
-    store_patch_pixel(p, b, y, x, v, 1.0f / 255.0f);
+    store_patch_pixel<SPLIT>(p, b, y, x, v, 1.0f / 255.0f);
 }
 
 // BOOST crops: p.rgb unused; image b is the crop rects[b] = (x0, y0, w, h) of the planar fp32 image, values used as they are
@@ -83,7 +94,8 @@ __global__ void zero_pad_cols_kernel(__half *out, long long rows, int kused, int
 // ---------------------------------------------------------------------------------------------------------------
 // tokens = [cls ; patch embeddings] + pos
 // ---------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) assemble_tokens_kernel(const __half *__restrict__ pe, const float *__restrict__ cls,
+template <typename T>
+__global__ void __launch_bounds__(256) assemble_tokens_kernel(const T *__restrict__ pe, const float *__restrict__ cls,
                                                               const float *__restrict__ pos, float *__restrict__ X, int B, int Np, int C) {
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;  // one thread per 4 channels
     const int c4 = C / 4;
@@ -95,7 +107,9 @@ __global__ void __launch_bounds__(256) assemble_tokens_kernel(const __half *__re
     const int b = (int)(row / (Np + 1));
     float4 v;
     if (t == 0) v = *reinterpret_cast<const float4 *>(cls + c);
-    else {
+    else if constexpr (sizeof(T) == 4) {
+        v = *reinterpret_cast<const float4 *>(pe + ((long long)b * Np + (t - 1)) * C + c);
+    } else {
         const __half2 *h = reinterpret_cast<const __half2 *>(pe + ((long long)b * Np + (t - 1)) * C + c);
         const float2 a = __half22float2(h[0]), d = __half22float2(h[1]);
         v = make_float4(a.x, a.y, d.x, d.y);
@@ -107,10 +121,23 @@ __global__ void __launch_bounds__(256) assemble_tokens_kernel(const __half *__re
     *reinterpret_cast<float4 *>(X + row * C + c) = v;
 }
 
+// four consecutive fp32 values as split fp16: hi at dst, lo at dst + lo_off, hi again at dst + 2 lo_off (8-byte stores)
+__device__ __forceinline__ void store_split4(__half *dst, long long lo_off, const float (&y)[4]) {
+    const __half2 h0 = __floats2half2_rn(y[0], y[1]), h1 = __floats2half2_rn(y[2], y[3]);
+    const float2 f0 = __half22float2(h0), f1 = __half22float2(h1);
+    const __half2 l0 = __floats2half2_rn(y[0] - f0.x, y[1] - f0.y), l1 = __floats2half2_rn(y[2] - f1.x, y[3] - f1.y);
+    uint2 hu, lu;
+    hu.x = *reinterpret_cast<const uint32_t *>(&h0); hu.y = *reinterpret_cast<const uint32_t *>(&h1);
+    lu.x = *reinterpret_cast<const uint32_t *>(&l0); lu.y = *reinterpret_cast<const uint32_t *>(&l1);
+    *reinterpret_cast<uint2 *>(dst) = hu;
+    *reinterpret_cast<uint2 *>(dst + lo_off) = lu;
+    *reinterpret_cast<uint2 *>(dst + 2 * lo_off) = hu;
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 // LayerNorm: one warp per row, fp32 two-pass statistics in registers, fp16 output
 // ---------------------------------------------------------------------------------------------------------------
-template <int VEC>  // float4 loads per lane: C = 128 * VEC
+template <int VEC, bool SPLIT = false>  // float4 loads per lane: C = 128 * VEC; SPLIT: rows of 3C, [hi | lo | hi]
 __global__ void __launch_bounds__(256) layernorm_f16_kernel(const float *__restrict__ x, long long rows, int C, const float *__restrict__ gamma,
                                                             const float *__restrict__ beta, float eps, __half *__restrict__ out,
                                                             int tokens_per_img, int drop_first) {
@@ -141,11 +168,17 @@ __global__ void __launch_bounds__(256) layernorm_f16_kernel(const float *__restr
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) q += __shfl_xor_sync(0xffffffffu, q, o);
     const float rstd = rsqrtf(q / (float)C + eps);
-    __half *orow_p = out + orow * C;
+    __half *orow_p = out + orow * (SPLIT ? 3 * C : C);
 #pragma unroll
     for (int i = 0; i < VEC; ++i) {
         const int c = (lane + 32 * i) * 4;
         const float4 g = *reinterpret_cast<const float4 *>(gamma + c), bt = *reinterpret_cast<const float4 *>(beta + c);
+        if (SPLIT) {
+            const float y[4] = {(v[i].x - mean) * rstd * g.x + bt.x, (v[i].y - mean) * rstd * g.y + bt.y,
+                                (v[i].z - mean) * rstd * g.z + bt.z, (v[i].w - mean) * rstd * g.w + bt.w};
+            store_split4(orow_p + c, C, y);
+            continue;
+        }
         const __half2 h0 = __floats2half2_rn((v[i].x - mean) * rstd * g.x + bt.x, (v[i].y - mean) * rstd * g.y + bt.y);
         const __half2 h1 = __floats2half2_rn((v[i].z - mean) * rstd * g.z + bt.z, (v[i].w - mean) * rstd * g.w + bt.w);
         uint2 u;
@@ -192,6 +225,36 @@ __global__ void __launch_bounds__(256) resize_bilinear_nhwc_kernel(const __half 
         oh[k] = __floats2half2_rn(r0, r1);
     }
     __stcs(reinterpret_cast<uint4 *>(out + ((size_t)(b * Hout + y) * Wout + x) * C + c), o);
+}
+
+// the same on split tensors [B, H, W, 3C]: one thread per (output pixel, 4 channels), hi + lo interpolated in fp32, re-split
+__global__ void __launch_bounds__(256) resize_bilinear_nhwc_split_kernel(const __half *__restrict__ in, int Hin, int Win, int C,
+                                                                         __half *__restrict__ out, int Hout, int Wout, float sy, float sx) {
+    const int c4 = C >> 2;
+    const int t = blockIdx.x * 256 + threadIdx.x;
+    if (t >= Wout * c4) return;
+    const int x = t / c4;
+    const int c = (t - x * c4) << 2;
+    const int y = blockIdx.y, b = blockIdx.z;
+    const float fy = sy * (float)y, fx = sx * (float)x;
+    const int y0 = min((int)fy, Hin - 1), x0 = min((int)fx, Win - 1);
+    const int y1 = min(y0 + 1, Hin - 1), x1 = min(x0 + 1, Win - 1);
+    const float ly = fy - (float)y0, lx = fx - (float)x0, hy = 1.f - ly, hx = 1.f - lx;
+    const __half *base = in + (size_t)b * Hin * Win * 3 * C + c;
+    const size_t px[4] = {(size_t)(y0 * Win + x0) * 3 * C, (size_t)(y0 * Win + x1) * 3 * C, (size_t)(y1 * Win + x0) * 3 * C,
+                          (size_t)(y1 * Win + x1) * 3 * C};
+    float f[4][4];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+        const uint2 hu = __ldg(reinterpret_cast<const uint2 *>(base + px[q])), lu = __ldg(reinterpret_cast<const uint2 *>(base + px[q] + C));
+        const float2 h0 = __half22float2(*reinterpret_cast<const __half2 *>(&hu.x)), h1 = __half22float2(*reinterpret_cast<const __half2 *>(&hu.y));
+        const float2 l0 = __half22float2(*reinterpret_cast<const __half2 *>(&lu.x)), l1 = __half22float2(*reinterpret_cast<const __half2 *>(&lu.y));
+        f[q][0] = h0.x + l0.x; f[q][1] = h0.y + l0.y; f[q][2] = h1.x + l1.x; f[q][3] = h1.y + l1.y;
+    }
+    float r[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) r[k] = hy * (hx * f[0][k] + lx * f[1][k]) + ly * (hx * f[2][k] + lx * f[3][k]);
+    store_split4(out + ((size_t)(b * Hout + y) * Wout + x) * 3 * C + c, C, r);
 }
 
 // single-channel fp32 resize: mode 0 = bilinear align_corners=True, mode 1 = bicubic align_corners=False (A = -0.75)
@@ -305,7 +368,24 @@ DM_EXPORT int dm_preprocess_patchify(const uint8_t *rgb, int B, int H, int W, in
     const int rc = patchify_setup(p, B, net_h, net_w, patch, mean_host, std_host, chan_map_host, out, kpad, stream);
     if (rc) return rc;
     const long long total = (long long)B * net_h * net_w;
-    preprocess_patchify_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(p);
+    preprocess_patchify_kernel<false><<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(p);
+    DM_LAUNCH_CHECK("preprocess_patchify_kernel");
+    return DM_OK;
+}
+
+// split patch matrix [B*gh*gw, 3*kpad]: the zero fill treats each row as three rows of kpad
+DM_EXPORT int dm_preprocess_patchify_split(const uint8_t *rgb, int B, int H, int W, int net_h, int net_w, int patch, const float *mean_host,
+                                           const float *std_host, const int *chan_map_host, void *out, int kpad, void *stream_) {
+    using namespace dm;
+    if (!rgb || !out || net_h % patch || net_w % patch || kpad < 3 * patch * patch) { set_error("dm_preprocess_patchify_split: bad arguments"); return DM_E_INVALID; }
+    cudaStream_t stream = (cudaStream_t)stream_;
+    PreParams p;
+    p.rgb = rgb; p.H = H; p.W = W;
+    const int rc = patchify_setup(p, 3 * B, net_h, net_w, patch, mean_host, std_host, chan_map_host, out, kpad, stream);
+    if (rc) return rc;
+    p.B = B;
+    const long long total = (long long)B * net_h * net_w;
+    preprocess_patchify_kernel<true><<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(p);
     DM_LAUNCH_CHECK("preprocess_patchify_kernel");
     return DM_OK;
 }
@@ -333,7 +413,17 @@ DM_EXPORT int dm_assemble_tokens(const void *pe, const float *cls, const float *
     using namespace dm;
     if (C % 4) { set_error("dm_assemble_tokens: C must be a multiple of 4"); return DM_E_INVALID; }
     const long long total = (long long)B * (Np + 1) * (C / 4);
-    assemble_tokens_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream_>>>((const __half *)pe, cls, pos, X, B, Np, C);
+    assemble_tokens_kernel<__half><<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream_>>>((const __half *)pe, cls, pos, X, B, Np, C);
+    DM_LAUNCH_CHECK("assemble_tokens_kernel");
+    return DM_OK;
+}
+
+/* the same with an fp32 patch embedding [B*Np, C] */
+DM_EXPORT int dm_assemble_tokens_f32(const float *pe, const float *cls, const float *pos, float *X, int B, int Np, int C, void *stream_) {
+    using namespace dm;
+    if (C % 4) { set_error("dm_assemble_tokens_f32: C must be a multiple of 4"); return DM_E_INVALID; }
+    const long long total = (long long)B * (Np + 1) * (C / 4);
+    assemble_tokens_kernel<float><<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream_>>>(pe, cls, pos, X, B, Np, C);
     DM_LAUNCH_CHECK("assemble_tokens_kernel");
     return DM_OK;
 }
@@ -351,6 +441,35 @@ DM_EXPORT int dm_layernorm_f16(const float *x, long long rows, int C, const floa
         default: set_error("dm_layernorm_f16: unsupported width %d", C); return DM_E_UNSUPPORTED;
     }
     DM_LAUNCH_CHECK("layernorm_f16_kernel");
+    return DM_OK;
+}
+
+DM_EXPORT int dm_layernorm_split(const float *x, long long rows, int C, const float *gamma, const float *beta, float eps, void *out,
+                                 int tokens_per_img, int drop_first, void *stream_) {
+    using namespace dm;
+    cudaStream_t stream = (cudaStream_t)stream_;
+    const unsigned grid = (unsigned)((rows + 7) / 8);
+    switch (C) {
+        case 384: layernorm_f16_kernel<3, true><<<grid, 256, 0, stream>>>(x, rows, C, gamma, beta, eps, (__half *)out, tokens_per_img, drop_first); break;
+        case 768: layernorm_f16_kernel<6, true><<<grid, 256, 0, stream>>>(x, rows, C, gamma, beta, eps, (__half *)out, tokens_per_img, drop_first); break;
+        case 1024: layernorm_f16_kernel<8, true><<<grid, 256, 0, stream>>>(x, rows, C, gamma, beta, eps, (__half *)out, tokens_per_img, drop_first); break;
+        default: set_error("dm_layernorm_split: unsupported width %d", C); return DM_E_UNSUPPORTED;
+    }
+    DM_LAUNCH_CHECK("layernorm_f16_kernel");
+    return DM_OK;
+}
+
+DM_EXPORT int dm_resize_bilinear_nhwc_split(const void *in, int B, int Hin, int Win, int C, void *out, int Hout, int Wout, void *stream_) {
+    using namespace dm;
+    if (C % 4) { set_error("dm_resize_bilinear_nhwc_split: C must be a multiple of 4"); return DM_E_INVALID; }
+    if (Hout > 65535 || B > 65535 || (long long)Hin * Win * 3 * C >= (1ll << 31) || (long long)Hout * Wout * 3 * C >= (1ll << 31)) {
+        set_error("dm_resize_bilinear_nhwc_split: image too large for the 32-bit index path"); return DM_E_UNSUPPORTED;
+    }
+    const float sy = Hout > 1 ? (float)(Hin - 1) / (float)(Hout - 1) : 0.f;
+    const float sx = Wout > 1 ? (float)(Win - 1) / (float)(Wout - 1) : 0.f;
+    const dim3 grid((unsigned)((Wout * (C / 4) + 255) / 256), (unsigned)Hout, (unsigned)B);
+    resize_bilinear_nhwc_split_kernel<<<grid, 256, 0, (cudaStream_t)stream_>>>((const __half *)in, Hin, Win, C, (__half *)out, Hout, Wout, sy, sx);
+    DM_LAUNCH_CHECK("resize_bilinear_nhwc_split_kernel");
     return DM_OK;
 }
 

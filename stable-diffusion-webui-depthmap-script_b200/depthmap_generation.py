@@ -57,13 +57,38 @@ def dav2_net_size(width, height, target, multiple_of=14):
             _constrain_to_multiple_of(sh * height, multiple_of, min_val=target))
 
 
-def _conv_w(w, cin_pad, cout_pad):
-    """[Cout, Cin, 3, 3] -> fp16 [cout_pad, 9*cin_pad], K ordered (ky, kx, cin)."""
+def _conv_w(w, cin_pad, cout_pad, dtype=None):
+    """[Cout, Cin, 3, 3] -> [cout_pad, 9*cin_pad] (fp16 unless `dtype`), K ordered (ky, kx, cin)."""
     import torch
+    dtype = dtype or torch.float16
     co, ci = w.shape[:2]
-    t = torch.zeros(cout_pad, 3, 3, cin_pad, dtype=torch.float16, device=w.device)
-    t[:co, :, :, :ci] = w.permute(0, 2, 3, 1).to(torch.float16)
+    t = torch.zeros(cout_pad, 3, 3, cin_pad, dtype=dtype, device=w.device)
+    t[:co, :, :, :ci] = w.permute(0, 2, 3, 1).to(dtype)
     return t.reshape(cout_pad, 9 * cin_pad).contiguous()
+
+
+class SplitWeight:
+    """A GEMM / conv operand of the split (fp32-class) path: `t` fp16 [N, 3K], `scale` fp32 [N] (see split_weight)."""
+
+    def __init__(self, t, scale):
+        self.t, self.scale = t, scale
+
+
+def split_weight(m, groups=1):
+    """fp32 [N, K] -> SplitWeight for dm_gemm_split_ex / dm_conv3x3_split_ex.  Row n is pre-scaled by 2^e[n], the power of two
+    that brings its largest magnitude into [1024, 2048), so that the low halves of the weights are normal fp16 numbers (a trained
+    weight of 1e-2 has a low half near 2e-6, a subnormal); scale = 2^-e[n] undoes it in the epilogue.  The K columns are `groups`
+    runs (the taps of a 3x3 filter), each packed [w_hi | w_hi | w_lo] against the activations' [a_hi | a_lo | a_hi]."""
+    import torch
+    m = m.float()
+    N, K = m.shape
+    amax = m.abs().amax(dim=1)
+    e = torch.where(amax > 0, torch.floor(torch.log2(1024.0 / amax.clamp_min(1e-30))), torch.zeros_like(amax)).clamp(-100, 100)
+    ms = m * torch.exp2(e)[:, None]
+    hi = ms.half()
+    lo = (ms - hi.float()).half()
+    g = lambda t: t.reshape(N, groups, K // groups)
+    return SplitWeight(torch.cat([g(hi), g(hi), g(lo)], dim=2).reshape(N, 3 * K).contiguous(), torch.exp2(-e).contiguous())
 
 
 def _pad_vec(b, n):
@@ -81,7 +106,10 @@ class DepthAnythingV2Engine:
     final resize of estimatedepthanything_v2 (src/depthmap_generation.py:548-559).  Also the base of DptBeitEngine: the
     two families share the ViT block sequence and the whole DPT decoder and differ only in the hooks below.
     circular=True: tiling mode, every padded convolution (the decoder's 3x3 convs and the reassemble stage's stride-2 one) pads
-    circularly."""
+    circularly.
+    split=True: the fp32-class path of no_half.  Every GEMM / convolution operand is a split tensor (fp16 hi + lo, 3x the width,
+    gemm_wgmma.cu) against split weights, with promoted fp32 accumulation; the residual stream, LayerNorm statistics and softmax
+    are fp32.  Only Depth-Anything-V2 itself has it (SUPPORTS_SPLIT)."""
 
     PATCH = 14
     MEAN = (0.485, 0.456, 0.406)
@@ -91,13 +119,17 @@ class DepthAnythingV2Engine:
     CHAN_MAP = (2, 1, 0)
     FINAL_RESIZE_MODE = 0  # bilinear, align_corners=True (src/depthmap_generation.py:558)
     CONFIGS = DAV2_CONFIGS
+    SUPPORTS_SPLIT = True
 
-    def __init__(self, state_dict, encoder, device, circular=False):
+    def __init__(self, state_dict, encoder, device, circular=False, split=False):
         import torch
+        if split and not type(self).SUPPORTS_SPLIT:
+            raise NotImplementedError(f"{type(self).__name__} has no split (no_half) path; it is implemented for Depth-Anything-V2 only")
         self.cfg = self.CONFIGS[encoder]
         self.encoder = encoder
         self.device = device
         self.circular = circular
+        self.split = bool(split)
         self.ops = _lib.Ops()
         self._buf_key = None
         self._bufs = {}
@@ -110,14 +142,18 @@ class DepthAnythingV2Engine:
         dev = self.device
         cfg = self.cfg
         C, Fch, oc = cfg['embed_dim'], cfg['features'], cfg['out_channels']
-        f16 = lambda t: t.detach().to(dev, torch.float16).contiguous()
+        split = self.split
+        # GEMM / conv operands: fp16, or (split) built in fp32 and packed by split_weight; `groups` = the taps of a 3x3 filter
+        wdt = torch.float32 if split else torch.float16
+        op = (lambda t, groups=1: split_weight(t, groups)) if split else (lambda t, groups=1: t)
+        gw = lambda t: op(t.detach().to(dev, wdt).contiguous())
         f32 = lambda t: t.detach().to(dev, torch.float32).contiguous()
         w = {}
         pw = sd['pretrained.patch_embed.proj.weight'].detach().to(dev).reshape(C, -1)
         self.kpad = _ru(pw.shape[1], 64)
-        t = torch.zeros(C, self.kpad, dtype=torch.float16, device=dev)
-        t[:, :pw.shape[1]] = pw.to(torch.float16)
-        w['pe_w'], w['pe_b'] = t, f32(sd['pretrained.patch_embed.proj.bias'])
+        t = torch.zeros(C, self.kpad, dtype=wdt, device=dev)
+        t[:, :pw.shape[1]] = pw.to(wdt)
+        w['pe_w'], w['pe_b'] = op(t), f32(sd['pretrained.patch_embed.proj.bias'])
         w['cls'] = f32(sd['pretrained.cls_token']).reshape(C)
         self._pos_embed = f32(sd['pretrained.pos_embed'])
         blocks = []
@@ -125,11 +161,11 @@ class DepthAnythingV2Engine:
             p = f'pretrained.blocks.{i}.'
             blocks.append(dict(
                 ln1_w=f32(sd[p + 'norm1.weight']), ln1_b=f32(sd[p + 'norm1.bias']),
-                qkv_w=f16(sd[p + 'attn.qkv.weight']), qkv_b=f32(sd[p + 'attn.qkv.bias']),
-                proj_w=f16(sd[p + 'attn.proj.weight']), proj_b=f32(sd[p + 'attn.proj.bias']), ls1=f32(sd[p + 'ls1.gamma']),
+                qkv_w=gw(sd[p + 'attn.qkv.weight']), qkv_b=f32(sd[p + 'attn.qkv.bias']),
+                proj_w=gw(sd[p + 'attn.proj.weight']), proj_b=f32(sd[p + 'attn.proj.bias']), ls1=f32(sd[p + 'ls1.gamma']),
                 ln2_w=f32(sd[p + 'norm2.weight']), ln2_b=f32(sd[p + 'norm2.bias']),
-                fc1_w=f16(sd[p + 'mlp.fc1.weight']), fc1_b=f32(sd[p + 'mlp.fc1.bias']),
-                fc2_w=f16(sd[p + 'mlp.fc2.weight']), fc2_b=f32(sd[p + 'mlp.fc2.bias']), ls2=f32(sd[p + 'ls2.gamma'])))
+                fc1_w=gw(sd[p + 'mlp.fc1.weight']), fc1_b=f32(sd[p + 'mlp.fc1.bias']),
+                fc2_w=gw(sd[p + 'mlp.fc2.weight']), fc2_b=f32(sd[p + 'mlp.fc2.bias']), ls2=f32(sd[p + 'ls2.gamma'])))
         w['blocks'] = blocks
         w['norm_w'], w['norm_b'] = f32(sd['pretrained.norm.weight']), f32(sd['pretrained.norm.bias'])
         # ---- DPT head; channel counts padded to multiples of 64 with zero weights (ViT-S/B have 48/96-wide maps) ----
@@ -137,34 +173,35 @@ class DepthAnythingV2Engine:
         self.Fp = _ru(Fch, 64)
         self.F2p = _ru(Fch // 2, 64)
         h = 'depth_head.'
+        conv_w = lambda wt, ci, co: op(_conv_w(wt, ci, co, wdt), 9)
         for i in range(4):
-            t = torch.zeros(self.ocp[i], C, dtype=torch.float16, device=dev)
-            t[:oc[i]] = sd[h + f'projects.{i}.weight'].detach().to(dev).reshape(oc[i], C).to(torch.float16)
-            w[f'proj{i}_w'], w[f'proj{i}_b'] = t, _pad_vec(sd[h + f'projects.{i}.bias'].detach().to(dev), self.ocp[i])
+            t = torch.zeros(self.ocp[i], C, dtype=wdt, device=dev)
+            t[:oc[i]] = sd[h + f'projects.{i}.weight'].detach().to(dev).reshape(oc[i], C).to(wdt)
+            w[f'proj{i}_w'], w[f'proj{i}_b'] = op(t), _pad_vec(sd[h + f'projects.{i}.bias'].detach().to(dev), self.ocp[i])
         for i, s in ((0, 4), (1, 2)):  # ConvTranspose2d(k = s): W[(i,j,co), ci] = w[ci, co, i, j]
             wt = sd[h + f'resize_layers.{i}.weight'].detach().to(dev)  # [ci, co, s, s]
-            t = torch.zeros(s, s, self.ocp[i], self.ocp[i], dtype=torch.float16, device=dev)
-            t[:, :, :oc[i], :oc[i]] = wt.permute(2, 3, 1, 0).to(torch.float16)
-            w[f'up{i}_w'] = t.reshape(s * s * self.ocp[i], self.ocp[i]).contiguous()
+            t = torch.zeros(s, s, self.ocp[i], self.ocp[i], dtype=wdt, device=dev)
+            t[:, :, :oc[i], :oc[i]] = wt.permute(2, 3, 1, 0).to(wdt)
+            w[f'up{i}_w'] = op(t.reshape(s * s * self.ocp[i], self.ocp[i]).contiguous())
             w[f'up{i}_b'] = _pad_vec(sd[h + f'resize_layers.{i}.bias'].detach().to(dev), self.ocp[i]).repeat(s * s).contiguous()
-        w['down3_w'] = _conv_w(sd[h + 'resize_layers.3.weight'].detach().to(dev), self.ocp[3], self.ocp[3])
+        w['down3_w'] = conv_w(sd[h + 'resize_layers.3.weight'].detach().to(dev), self.ocp[3], self.ocp[3])
         w['down3_b'] = _pad_vec(sd[h + 'resize_layers.3.bias'].detach().to(dev), self.ocp[3])
         for i in range(4):
-            w[f'rn{i}_w'] = _conv_w(sd[h + f'scratch.layer{i + 1}_rn.weight'].detach().to(dev), self.ocp[i], self.Fp)
+            w[f'rn{i}_w'] = conv_w(sd[h + f'scratch.layer{i + 1}_rn.weight'].detach().to(dev), self.ocp[i], self.Fp)
         for i in range(1, 5):
             r = h + f'scratch.refinenet{i}.'
-            t = torch.zeros(self.Fp, self.Fp, dtype=torch.float16, device=dev)
-            t[:Fch, :Fch] = sd[r + 'out_conv.weight'].detach().to(dev).reshape(Fch, Fch).to(torch.float16)
-            w[f'rf{i}_out_w'], w[f'rf{i}_out_b'] = t, _pad_vec(sd[r + 'out_conv.bias'].detach().to(dev), self.Fp)
+            t = torch.zeros(self.Fp, self.Fp, dtype=wdt, device=dev)
+            t[:Fch, :Fch] = sd[r + 'out_conv.weight'].detach().to(dev).reshape(Fch, Fch).to(wdt)
+            w[f'rf{i}_out_w'], w[f'rf{i}_out_b'] = op(t), _pad_vec(sd[r + 'out_conv.bias'].detach().to(dev), self.Fp)
             for u in (1, 2):
                 for cv in (1, 2):
                     k = r + f'resConfUnit{u}.conv{cv}.'
                     if k + 'weight' in sd:
-                        w[f'rf{i}_u{u}c{cv}_w'] = _conv_w(sd[k + 'weight'].detach().to(dev), self.Fp, self.Fp)
+                        w[f'rf{i}_u{u}c{cv}_w'] = conv_w(sd[k + 'weight'].detach().to(dev), self.Fp, self.Fp)
                         w[f'rf{i}_u{u}c{cv}_b'] = _pad_vec(sd[k + 'bias'].detach().to(dev), self.Fp)
-        w['oc1_w'] = _conv_w(sd[h + 'scratch.output_conv1.weight'].detach().to(dev), self.Fp, self.F2p)
+        w['oc1_w'] = conv_w(sd[h + 'scratch.output_conv1.weight'].detach().to(dev), self.Fp, self.F2p)
         w['oc1_b'] = _pad_vec(sd[h + 'scratch.output_conv1.bias'].detach().to(dev), self.F2p)
-        w['oc2_w'] = _conv_w(sd[h + 'scratch.output_conv2.0.weight'].detach().to(dev), self.F2p, 32)
+        w['oc2_w'] = conv_w(sd[h + 'scratch.output_conv2.0.weight'].detach().to(dev), self.F2p, 32)
         w['oc2_b'] = f32(sd[h + 'scratch.output_conv2.0.bias'])
         w['oc3_w'] = f32(sd[h + 'scratch.output_conv2.2.weight']).reshape(32)
         self.oc3_b = float(sd[h + 'scratch.output_conv2.2.bias'].detach().float().reshape(-1)[0])
@@ -200,10 +237,13 @@ class DepthAnythingV2Engine:
         C, Fp = self.cfg['embed_dim'], self.Fp
         gh, gw = nh // self.PATCH, nw // self.PATCH
         Np, N = gh * gw, gh * gw + 1
-        h16 = lambda *s: torch.empty(*s, dtype=torch.float16, device=dev)
+        # split: every fp16 activation is a split tensor of 3x the width; the patch embedding is fp32 (the token assembly adds
+        # the class token and position embedding to it in fp32)
+        wide = 3 if self.split else 1
+        h16 = lambda *s: torch.empty(*s[:-1], wide * s[-1], dtype=torch.float16, device=dev)
         b = {}
         b['patches'] = h16(B * Np, self.kpad)
-        b['pe'] = h16(B * Np, C)
+        b['pe'] = torch.empty(B * Np, C, dtype=torch.float32, device=dev) if wide == 3 else h16(B * Np, C)
         b['x'] = torch.empty(B * N, C, dtype=torch.float32, device=dev)
         b['h'] = h16(B * N, C)
         b['qkv'] = h16(B * N, 3 * C)
@@ -243,11 +283,36 @@ class DepthAnythingV2Engine:
         return dav2_net_size(W, H, net_w)  # estimatedepthanything_v2 passes w as input_size (:552)
 
     def attention(self, i, b, B, N, heads, C, gh, gw):
+        if self.split:
+            self.ops.call("dm_attention_split", b['qkv'], B, N, heads, (C // heads) ** -0.5, b['att'])
+            return
         self.ops.call("dm_attention_f16", b['qkv'], B, N, heads, (C // heads) ** -0.5, None, 0, b['att'])
 
     def emit_feature(self, b, fi, B, N, C):
         """get_intermediate_layers(norm=True) without the class token (dinov2.py:297-321)."""
-        self.ops.call("dm_layernorm_f16", b['x'], B * N, C, self.w['norm_w'], self.w['norm_b'], 1e-6, b['feat'][fi], N, 1)
+        self.ops.call(self._ln, b['x'], B * N, C, self.w['norm_w'], self.w['norm_b'], 1e-6, b['feat'][fi], N, 1)
+
+    # ---- kernel calls of the two paths (split: the same layer on split operands, see split_weight) -----------------------
+    @property
+    def _ln(self):
+        return "dm_layernorm_split" if self.split else "dm_layernorm_f16"
+
+    @property
+    def _resize(self):
+        return "dm_resize_bilinear_nhwc_split" if self.split else "dm_resize_bilinear_nhwc_f16"
+
+    def _gemm(self, A, lda, W, ldw, M, N, K, **kw):
+        """ops.gemm, or its split form: depths and pitches of the split operands are 3x the logical ones (ldx is fp32's)"""
+        if not self.split:
+            return self.ops.gemm(A, lda, W, ldw, M, N, K, **kw)
+        if 'ldc' in kw:
+            kw['ldc'] *= 3
+        self.ops.gemm_split(A, 3 * lda, W.t, 3 * ldw, W.scale, M, N, 3 * K, **kw)
+
+    def _conv(self, x, B, H, W_, Cin, Wt, Cout, **kw):
+        if not self.split:
+            return self.ops.conv3x3(x, B, H, W_, Cin, Wt, Cout, **kw)
+        self.ops.conv3x3_split(x, B, H, W_, Cin, Wt.t, Wt.scale, Cout, **kw)
 
     # ---- forward ---------------------------------------------------------------------------------------------------
     def forward_batch(self, rgb, net_w, net_h=None, out_hw=None):
@@ -257,8 +322,9 @@ class DepthAnythingV2Engine:
         P_ = self.PATCH
         b = self._buffers(B, nh, nw)
         # image2tensor; the kernel zero-fills the patch matrix's K padding first, if it has any
-        self.ops.call("dm_preprocess_patchify", rgb, B, H, W, nh, nw, P_, (ctypes.c_float * 3)(*self.MEAN), (ctypes.c_float * 3)(*self.STD),
-                      (ctypes.c_int * 3)(*self.CHAN_MAP), b['patches'], self.kpad, launches=1 + (self.kpad > 3 * P_ * P_))
+        self.ops.call("dm_preprocess_patchify_split" if self.split else "dm_preprocess_patchify", rgb, B, H, W, nh, nw, P_,
+                      (ctypes.c_float * 3)(*self.MEAN), (ctypes.c_float * 3)(*self.STD), (ctypes.c_int * 3)(*self.CHAN_MAP), b['patches'],
+                      self.kpad, launches=1 + (self.kpad > 3 * P_ * P_))
         self.run_network(b, B, nh, nw)
         return self.run_head(b, B, H, W, nh, nw, out_hw)
 
@@ -271,59 +337,65 @@ class DepthAnythingV2Engine:
         gh, gw = nh // P_, nw // P_
         Np, N = gh * gw, gh * gw + 1
         # patch embedding + tokens
-        ops.gemm(b['patches'], self.kpad, w['pe_w'], self.kpad, B * Np, C, self.kpad, bias=w['pe_b'], C=b['pe'], ldc=C)
-        ops.call("dm_assemble_tokens", b['pe'], w['cls'], self._pos(gh, gw) if self._pos_embed is not None else None, b['x'], B, Np, C)
+        if self.split:
+            self._gemm(b['patches'], self.kpad, w['pe_w'], self.kpad, B * Np, C, self.kpad, epi=_lib.EPI_STORE_F32, bias=w['pe_b'], X=b['pe'], ldx=C)
+        else:
+            ops.gemm(b['patches'], self.kpad, w['pe_w'], self.kpad, B * Np, C, self.kpad, bias=w['pe_b'], C=b['pe'], ldc=C)
+        ops.call("dm_assemble_tokens_f32" if self.split else "dm_assemble_tokens", b['pe'], w['cls'],
+                 self._pos(gh, gw) if self._pos_embed is not None else None, b['x'], B, Np, C)
         rows = B * N
         fi = 0
         for i, blk in enumerate(w['blocks']):
-            ops.call("dm_layernorm_f16", b['x'], rows, C, blk['ln1_w'], blk['ln1_b'], 1e-6, b['h'], 1, 0)
-            ops.gemm(b['h'], C, blk['qkv_w'], C, rows, 3 * C, C, bias=blk['qkv_b'], C=b['qkv'], ldc=3 * C)
+            ops.call(self._ln, b['x'], rows, C, blk['ln1_w'], blk['ln1_b'], 1e-6, b['h'], 1, 0)
+            self._gemm(b['h'], C, blk['qkv_w'], C, rows, 3 * C, C, bias=blk['qkv_b'], C=b['qkv'], ldc=3 * C)
             self.attention(i, b, B, N, heads, C, gh, gw)
-            ops.gemm(b['att'], C, blk['proj_w'], C, rows, C, C, epi=_lib.EPI_RESID_F32, bias=blk['proj_b'], X=b['x'], ldx=C, gamma=blk['ls1'])
-            ops.call("dm_layernorm_f16", b['x'], rows, C, blk['ln2_w'], blk['ln2_b'], 1e-6, b['h'], 1, 0)
-            ops.gemm(b['h'], C, blk['fc1_w'], C, rows, 4 * C, C, act=_lib.ACT_GELU, bias=blk['fc1_b'], C=b['mlp'], ldc=4 * C)
-            ops.gemm(b['mlp'], 4 * C, blk['fc2_w'], 4 * C, rows, C, 4 * C, epi=_lib.EPI_RESID_F32, bias=blk['fc2_b'], X=b['x'], ldx=C, gamma=blk['ls2'])
+            self._gemm(b['att'], C, blk['proj_w'], C, rows, C, C, epi=_lib.EPI_RESID_F32, bias=blk['proj_b'], X=b['x'], ldx=C, gamma=blk['ls1'])
+            ops.call(self._ln, b['x'], rows, C, blk['ln2_w'], blk['ln2_b'], 1e-6, b['h'], 1, 0)
+            self._gemm(b['h'], C, blk['fc1_w'], C, rows, 4 * C, C, act=_lib.ACT_GELU, bias=blk['fc1_b'], C=b['mlp'], ldc=4 * C)
+            self._gemm(b['mlp'], 4 * C, blk['fc2_w'], 4 * C, rows, C, 4 * C, epi=_lib.EPI_RESID_F32, bias=blk['fc2_b'], X=b['x'], ldx=C, gamma=blk['ls2'])
             if i in cfg['layers']:
                 self.emit_feature(b, fi, B, N, C)
                 fi += 1
         # ---- DPT head (dpt.py:117-150) ----
         sizes = b['sizes']
         for i in range(4):
-            ops.gemm(b['feat'][i], C, w[f'proj{i}_w'], C, B * Np, self.ocp[i], C, bias=w[f'proj{i}_b'], C=b['p'][i], ldc=self.ocp[i])
-        ops.gemm(b['p'][0], self.ocp[0], w['up0_w'], self.ocp[0], B * Np, 16 * self.ocp[0], self.ocp[0], epi=_lib.EPI_PIXSHUF, bias=w['up0_b'],
-                 C=b['r'][0], ps=(4, self.ocp[0], gh, gw))
-        ops.gemm(b['p'][1], self.ocp[1], w['up1_w'], self.ocp[1], B * Np, 4 * self.ocp[1], self.ocp[1], epi=_lib.EPI_PIXSHUF, bias=w['up1_b'],
-                 C=b['r'][1], ps=(2, self.ocp[1], gh, gw))
+            self._gemm(b['feat'][i], C, w[f'proj{i}_w'], C, B * Np, self.ocp[i], C, bias=w[f'proj{i}_b'], C=b['p'][i], ldc=self.ocp[i])
+        self._gemm(b['p'][0], self.ocp[0], w['up0_w'], self.ocp[0], B * Np, 16 * self.ocp[0], self.ocp[0], epi=_lib.EPI_PIXSHUF, bias=w['up0_b'],
+                   C=b['r'][0], ps=(4, self.ocp[0], gh, gw))
+        self._gemm(b['p'][1], self.ocp[1], w['up1_w'], self.ocp[1], B * Np, 4 * self.ocp[1], self.ocp[1], epi=_lib.EPI_PIXSHUF, bias=w['up1_b'],
+                   C=b['r'][1], ps=(2, self.ocp[1], gh, gw))
         r2 = b['p'][2]
-        ops.call("dm_im2col_s2_circular_f16" if self.circular else "dm_im2col_s2_f16", b['p'][3], B, gh, gw, self.ocp[3], b['cols3'])
-        ops.gemm(b['cols3'], 9 * self.ocp[3], w['down3_w'], 9 * self.ocp[3], B * sizes[3][0] * sizes[3][1], self.ocp[3], 9 * self.ocp[3],
-                 bias=w['down3_b'], C=b['r'][3], ldc=self.ocp[3])
+        # the im2col is channel-agnostic: on a split tensor it gathers 3x the channels, which down3_w's per-tap split layout matches
+        ops.call("dm_im2col_s2_circular_f16" if self.circular else "dm_im2col_s2_f16", b['p'][3], B, gh, gw,
+                 self.ocp[3] * (3 if self.split else 1), b['cols3'])
+        self._gemm(b['cols3'], 9 * self.ocp[3], w['down3_w'], 9 * self.ocp[3], B * sizes[3][0] * sizes[3][1], self.ocp[3], 9 * self.ocp[3],
+                   bias=w['down3_b'], C=b['r'][3], ldc=self.ocp[3])
         rs = [b['r'][0], b['r'][1], r2, b['r'][3]]
         for i in range(4):  # layer{i}_rn (no bias) -> l_i and relu(l_i)
-            ops.conv3x3(rs[i], B, sizes[i][0], sizes[i][1], self.ocp[i], w[f'rn{i}_w'], Fp, C=b['l'][i], C2=b['lr'][i], halo=b['halo'])
+            self._conv(rs[i], B, sizes[i][0], sizes[i][1], self.ocp[i], w[f'rn{i}_w'], Fp, C=b['l'][i], C2=b['lr'][i], halo=b['halo'])
         # refinenet4: resConfUnit2(l4) -> resize -> out_conv.  The 1x1 out_conv (+ bias) commutes with the bilinear
         # interpolation (a per-pixel channel mix against per-channel spatial weights that sum to one), so it runs BEFORE the
         # up-sample: a quarter of the MACs and no full-resolution intermediate (dmidas/blocks.py:425-437 has it after).
         s3 = sizes[3]
-        ops.conv3x3(b['lr'][3], B, s3[0], s3[1], Fp, w['rf4_u2c1_w'], Fp, act=_lib.ACT_RELU, bias=w['rf4_u2c1_b'], C=b['t3'], halo=b['halo'])
-        ops.conv3x3(b['t3'], B, s3[0], s3[1], Fp, w['rf4_u2c2_w'], Fp, bias=w['rf4_u2c2_b'], C=b['u3'], R=b['l'][3], halo=b['halo'])
+        self._conv(b['lr'][3], B, s3[0], s3[1], Fp, w['rf4_u2c1_w'], Fp, act=_lib.ACT_RELU, bias=w['rf4_u2c1_b'], C=b['t3'], halo=b['halo'])
+        self._conv(b['t3'], B, s3[0], s3[1], Fp, w['rf4_u2c2_w'], Fp, bias=w['rf4_u2c2_b'], C=b['u3'], R=b['l'][3], halo=b['halo'])
         up = b['up_sizes']
-        ops.gemm(b['u3'], Fp, w['rf4_out_w'], Fp, B * s3[0] * s3[1], Fp, Fp, bias=w['rf4_out_b'], C=b['v'][0], ldc=Fp)
-        ops.call("dm_resize_bilinear_nhwc_f16", b['v'][0], B, s3[0], s3[1], Fp, b['path'][0], up[0][0], up[0][1])
+        self._gemm(b['u3'], Fp, w['rf4_out_w'], Fp, B * s3[0] * s3[1], Fp, Fp, bias=w['rf4_out_b'], C=b['v'][0], ldc=Fp)
+        ops.call(self._resize, b['v'][0], B, s3[0], s3[1], Fp, b['path'][0], up[0][0], up[0][1])
         # refinenet3, 2, 1: output = path + RCU1(l_i); output = RCU2(output); out_conv; resize (commuted, see above)
         for step, (li, rf) in enumerate(((2, 3), (1, 2), (0, 1))):
             s = sizes[li]
             path = b['path'][step]
-            ops.conv3x3(b['lr'][li], B, s[0], s[1], Fp, w[f'rf{rf}_u1c1_w'], Fp, act=_lib.ACT_RELU, bias=w[f'rf{rf}_u1c1_b'], C=b[f't{li}'],
+            self._conv(b['lr'][li], B, s[0], s[1], Fp, w[f'rf{rf}_u1c1_w'], Fp, act=_lib.ACT_RELU, bias=w[f'rf{rf}_u1c1_b'], C=b[f't{li}'],
                         halo=b['halo'])
-            ops.conv3x3(b[f't{li}'], B, s[0], s[1], Fp, w[f'rf{rf}_u1c2_w'], Fp, bias=w[f'rf{rf}_u1c2_b'], C=b[f'o{li}'], C2=b[f'or{li}'],
+            self._conv(b[f't{li}'], B, s[0], s[1], Fp, w[f'rf{rf}_u1c2_w'], Fp, bias=w[f'rf{rf}_u1c2_b'], C=b[f'o{li}'], C2=b[f'or{li}'],
                         R=b['l'][li], R2=path, halo=b['halo'])
-            ops.conv3x3(b[f'or{li}'], B, s[0], s[1], Fp, w[f'rf{rf}_u2c1_w'], Fp, act=_lib.ACT_RELU, bias=w[f'rf{rf}_u2c1_b'], C=b[f't{li}'],
+            self._conv(b[f'or{li}'], B, s[0], s[1], Fp, w[f'rf{rf}_u2c1_w'], Fp, act=_lib.ACT_RELU, bias=w[f'rf{rf}_u2c1_b'], C=b[f't{li}'],
                         halo=b['halo'])
-            ops.conv3x3(b[f't{li}'], B, s[0], s[1], Fp, w[f'rf{rf}_u2c2_w'], Fp, bias=w[f'rf{rf}_u2c2_b'], C=b[f'u{li}'], R=b[f'o{li}'], halo=b['halo'])
+            self._conv(b[f't{li}'], B, s[0], s[1], Fp, w[f'rf{rf}_u2c2_w'], Fp, bias=w[f'rf{rf}_u2c2_b'], C=b[f'u{li}'], R=b[f'o{li}'], halo=b['halo'])
             t = up[step + 1]
-            ops.gemm(b[f'u{li}'], Fp, w[f'rf{rf}_out_w'], Fp, B * s[0] * s[1], Fp, Fp, bias=w[f'rf{rf}_out_b'], C=b['v'][step + 1], ldc=Fp)
-            ops.call("dm_resize_bilinear_nhwc_f16", b['v'][step + 1], B, s[0], s[1], Fp, b['path'][step + 1], t[0], t[1])
+            self._gemm(b[f'u{li}'], Fp, w[f'rf{rf}_out_w'], Fp, B * s[0] * s[1], Fp, Fp, bias=w[f'rf{rf}_out_b'], C=b['v'][step + 1], ldc=Fp)
+            ops.call(self._resize, b['v'][step + 1], B, s[0], s[1], Fp, b['path'][step + 1], t[0], t[1])
 
     def run_head(self, b, B, H, W, nh, nw, out_hw=None, resize=True):
         """output_conv (dpt.py:139-150 / dpt_depth.py:150-158) + the final resize to the image size.  resize=False returns the
@@ -332,10 +404,10 @@ class DepthAnythingV2Engine:
         ops, w = self.ops, self.w
         Fp = self.Fp
         t = b['up_sizes'][3]
-        ops.conv3x3(b['path'][3], B, t[0], t[1], Fp, w['oc1_w'], self.F2p, bias=w['oc1_b'], C=b['oc1'], halo=b['halo'])
-        ops.call("dm_resize_bilinear_nhwc_f16", b['oc1'], B, t[0], t[1], self.F2p, b['oc1u'], nh, nw)
+        self._conv(b['path'][3], B, t[0], t[1], Fp, w['oc1_w'], self.F2p, bias=w['oc1_b'], C=b['oc1'], halo=b['halo'])
+        ops.call(self._resize, b['oc1'], B, t[0], t[1], self.F2p, b['oc1u'], nh, nw)
         # conv3x3 -> ReLU -> conv1x1 -> ReLU (+ the outer F.relu, idempotent) fused into one epilogue
-        ops.conv3x3(b['oc1u'], B, nh, nw, self.F2p, w['oc2_w'], 32, epi=_lib.EPI_HEAD, act=_lib.ACT_RELU, bias=w['oc2_b'], X=b['d'],
+        self._conv(b['oc1u'], B, nh, nw, self.F2p, w['oc2_w'], 32, epi=_lib.EPI_HEAD, act=_lib.ACT_RELU, bias=w['oc2_b'], X=b['d'],
                     gamma=w['oc3_w'], head_b2=self.oc3_b, halo=b['halo'])
         if not resize:
             return b['d']
@@ -421,6 +493,7 @@ class DptBeitEngine(DepthAnythingV2Engine):
     PATCH = 16
     MEAN = (0.5, 0.5, 0.5)
     STD = (0.5, 0.5, 0.5)
+    SUPPORTS_SPLIT = False
     CHAN_MAP = (2, 1, 0)        # estimatemidas receives the BGR-swapped image of get_raw_prediction (:381) unchanged
     FINAL_RESIZE_MODE = 1       # bicubic, align_corners=False (:487-497)
     CONFIGS = BEIT_CONFIGS
@@ -1486,6 +1559,24 @@ CHECKPOINTS = {
     14: ("./models/depth_anything_v2/depth_anything_v2_vitl.pth", _flat, _op_or_native(DepthAnythingV2Engine, 'vitl')),
 }
 PIX2PIX_CHECKPOINT = "./models/pix2pix/latest_net_G.pth"
+DAV2_ENCODERS = {12: 'vits', 13: 'vitb', 14: 'vitl'}
+
+
+def no_half_route(model_type, boost, precision):
+    """What the `no_half` setting does to a model load: "split" (Depth-Anything-V2: the reference then runs the whole network in
+    fp32, src/depthmap_generation.py:548-559, so it gets the fp32-class split path), "unchanged" (the reference's arithmetic does
+    not change either: 0 and 7 always run in fp32 here and there, BOOST never halves its base network, and MiDaS 1, 2, 3, 5 under
+    precision "autocast" keep fp16 convolutions and matmuls through torch.autocast, :455-499), or NotImplementedError where the
+    reference would run an fp32 network this build has no fp32-class path for."""
+    if model_type in DAV2_ENCODERS:
+        return "split"
+    if model_type in (8, 9):
+        raise NotImplementedError(f"no_half is not implemented in depthmap_b200 for model type {model_type} (ZoeDepth on the BEiT core); "
+                                  f"it is implemented for Depth-Anything-V2 (12, 13, 14) and leaves 0, 7, BOOST and autocast MiDaS as they are")
+    if model_type in (1, 2, 3, 5) and not boost and precision == "full":
+        raise NotImplementedError(f"no_half with precision \"full\" is not implemented in depthmap_b200 for model type {model_type} (an fp32 "
+                                  f"MiDaS network); with precision \"autocast\" the reference keeps fp16 arithmetic and so does this build")
+    return "unchanged"
 
 
 class ModelHolder:
@@ -1528,19 +1619,19 @@ class ModelHolder:
         if boost and model_type not in BASE_NETWORKS:
             raise NotImplementedError(f"BOOST is implemented in depthmap_b200 for the base networks LeReS res101 (model type 0), "
                                       f"DPT-BEiT-L 512 / 384 (1, 2), DPT-Large 384 (3) and MiDaS v2.1 (5), not for model type {model_type}")
-        if getattr(self, "no_half", False):
-            # reference: `no_half` keeps the network in fp32 (src/depthmap_generation.py:268-275).  The H100 path feeds the tensor
-            # cores fp16 operands (fp32 accumulation, fp32 residual stream) and has no fp32-operand variant: say so instead of
-            # silently ignoring the setting
-            raise NotImplementedError("no_half (fp32 network) is not implemented in depthmap_b200: the tensor-core path uses fp16 operands "
-                                      "with fp32 accumulation; unset the setting")
+        # `no_half` is read here, at load time; like the reference, ensure_models does not reload when only the setting changes
+        route = no_half_route(model_type, boost, self.precision) if self.no_half else "unchanged"
         if model_type not in CHECKPOINTS:
             raise NotImplementedError(f"model_type {model_type} is not implemented in depthmap_b200 yet "
                                       f"(implemented: 0 = LeReS res101; 1, 2 = DPT-BEiT-L 512/384; 3 = DPT-Large 384; 5 = MiDaS v2.1; 7 = ZoeDepth-N; "
                                       f"8 = ZoeDepth-K; 9 = ZoeDepth-NK; 12, 13, 14 = Depth-Anything-V2 S/B/L)")
         dev = torch.device(device)
         path, unwrap, make = CHECKPOINTS[model_type]
-        model = make(self._load_checkpoint(model_type, path, unwrap), model_type, dev, boost, bool(tiling_mode))
+        if route == "split":     # always the op-level engine: the model-level handle has no split path
+            model = DepthAnythingV2Engine(self._load_checkpoint(model_type, path, unwrap), DAV2_ENCODERS[model_type], dev,
+                                          bool(tiling_mode), split=True)
+        else:
+            model = make(self._load_checkpoint(model_type, path, unwrap), model_type, dev, boost, bool(tiling_mode))
         if boost:      # reference :284-299: the pix2pix merge network ('latest_net_G.pth', netG = unet_1024, norm none)
             from .boost import BoostPipeline, UnetMergeEngine
             self.pix2pix_model = BoostPipeline(model, UnetMergeEngine(self._load_checkpoint("pix2pix", PIX2PIX_CHECKPOINT), dev), dev, model_type)
