@@ -152,13 +152,15 @@ int dm_circular_halo_f16(const void *act, int B, int H, int W, int C, void *halo
 int dm_conv3x3_circular_ex(const void *act, void *halo, int B, int H, int W, int Cin, const void *Wt, const dm_gemm_desc *desc_host,
                            void *stream);
 /* Split mode (fp32-class GEMM for no_half).  A split tensor stores an fp32 value v as fp16 hi = rn(v), lo = rn(v - hi), each
- * row of logical width n as [hi | lo | hi] (3n halves; NHWC tensors per pixel).  Split weights [N, K] are the pre-scaled fp32
- * weights w * 2^e[n] packed [w_hi | w_hi | w_lo] (a conv filter per tap), wscale[n] = 2^-e[n] (fp32, 8-byte aligned).
+ * row of logical width n as [hi | lo | hi] (3n halves; NHWC tensors per pixel).  hi is an fp16 number, so the format holds
+ * |v| < 65504 only (larger values overflow hi to inf); below 2^-14 hi is subnormal and the format keeps v to 2^-25 absolute.
+ * Split weights [N, K] are the pre-scaled fp32 weights w * 2^e[n] packed [w_hi | w_hi | w_lo] (a conv filter per tap),
+ * wscale[n] = 2^-e[n] (fp32, 8-byte aligned).
  * dm_gemm_split_ex: A split [M, K/3 logical] with desc->K = the tripled depth (K % 64 == 0); the epilogue multiplies the
  * accumulator by wscale, then applies the desc's epilogue.  STORE_F16 / PIXSHUF write split outputs (C rows of pitch
  * ldc >= 3N: hi at column n, lo at N + n, hi at 2N + n; pixel shuffle: 3*ps_cout halves per output pixel), C2 the split relu
  * copy, R / R2 are split residuals (pitches >= 3N); RESID_F32, STORE_F32 and HEAD write fp32 as in dm_gemm_ex.  The tensor
- * core's truncating accumulator is added into an fp32 register sum every 4 k-blocks (gemm_wgmma.cu). */
+ * core's truncating accumulator is added into an fp32 register sum after every k-block (SPLIT_PROMOTE = 1, gemm_wgmma.cu). */
 int dm_gemm_split_ex(const void *A, int lda, const void *W, int ldw, const float *wscale, const dm_gemm_desc *desc_host, void *stream);
 /* Split 3x3 pad-1 conv: act split NHWC [B, H, W, 3*Cin] (Cin logical, % 64 == 0), Wt split [Cout, 9*3*Cin] per tap; desc->ldc /
  * ldr / ldr2 are the output / residual pixel pitches (>= 3 Cout).  halo: NULL = zero padding (one kernel), else circular

@@ -1,5 +1,7 @@
-"""CPU: every entry point include/depthmap_b200.h declares is exercised by name in some test file, or is listed below with the
-test that covers it through a wrapper.  A new entry point without a test fails here."""
+"""CPU: every entry point include/depthmap_b200.h declares is exercised by name in a test file that runs kernels (a GPU test
+file, or test_cabi.py, which calls the loaded library's host entry points), or is listed below with the test that covers it
+through a wrapper.  A name that only a CPU test mentions (a string in a fake library's trace, say) does not count: nothing ran
+it.  A new entry point without a test fails here."""
 import os
 import re
 
@@ -37,6 +39,11 @@ INDIRECT = {
     "dm_unet_interleave": "the merge U-Net (test_boost_gpu.py::test_merge_unet_vs_oracle)",
     "dm_unet_final": "the merge U-Net (test_boost_gpu.py::test_merge_unet_vs_oracle)",
     "dm_unet_last": "the merge U-Net (test_boost_gpu.py::test_merge_unet_vs_oracle)",
+    "dm_conv3x3_ex": "Ops.conv3x3 without a halo, the zero-padded conv of every fp16 engine (test_tiling_gpu.py::test_circular_conv3x3_vs_torch)",
+    "dm_leres_stem_im2col": "the LeReS engine's stem on uint8 images (test_leres_gpu.py::test_leres_vs_oracle)",
+    "dm_leres_stem_im2col_f32": "the LeReS stem on one float crop (test_boost_gpu.py::test_leres_on_float_crop_vs_oracle)",
+    "dm_leres_stem_im2col_f32_batch": "the LeReS stem on BOOST's batched crops (test_boost_gpu.py::test_estimateboost_vs_oracle)",
+    "dm_vit_pos_embed": "DptVitEngine's position embedding (test_model_cabi_gpu.py::test_native_vit_equals_op_level_path)",
 }
 
 
@@ -47,13 +54,16 @@ def declared_entry_points():
 
 
 def _test_sources():
+    """the test files that run kernels: GPU test files (marked gpu), and test_cabi.py"""
     me = os.path.abspath(__file__)
     out = {}
     for name in sorted(os.listdir(TESTS)):
         path = os.path.join(TESTS, name)
         if name.endswith(".py") and os.path.abspath(path) != me:
             with open(path) as f:
-                out[name] = f.read()
+                src = f.read()
+            if re.search(r"\bpytest\.mark\.gpu\b", src) or name == "test_cabi.py":
+                out[name] = src
     return out
 
 
@@ -77,3 +87,13 @@ def test_indirect_table_is_current():
     sources = _test_sources()
     direct = sorted(n for n in INDIRECT if any(re.search(r"\b" + n + r"\b", s) for s in sources.values()))
     assert not direct, f"INDIRECT entries that now have a direct test: {direct}"
+
+
+def test_split_entry_points_are_called_directly():
+    """the no_half (split) kernels are each called by name in a GPU test, not only reached through the network"""
+    split = [n for n in declared_entry_points() if "split" in n or n == "dm_assemble_tokens_f32"]
+    assert len(split) == 7, split
+    sources = _test_sources()
+    indirect = sorted(set(split) & set(INDIRECT))
+    missing = [n for n in split if not any(re.search(r"\b" + n + r"\b", s) for s in sources.values())]
+    assert not indirect and not missing, (indirect, missing)
