@@ -1,9 +1,8 @@
 """Depth-network workloads for bench.py (kept separate so bench.py stays importable before the tensor-core path exists).
 
-Timed region: the model-level C-ABI handle (NativeDepthModel -> dm_depth_forward) + the HBM-side kernels.  A second, op-level
-instance of the same network (the Python engine that issues the same kernels one C call at a time) exists only for the PROBE
-pass after the timed region: CUDA events around every attention launch and around the block-0 fc1 GEMM, which gives the
-dominant kernel's share of the step and its roofline live, in this run."""
+Timed region: the network's engine (depthmap_generation.py, one C call per kernel, the network replayed from its CUDA graph)
++ the HBM-side kernels.  The same engine serves the PROBE pass after the timed region: CUDA events around every attention launch
+and around the block-0 fc1 GEMM, which gives the dominant kernel's share of the step and its roofline live, in this run."""
 from __future__ import annotations
 
 import os
@@ -16,20 +15,20 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 
 
 class _NetWorkload:
-    """Shared parts of the network workloads: native model for the timed region, op-level engine for the kernel probe."""
+    """Shared parts of the network workloads: one engine for the timed region and the kernel probe."""
     heads = 16
     C = 1024
 
     def probe(self, n=20):
-        """Dominant-kernel timing, live in this run: the op-level engine runs one forward (so its buffers hold this workload's
-        real activations), then the fused attention kernel of the LAST block and the fc1 GEMM are launched n times back to back
-        on those buffers with CUDA events around the loop (GPU-bound: no host gaps inside the interval); the forward itself is
-        timed on the native model (the thing the timed region runs)."""
+        """Dominant-kernel timing, live in this run: the engine runs a forward (so its buffers hold this workload's real
+        activations), then the fused attention kernel of the LAST block and the fc1 GEMM are launched n times back to back on
+        those buffers with CUDA events around the loop (GPU-bound: no host gaps inside the interval); the forward itself is timed
+        as the timed region runs it."""
         import torch
         from depthmap_b200 import _lib
         eng = self.engine
         for _ in range(2):
-            self._engine_forward()
+            self._model_forward()
         torch.cuda.synchronize()
         b = eng._bufs
         cfg = eng.cfg
@@ -68,12 +67,12 @@ class _NetWorkload:
                 "frac": a / peaks["bf16_tflops"], "traffic": None,
                 "peak_source": peaks["source"], "algorithmic_flops_per_launch": attn_flops,
                 "kernel_ms": pr["attn_ms_per_launch"], "launches_per_step": pr["attn_launches"],
-                "share_of_step": share, "share_note": "attention launches per forward x kernel time / forward time of the model handle, all CUDA events, this run",
+                "share_of_step": share, "share_note": "attention launches per forward x kernel time / forward time of the engine, all CUDA events, this run",
                 "secondary": {"kernel": self.FC1_KERNEL, "achieved": f, "frac": f / peaks["bf16_tflops"], "kernel_ms": pr["fc1_ms"],
                               "algorithmic_flops_per_launch": self.fc1_flops}}
 
     def _model_forward(self):
-        return self.model.forward_batch(self.rgb, self.W, self.H)
+        return self.engine.forward_batch(self.rgb, self.W, self.H)
 
     def extra(self, ms_step, peaks):
         fwd = self.FLOP_PER_IMAGE * self.B / (ms_step * 1e-3) / 1e12
@@ -130,12 +129,9 @@ class Dav2Stereo(_NetWorkload):
     def __init__(self, dev, rank):
         import torch
         from bench import make_images
-        from depthmap_b200.depthmap_generation import DepthAnythingV2Engine, NativeDepthModel
+        from depthmap_b200.depthmap_generation import DepthAnythingV2Engine
         self.dev = dev
-        sd = self._state_dict()
-        self.model = NativeDepthModel(sd, self.MODEL_TYPE, dev)
-        self.engine = DepthAnythingV2Engine(sd, self.encoder, dev)      # probe pass only
-        del sd
+        self.engine = DepthAnythingV2Engine(self._state_dict(), self.encoder, dev)
         rgb, _ = make_images(self.B, self.H, self.W, rank)
         self.rgb_h = torch.from_numpy(rgb).pin_memory()
         self.rgb = self.rgb_h.to(dev)
@@ -156,18 +152,13 @@ class Dav2Stereo(_NetWorkload):
         from depthmap_b200.core import normalize_prediction_batch
         from depthmap_b200.normalmap_generation import create_normalmap_batch
         from depthmap_b200.stereoimage_generation import create_stereoimages_batch
-        n0 = self.model.launches
-        pred = self.model.forward_batch(rgb, self.W, self.H)
+        n0 = self.engine.ops.launches
+        pred = self.engine.forward_batch(rgb, self.W, self.H)
         depth = normalize_prediction_batch(pred, False)
         sbs = create_stereoimages_batch(rgb, depth, 2.5, 0.0, ['left-right'], 0.0, 1.0, self.fill)[0]
         normal = create_normalmap_batch(depth)
-        n1 = self.model.launches
-        if n1 > n0:
-            self.launches_per_step = (n1 - n0) + 3 + 3 + 1
+        self.launches_per_step = (self.engine.ops.launches - n0) + 3 + 3 + 1
         return depth, sbs, normal
-
-    def _engine_forward(self):
-        return self.engine.forward_batch(self.rgb, self.W)
 
     def step_resident(self, time_kernel=False):
         return self.step(self.rgb, time_kernel)
@@ -222,12 +213,9 @@ class DepthBeit512(_NetWorkload):
     def __init__(self, dev, rank):
         import torch
         from bench import make_images
-        from depthmap_b200.depthmap_generation import DptBeitEngine, NativeDepthModel
+        from depthmap_b200.depthmap_generation import DptBeitEngine
         self.dev = dev
-        sd = self._state_dict()
-        self.model = NativeDepthModel(sd, self.MODEL_TYPE, dev)
-        self.engine = DptBeitEngine(sd, self.model_name, dev)           # probe pass only
-        del sd
+        self.engine = DptBeitEngine(self._state_dict(), self.model_name, dev)
         rgb, _ = make_images(self.B, self.H, self.W, rank)
         self.rgb_h = torch.from_numpy(rgb).pin_memory()
         self.rgb = self.rgb_h.to(dev)
@@ -244,16 +232,11 @@ class DepthBeit512(_NetWorkload):
     def step(self, rgb, time_kernel=False):
         import torch
         from depthmap_b200.core import normalize_prediction_batch
-        n0 = self.model.launches
-        pred = self.model.forward_batch(rgb, self.W, self.H)
+        n0 = self.engine.ops.launches
+        pred = self.engine.forward_batch(rgb, self.W, self.H)
         depth = normalize_prediction_batch(pred, False)
-        n1 = self.model.launches
-        if n1 > n0:
-            self.launches_per_step = (n1 - n0) + 3
+        self.launches_per_step = (self.engine.ops.launches - n0) + 3
         return (depth,)
-
-    def _engine_forward(self):
-        return self.engine.forward_batch(self.rgb, self.W, self.H)
 
     def step_resident(self, time_kernel=False):
         return self.step(self.rgb, time_kernel)
@@ -314,7 +297,6 @@ class ZoeAnaglyph(_NetWorkload):
         from depthmap_b200.depthmap_generation import ZoeDepthNKEngine
         self.dev = dev
         self.engine = ZoeDepthNKEngine(self._state_dict(), dev)
-        self.model = self.engine
         rgb, _ = make_images(self.B, self.H, self.W, rank)
         self.rgb_h = torch.from_numpy(rgb).pin_memory()
         self.rgb = self.rgb_h.to(dev)
@@ -349,9 +331,6 @@ class ZoeAnaglyph(_NetWorkload):
 
     def e2e_bytes(self):
         return self.rgb_h.numel(), self.B * self.H * self.W * (2 + 3)
-
-    def _engine_forward(self):
-        return self.engine.forward_batch(self.rgb, self.NET_W, self.NET_H)
 
     def _model_forward(self):
         return self.engine.forward_batch(self.rgb, self.NET_W, self.NET_H)

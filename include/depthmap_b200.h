@@ -300,43 +300,15 @@ int dm_video_select_bounds(const void *workspace, double gamma_lo, double gamma_
 int dm_video_scale_f64(const float *x, long long n, const double *ab, double *out, void *stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
- * §8(b) — model-level entry points (csrc/model.cu): a handle that owns the packed checkpoint, the activation buffers, the
- * resolution-dependent tables and one captured CUDA graph per shape; a forward is ONE call.
- *   replaces  the network part of ModelHolder.load_models / get_raw_prediction (src/depthmap_generation.py:76-301,375-403)
- *             for model types 1, 2 (MiDaS 3.1 DPT-BEiT-L 512 / 384), 3 (MiDaS 3.0 DPT-Large 384) and 12, 13, 14 (Depth-Anything-V2 S / B / L).
- * dm_weight: one tensor of the upstream checkpoint (state_dict key, HOST pointer, dtype 0 = fp32 / 1 = fp16 / 2 = bf16, shape);
- * the blob is only read during dm_model_create.  dtype of the model: 0 = fp16 operands, fp32 accumulation (the only one).
- * dm_depth_forward: rgb uint8 [B,H,W,3] (device) -> depth_out fp32 [B,out_h,out_w] (device), asynchronous on `stream`; the net
- * size follows the reference's Resize rule for the family from (net_w, net_h) (dm_model_net_size).  The first call of a
- * shape allocates and runs eagerly, the second captures a CUDA graph, later calls replay it (DEPTHMAP_B200_MODEL_GRAPH=0
- * disables); inside an outer stream capture the launches are simply recorded into that capture.
- * Thread-compatible: one handle per thread; handles are independent.
+ * Resolution-dependent tables of the ViT trunks (csrc/pos_tables.cu), computed once per resolution by the engines:
+ * HOST pointers, float32 arithmetic in torch's operation order.
  * ------------------------------------------------------------------------------------------------------------- */
-typedef struct dm_weight {
-    const char *name;
-    const void *data_host;
-    int32_t dtype;
-    int32_t ndim;
-    int64_t shape[4];
-} dm_weight;
-typedef struct dm_weight_blob {
-    const dm_weight *items;
-    int32_t count;
-} dm_weight_blob;
-typedef struct dm_model dm_model_t;
-/* Resolution-dependent tables exactly as the model computes them (HOST pointers, float32 arithmetic in torch's order):
- * DINOv2 interpolate_pos_encoding (dinov2.py:179-210): pos_embed [1 + n*n, C] -> out [1 + gh*gw, C];
+/* DINOv2 interpolate_pos_encoding (dinov2.py:179-210): pos_embed [1 + n*n, C] -> out [1 + gh*gw, C];
  * BEiT _get_rel_pos_bias table half (dmidas/backbones/beit.py:29-50): table [(2w-1)^2 + 3, heads] -> out [heads, (2gh-1)(2gw-1)+3] * log2(e). */
 int dm_dinov2_pos_embed(const float *pos_embed_host, int n, int C, int gh, int gw, float *out_host);
 int dm_beit_rel_table(const float *table_host, int window, int heads, int gh, int gw, float *out_host);
 /* MiDaS 3.0 _resize_pos_embed (dmidas/backbones/vit.py:16-31): pos_embed [1 + n*n, C] -> out [1 + gh*gw, C], bilinear */
 int dm_vit_pos_embed(const float *pos_embed_host, int n, int C, int gh, int gw, float *out_host);
-int dm_model_create(dm_model_t **out, int model_type, const dm_weight_blob *weights, int device, int dtype);
-int dm_model_destroy(dm_model_t *model);
-int dm_model_net_size(const dm_model_t *model, int W, int H, int net_w, int net_h, int *nw_out, int *nh_out);
-long long dm_model_launches(const dm_model_t *model);
-int dm_depth_forward(dm_model_t *model, const uint8_t *rgb, int B, int H, int W, int net_w, int net_h, float *depth_out, int out_h, int out_w,
-                     void *stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * D8 — LeReS (ResNeXt-101 32x8d + FTB / FFM / AO decoder), csrc/leres_kernels.cu: the non-GEMM pieces.   replaces parts of

@@ -32,16 +32,6 @@ class StereoParams(ctypes.Structure):
     ]
 
 
-class Weight(ctypes.Structure):
-    """mirror of dm_weight"""
-    _fields_ = [("name", ctypes.c_char_p), ("data_host", ctypes.c_void_p), ("dtype", ctypes.c_int32), ("ndim", ctypes.c_int32),
-                ("shape", ctypes.c_int64 * 4)]
-
-
-class WeightBlob(ctypes.Structure):
-    _fields_ = [("items", ctypes.POINTER(Weight)), ("count", ctypes.c_int32)]
-
-
 class GemmDesc(ctypes.Structure):
     """mirror of dm_gemm_desc (include/depthmap_b200.h)"""
     _fields_ = [
@@ -79,7 +69,7 @@ EXPORTS = [
     "dm_zoe_seed_bins", "dm_zoe_attractor_single", "dm_zoe_clb_single",
     "dm_video_workspace_bytes", "dm_video_blend", "dm_video_minmax", "dm_video_scale_f32", "dm_video_select_init", "dm_video_select_hist",
     "dm_video_select_pick", "dm_video_select_bounds", "dm_video_scale_f64",
-    "dm_model_create", "dm_model_destroy", "dm_model_net_size", "dm_model_launches", "dm_depth_forward", "dm_dinov2_pos_embed", "dm_beit_rel_table", "dm_vit_pos_embed",
+    "dm_dinov2_pos_embed", "dm_beit_rel_table", "dm_vit_pos_embed",
     "dm_leres_stem_im2col", "dm_maxpool3x3s2_nhwc_f16", "dm_subsample2_nhwc_f16", "dm_add_f16", "dm_resize_f32_ld",
     "dm_boost_partials", "dm_unet_first_cols", "dm_unet_down_cols", "dm_unet_up_cols", "dm_unet_interleave", "dm_unet_final", "dm_unet_first", "dm_unet_last", "dm_sum_chunks_f32", "dm_boost_minmax",
     "dm_boost_merge_input", "dm_boost_post", "dm_boost_fit_sums", "dm_boost_blend", "dm_boost_resize_cubic", "dm_boost_u8_to_planar",
@@ -134,16 +124,9 @@ def load() -> ctypes.CDLL:
             L.dm_video_select_pick.argtypes = [vp, i32, vp]
             L.dm_video_select_bounds.argtypes = [vp, dbl, dbl, vp, vp]
             L.dm_video_scale_f64.argtypes = [vp, ll, vp, vp, vp]
-        if hasattr(L, "dm_model_create"):
-            L.dm_model_create.argtypes = [c.POINTER(vp), i32, c.POINTER(WeightBlob), i32, i32]
-            L.dm_model_destroy.argtypes = [vp]
-            L.dm_model_net_size.argtypes = [vp, i32, i32, i32, i32, c.POINTER(i32), c.POINTER(i32)]
-            L.dm_model_launches.argtypes = [vp]
-            L.dm_model_launches.restype = c.c_longlong
-            L.dm_depth_forward.argtypes = [vp, vp, i32, i32, i32, i32, i32, vp, i32, i32, vp]
-            L.dm_dinov2_pos_embed.argtypes = [vp, i32, i32, i32, i32, vp]
-            L.dm_beit_rel_table.argtypes = [vp, i32, i32, i32, i32, vp]
-            L.dm_vit_pos_embed.argtypes = [vp, i32, i32, i32, i32, vp]
+        L.dm_dinov2_pos_embed.argtypes = [vp, i32, i32, i32, i32, vp]
+        L.dm_beit_rel_table.argtypes = [vp, i32, i32, i32, i32, vp]
+        L.dm_vit_pos_embed.argtypes = [vp, i32, i32, i32, i32, vp]
         _bind_optional(L)
         _lib = L
         return L

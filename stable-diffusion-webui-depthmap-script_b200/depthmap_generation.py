@@ -134,6 +134,8 @@ class DepthAnythingV2Engine:
         self._buf_key = None
         self._bufs = {}
         self._pos_cache = {}
+        # from the second call on at a given (B, net size) the launches of run_network + run_head replay from a CUDA graph
+        self._graphs = _lib.GraphCache(self.ops, "DEPTHMAP_B200_MODEL_GRAPH", type(self).__name__)
         self._pack(state_dict)
 
     # ---- weight packing --------------------------------------------------------------------------------------------
@@ -218,7 +220,7 @@ class DepthAnythingV2Engine:
             C = pe.shape[-1]
             N = pe.shape[1] - 1
             n = int(round(math.sqrt(N)))
-            # host arithmetic shared with the model-level C-ABI (csrc/model.cu), so both paths use bit-identical tables
+            # host arithmetic in float32 and torch's operation order (csrc/pos_tables.cu)
             src = np.ascontiguousarray(pe.reshape(N + 1, C).cpu().numpy(), dtype=np.float32)
             dst = np.empty((gh * gw + 1, C), dtype=np.float32)
             _lib.check(getattr(self.ops.L, self.POS_EMBED)(src.ctypes.data, n, C, gh, gw, dst.ctypes.data), self.POS_EMBED)
@@ -231,6 +233,10 @@ class DepthAnythingV2Engine:
         key = (B, nh, nw)
         if self._buf_key == key:
             return self._bufs
+        # the graphs read and write the buffers about to be freed.  Their key is the buffers' key, so at most one shape has
+        # graphs at a time; the resolution tables they read (_pos, rel_tables) are only evicted when a new resolution arrives,
+        # which always lands here first.
+        self._graphs.clear()
         self._bufs = {}
         self._buf_key = None
         dev = self.device
@@ -317,6 +323,7 @@ class DepthAnythingV2Engine:
     # ---- forward ---------------------------------------------------------------------------------------------------
     def forward_batch(self, rgb, net_w, net_h=None, out_hw=None):
         """rgb: uint8 CUDA [B,H,W,3] -> float32 CUDA [B,H,W] raw prediction (what the reference's estimate* returns)."""
+        import torch
         B, H, W, _ = rgb.shape
         nw, nh = self.net_size(W, H, net_w, net_h if net_h is not None else net_w)
         P_ = self.PATCH
@@ -325,8 +332,16 @@ class DepthAnythingV2Engine:
         self.ops.call("dm_preprocess_patchify_split" if self.split else "dm_preprocess_patchify", rgb, B, H, W, nh, nw, P_,
                       (ctypes.c_float * 3)(*self.MEAN), (ctypes.c_float * 3)(*self.STD), (ctypes.c_int * 3)(*self.CHAN_MAP), b['patches'],
                       self.kpad, launches=1 + (self.kpad > 3 * P_ * P_))
+        d = self._graphs.run((B, nh, nw), lambda: self._network(b, B, nh, nw))
+        oh, ow = out_hw if out_hw is not None else (H, W)
+        out = torch.empty(B, oh, ow, dtype=torch.float32, device=self.device)
+        self.ops.call("dm_resize_f32", d, B, nh, nw, out, oh, ow, self.FINAL_RESIZE_MODE)
+        return out
+
+    def _network(self, b, B, nh, nw):
+        """patch matrix in b['patches'] -> the net-size prediction b['d']"""
         self.run_network(b, B, nh, nw)
-        return self.run_head(b, B, H, W, nh, nw, out_hw)
+        return self.run_head(b, B, nh, nw)
 
     def run_network(self, b, B, nh, nw):
         """patch embedding -> transformer blocks -> reassemble -> fusion blocks; leaves refinenet1's output in b['path'][3]
@@ -397,10 +412,9 @@ class DepthAnythingV2Engine:
             self._gemm(b[f'u{li}'], Fp, w[f'rf{rf}_out_w'], Fp, B * s[0] * s[1], Fp, Fp, bias=w[f'rf{rf}_out_b'], C=b['v'][step + 1], ldc=Fp)
             ops.call(self._resize, b['v'][step + 1], B, s[0], s[1], Fp, b['path'][step + 1], t[0], t[1])
 
-    def run_head(self, b, B, H, W, nh, nw, out_hw=None, resize=True):
-        """output_conv (dpt.py:139-150 / dpt_depth.py:150-158) + the final resize to the image size.  resize=False returns the
-        net-size prediction [B, nh, nw] itself (a pooled buffer, valid until the next forward at this shape)."""
-        import torch
+    def run_head(self, b, B, nh, nw):
+        """output_conv (dpt.py:139-150 / dpt_depth.py:150-158) -> the net-size prediction [B, nh, nw] (a pooled buffer, valid until
+        the next forward at this shape)."""
         ops, w = self.ops, self.w
         Fp = self.Fp
         t = b['up_sizes'][3]
@@ -409,12 +423,7 @@ class DepthAnythingV2Engine:
         # conv3x3 -> ReLU -> conv1x1 -> ReLU (+ the outer F.relu, idempotent) fused into one epilogue
         self._conv(b['oc1u'], B, nh, nw, self.F2p, w['oc2_w'], 32, epi=_lib.EPI_HEAD, act=_lib.ACT_RELU, bias=w['oc2_b'], X=b['d'],
                     gamma=w['oc3_w'], head_b2=self.oc3_b, halo=b['halo'])
-        if not resize:
-            return b['d']
-        oh, ow = out_hw if out_hw is not None else (H, W)
-        out = torch.empty(B, oh, ow, dtype=torch.float32, device=self.device)
-        ops.call("dm_resize_f32", b['d'], B, nh, nw, out, oh, ow, self.FINAL_RESIZE_MODE)
-        return out
+        return b['d']
 
     def to(self, device):
         return self
@@ -567,7 +576,7 @@ class DptBeitEngine(DepthAnythingV2Engine):
             nrd_new = new_h * new_w + 3
             heads = self.cfg['heads']
             for t in self._tables:
-                # host arithmetic shared with the model-level C-ABI (csrc/model.cu: beit_rel_table_host)
+                # host arithmetic in float32 and torch's operation order (csrc/pos_tables.cu)
                 src = np.ascontiguousarray(t.cpu().numpy(), dtype=np.float32)
                 dst = np.empty((heads, nrd_new), dtype=np.float32)
                 _lib.check(self.ops.L.dm_beit_rel_table(src.ctypes.data, win, heads, gh, gw, dst.ctypes.data), "dm_beit_rel_table")
@@ -607,8 +616,7 @@ class DptBeitEngine(DepthAnythingV2Engine):
             b = self._buffers(B, nh, nw)
             self.ops.call("dm_preprocess_patchify_f32_crops", planar, hi, wi, r, B, nh, nw, self.PATCH, m, sd, cm, b['patches'], self.kpad,
                           launches=1 + (self.kpad > 3 * self.PATCH ** 2))
-            self.run_network(b, B, nh, nw)
-            d = self.run_head(b, B, nh, nw, nh, nw, resize=False)
+            d = self._network(b, B, nh, nw)
             for i, k in enumerate(ks):
                 w, h = int(rects[k][2]), int(rects[k][3])
                 o = torch.empty(h, w, dtype=torch.float32, device=self.device)
@@ -1105,87 +1113,6 @@ class MidasV21Engine(_ResNeXtEngine):
         return d
 
 
-class NativeDepthModel:
-    """Thin caller of the model-level C-ABI (include/depthmap_b200.h: dm_model_create / dm_depth_forward / dm_model_destroy,
-    csrc/model.cu): the handle owns the packed weights, the activation buffers, the resolution tables and a captured CUDA
-    graph per shape; a forward is one C call.  Model types 1, 2 (DPT-BEiT-L 512 / 384) and 12, 13, 14 (Depth-Anything-V2)."""
-
-    _DT = {"torch.float32": 0, "torch.float16": 1, "torch.bfloat16": 2}
-
-    def __init__(self, state_dict, model_type, device):
-        import torch
-        self.L = _lib.load()
-        if not hasattr(self.L, "dm_model_create"):
-            raise RuntimeError("depthmap_b200: native library lacks dm_model_create; rebuild csrc (no fallback exists)")
-        self.device = torch.device(device)
-        self.model_type = model_type
-        keep, items = [], []
-        for name, t in state_dict.items():
-            if not torch.is_tensor(t) or not t.is_floating_point():
-                continue
-            t = t.detach().to("cpu")
-            if str(t.dtype) not in self._DT:
-                t = t.float()
-            t = t.contiguous()
-            keep.append(t)
-            w = _lib.Weight()
-            w.name = name.encode()
-            w.data_host = t.data_ptr()
-            w.dtype = self._DT[str(t.dtype)]
-            w.ndim = min(t.dim(), 4)
-            shape = list(t.shape) if t.dim() <= 4 else [int(t.numel())]
-            if t.dim() > 4:
-                w.ndim = 1
-            for k in range(4):
-                w.shape[k] = shape[k] if k < len(shape) else 1
-            items.append(w)
-        arr = (_lib.Weight * len(items))(*items)
-        blob = _lib.WeightBlob(arr, len(items))
-        h = ctypes.c_void_p()
-        idx = self.device.index if self.device.index is not None else torch.cuda.current_device()
-        _lib.check(self.L.dm_model_create(ctypes.byref(h), int(model_type), ctypes.byref(blob), int(idx), 0), "dm_model_create")
-        self.handle = h
-        del keep
-
-    def net_size(self, W, H, net_w, net_h):
-        nw, nh = ctypes.c_int(), ctypes.c_int()
-        _lib.check(self.L.dm_model_net_size(self.handle, W, H, net_w, net_h, ctypes.byref(nw), ctypes.byref(nh)), "dm_model_net_size")
-        return nw.value, nh.value
-
-    @property
-    def launches(self):
-        return int(self.L.dm_model_launches(self.handle))
-
-    def forward_batch(self, rgb, net_w, net_h=None, out_hw=None):
-        """rgb: uint8 CUDA [B,H,W,3] -> float32 CUDA [B,H,W] raw prediction."""
-        import torch
-        if self.handle is None:
-            raise RuntimeError("model was destroyed")
-        if rgb.dtype != torch.uint8 or rgb.dim() != 4 or rgb.shape[-1] != 3:
-            raise ValueError("rgb must be a uint8 tensor [B,H,W,3]")
-        rgb = rgb.contiguous()
-        B, H, W, _ = rgb.shape
-        oh, ow = out_hw if out_hw is not None else (H, W)
-        out = torch.empty(B, oh, ow, dtype=torch.float32, device=rgb.device)
-        _lib.check(self.L.dm_depth_forward(self.handle, rgb.data_ptr(), B, H, W, int(net_w), int(net_h if net_h is not None else net_w),
-                                           out.data_ptr(), oh, ow, _lib.stream_ptr()), "dm_depth_forward")
-        return out
-
-    def close(self):
-        if getattr(self, "handle", None) is not None:
-            self.L.dm_model_destroy(self.handle)
-            self.handle = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def to(self, device):
-        return self
-
-
 ZOE_CONFIG = dict(n_bins=64, emb=128, min_temp=0.0212, max_temp=50.0, router_dim=128, router_heads=4, router_layers=4)
 
 
@@ -1536,27 +1463,26 @@ _midas = _unwrap_key("model", "optimizer")      # dmidas/base_model.py:13
 _zoe = _unwrap_key("model", "model")            # dzoedepth/models/model_io.py:52-53
 
 
-def _op_or_native(cls, name):
-    """the model-level handle (zero padding only), or the op-level engine under BOOST (float crops) or tiling (circular padding)"""
-    return lambda sd, t, dev, boost, tiling: cls(sd, name, dev, tiling) if boost or tiling else NativeDepthModel(sd, t, dev)
+def _vit(cls, name):
+    return lambda sd, dev, tiling, split: cls(sd, name, dev, tiling, split)
 
 
-# model type -> (default checkpoint path, unwrap, engine(state_dict, model type, device, boost, tiling)).  The MiDaS DPT and
-# Depth-Anything-V2 models run through the model-level handle unless BOOST or tiling mode needs the op-level engine.
+# model type -> (default checkpoint path, unwrap, engine(state_dict, device, tiling, split)).  `split` (the no_half path) is only
+# ever set for Depth-Anything-V2 (no_half_route).
 CHECKPOINTS = {
-    0: ("./models/leres/res101.pth", _unwrap_leres, lambda sd, t, dev, boost, tiling: LeresEngine(sd, dev, tiling)),
-    1: ("./models/midas/dpt_beit_large_512.pt", _midas, _op_or_native(DptBeitEngine, 'beitl16_512')),
-    2: ("./models/midas/dpt_beit_large_384.pt", _midas, _op_or_native(DptBeitEngine, 'beitl16_384')),
-    3: ("./models/midas/dpt_large-midas-2f21e586.pt", _midas, _op_or_native(DptVitEngine, 'vitl16_384')),
-    5: ("./models/midas/midas_v21-f6b98070.pt", _midas, lambda sd, t, dev, boost, tiling: MidasV21Engine(sd, dev, tiling)),
+    0: ("./models/leres/res101.pth", _unwrap_leres, lambda sd, dev, tiling, split: LeresEngine(sd, dev, tiling)),
+    1: ("./models/midas/dpt_beit_large_512.pt", _midas, _vit(DptBeitEngine, 'beitl16_512')),
+    2: ("./models/midas/dpt_beit_large_384.pt", _midas, _vit(DptBeitEngine, 'beitl16_384')),
+    3: ("./models/midas/dpt_large-midas-2f21e586.pt", _midas, _vit(DptVitEngine, 'vitl16_384')),
+    5: ("./models/midas/midas_v21-f6b98070.pt", _midas, lambda sd, dev, tiling, split: MidasV21Engine(sd, dev, tiling)),
     7: ("./models/zoedepth/" + ZOE_SINGLE_VARIANTS['n']['checkpoint'], _zoe,
-        lambda sd, t, dev, boost, tiling: ZoeDepthEngine(sd, dev, 'n', circular=tiling)),
+        lambda sd, dev, tiling, split: ZoeDepthEngine(sd, dev, 'n', circular=tiling)),
     8: ("./models/zoedepth/" + ZOE_SINGLE_VARIANTS['k']['checkpoint'], _zoe,
-        lambda sd, t, dev, boost, tiling: ZoeDepthEngine(sd, dev, 'k', circular=tiling)),
-    9: ("./models/zoedepth/ZoeD_M12_NK.pt", _zoe, lambda sd, t, dev, boost, tiling: ZoeDepthNKEngine(sd, dev, circular=tiling)),
-    12: ("./models/depth_anything_v2/depth_anything_v2_vits.pth", _flat, _op_or_native(DepthAnythingV2Engine, 'vits')),
-    13: ("./models/depth_anything_v2/depth_anything_v2_vitb.pth", _flat, _op_or_native(DepthAnythingV2Engine, 'vitb')),
-    14: ("./models/depth_anything_v2/depth_anything_v2_vitl.pth", _flat, _op_or_native(DepthAnythingV2Engine, 'vitl')),
+        lambda sd, dev, tiling, split: ZoeDepthEngine(sd, dev, 'k', circular=tiling)),
+    9: ("./models/zoedepth/ZoeD_M12_NK.pt", _zoe, lambda sd, dev, tiling, split: ZoeDepthNKEngine(sd, dev, circular=tiling)),
+    12: ("./models/depth_anything_v2/depth_anything_v2_vits.pth", _flat, _vit(DepthAnythingV2Engine, 'vits')),
+    13: ("./models/depth_anything_v2/depth_anything_v2_vitb.pth", _flat, _vit(DepthAnythingV2Engine, 'vitb')),
+    14: ("./models/depth_anything_v2/depth_anything_v2_vitl.pth", _flat, _vit(DepthAnythingV2Engine, 'vitl')),
 }
 PIX2PIX_CHECKPOINT = "./models/pix2pix/latest_net_G.pth"
 DAV2_ENCODERS = {12: 'vits', 13: 'vitb', 14: 'vitl'}
@@ -1627,11 +1553,7 @@ class ModelHolder:
                                       f"8 = ZoeDepth-K; 9 = ZoeDepth-NK; 12, 13, 14 = Depth-Anything-V2 S/B/L)")
         dev = torch.device(device)
         path, unwrap, make = CHECKPOINTS[model_type]
-        if route == "split":     # always the op-level engine: the model-level handle has no split path
-            model = DepthAnythingV2Engine(self._load_checkpoint(model_type, path, unwrap), DAV2_ENCODERS[model_type], dev,
-                                          bool(tiling_mode), split=True)
-        else:
-            model = make(self._load_checkpoint(model_type, path, unwrap), model_type, dev, boost, bool(tiling_mode))
+        model = make(self._load_checkpoint(model_type, path, unwrap), dev, bool(tiling_mode), route == "split")
         if boost:      # reference :284-299: the pix2pix merge network ('latest_net_G.pth', netG = unet_1024, norm none)
             from .boost import BoostPipeline, UnetMergeEngine
             self.pix2pix_model = BoostPipeline(model, UnetMergeEngine(self._load_checkpoint("pix2pix", PIX2PIX_CHECKPOINT), dev), dev, model_type)
@@ -1677,8 +1599,6 @@ class ModelHolder:
 
     def unload_models(self):
         if self.depth_model is not None or self.pix2pix_model is not None:
-            if hasattr(self.depth_model, "close"):
-                self.depth_model.close()
             self.depth_model = None
             self.pix2pix_model = None
             gc.collect()
@@ -1693,11 +1613,14 @@ class ModelHolder:
     # ---- prediction ------------------------------------------------------------------------------------------------
     def get_raw_prediction_batch(self, rgb, net_width, net_height):
         """uint8 CUDA [B,H,W,3] -> (float32 CUDA [B,H,W], invert flag).  Batched form of get_raw_prediction."""
+        import torch
         if self.depth_model is None:
             raise RuntimeError("no depth model loaded; call ensure_models first")
+        if not torch.is_tensor(rgb) or rgb.dtype != torch.uint8 or rgb.dim() != 4 or rgb.shape[-1] != 3:
+            raise ValueError("rgb must be a uint8 tensor [B,H,W,3]")      # the kernels read the tensor's memory as such
+        rgb = rgb.contiguous()
         if self.pix2pix_model is not None:
             # boost: estimateboost works on one image at a time (its resolutions and patches depend on the image); the net size is ignored
-            import torch
             preds = [self.pix2pix_model.run(rgb[i].cpu().numpy(), self.boost_rmax, to_host=False) for i in range(rgb.shape[0])]
             return torch.stack(preds), self.depth_model_type in [0, 7, 8, 9, 10]
         if self.depth_model_type in (0, 1, 2, 3, 5, 7, 8, 9, 12, 13, 14):

@@ -108,21 +108,25 @@ def test_beit_large_512_net_1600_vs_oracle(cuda_device):
     precision.check(f"{name} net 1600 (streamed relative-position table)", got, want, ref16)
 
 
-def test_native_model_net_1536_equals_engine(cuda_device):
-    """model-level handle, type 1 at net 1536 (a 96 x 96 window, whose whole table would not fit in shared memory): a result,
-    bit-identical to the op-level engine"""
+def test_graph_net_1536_equals_eager(cuda_device, monkeypatch):
+    """type 1 at net 1536 (a 96 x 96 window, whose whole table would not fit in shared memory) through the engine's CUDA graph
+    (call 2 captures, call 3 replays): a result, bit-identical to the eager engine"""
     import torch
-    from depthmap_b200.depthmap_generation import DptBeitEngine, NativeDepthModel
+    from depthmap_b200.depthmap_generation import DptBeitEngine
     from oracle import synth_weights
     sd = synth_weights.make_beit_dpt_state_dict('beitl16_512', seed=3)
     rgb = torch.from_numpy(synth_rgb(1536, 1536, 41)).unsqueeze(0).to(cuda_device)
-    native = NativeDepthModel(sd, 1, cuda_device)
-    a = native.forward_batch(rgb, 1536, 1536).clone()
-    native.close()
+    monkeypatch.setenv("DEPTHMAP_B200_MODEL_GRAPH", "0")
+    eager = DptBeitEngine(sd, 'beitl16_512', cuda_device)
+    a = eager.forward_batch(rgb, 1536, 1536)
+    del eager
+    torch.cuda.empty_cache()
+    monkeypatch.delenv("DEPTHMAP_B200_MODEL_GRAPH")
     eng = DptBeitEngine(sd, 'beitl16_512', cuda_device)
-    b = eng.forward_batch(rgb, 1536, 1536)
     assert torch.isfinite(a).all() and float(a.max() - a.min()) > 0
-    assert torch.equal(a, b)
+    for call in range(3):
+        assert torch.equal(eng.forward_batch(rgb, 1536, 1536), a), call
+    assert eng._graphs._graphs
 
 
 # ---- B: pre-processing of float crops -----------------------------------------------------------------------------------

@@ -133,6 +133,7 @@ def fake(monkeypatch):
     monkeypatch.setattr(torch.cuda, "current_stream", lambda *a: cur[0])
     monkeypatch.setattr(torch.cuda, "synchronize", lambda *a: None)
     monkeypatch.setattr(torch.cuda, "empty_cache", lambda: None)
+    monkeypatch.setenv("DEPTHMAP_B200_MODEL_GRAPH", "0")
     monkeypatch.setenv("DEPTHMAP_B200_LERES_GRAPH", "0")
     monkeypatch.setenv("DEPTHMAP_B200_UNET_GRAPH", "0")
     return rec

@@ -30,8 +30,6 @@ INDIRECT = {
     "dm_video_select_hist": "video_mode.process_predictions_batch's percentile selection (test_video_gpu.py)",
     "dm_video_select_pick": "video_mode.process_predictions_batch's percentile selection (test_video_gpu.py)",
     "dm_video_select_bounds": "video_mode.process_predictions_batch's percentile selection (test_video_gpu.py)",
-    "dm_model_net_size": "NativeModel.net_size against the engine's (test_model_cabi_gpu.py)",
-    "dm_model_launches": "NativeModel's launch count, compared with the op-level engine's (test_model_cabi_gpu.py)",
     "dm_unet_first": "the merge U-Net at its only shape, 1024^2, held to 1e-4 (test_boost_gpu.py::test_merge_unet_vs_oracle)",
     "dm_unet_first_cols": "the merge U-Net (test_boost_gpu.py::test_merge_unet_vs_oracle)",
     "dm_unet_down_cols": "the merge U-Net (test_boost_gpu.py::test_merge_unet_vs_oracle)",
@@ -43,7 +41,6 @@ INDIRECT = {
     "dm_leres_stem_im2col": "the LeReS engine's stem on uint8 images (test_leres_gpu.py::test_leres_vs_oracle)",
     "dm_leres_stem_im2col_f32": "the LeReS stem on one float crop (test_boost_gpu.py::test_leres_on_float_crop_vs_oracle)",
     "dm_leres_stem_im2col_f32_batch": "the LeReS stem on BOOST's batched crops (test_boost_gpu.py::test_estimateboost_vs_oracle)",
-    "dm_vit_pos_embed": "DptVitEngine's position embedding (test_model_cabi_gpu.py::test_native_vit_equals_op_level_path)",
 }
 
 

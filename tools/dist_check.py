@@ -18,7 +18,7 @@ def main():
     import torch
     import torch.distributed as dist
     from depthmap_b200.core import normalize_prediction_batch
-    from depthmap_b200.depthmap_generation import NativeDepthModel
+    from depthmap_b200.depthmap_generation import DepthAnythingV2Engine
     from depthmap_b200.dist import all_gather_batch, shard_range
     from depthmap_b200.normalmap_generation import create_normalmap_batch
     from depthmap_b200.stereoimage_generation import create_stereoimages_batch
@@ -31,7 +31,7 @@ def main():
     dist.init_process_group("nccl", device_id=dev, timeout=datetime.timedelta(minutes=5))
     n = 2 * world + 1                                   # uneven shards on purpose
     rgb = torch.from_numpy(np.stack([synth_rgb(84, 112, 300 + i) for i in range(n)])).to(dev)
-    model = NativeDepthModel(synth_weights.make_dav2_state_dict('vits', seed=1), 12, dev)
+    model = DepthAnythingV2Engine(synth_weights.make_dav2_state_dict('vits', seed=1), 'vits', dev)
 
     def pipeline(x):
         pred = model.forward_batch(x, 84, 84)

@@ -1,5 +1,5 @@
 """Tool for ncu: one eager step of a bench workload between cudaProfilerStart / Stop (use `ncu --profile-from-start off`).
-The model handle's own CUDA graph is disabled so that every kernel is an individual launch.
+The ViT / DPT engines' CUDA graph is disabled so that every kernel is an individual launch.
 usage: DEPTHMAP_B200_MODEL_GRAPH=0 python tools/profile_step.py [depth_beit512|dav2_stereo|stereo2048] [batch]"""
 import os
 import sys
