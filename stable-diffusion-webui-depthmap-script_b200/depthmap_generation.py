@@ -57,14 +57,38 @@ def dav2_net_size(width, height, target, multiple_of=14):
             _constrain_to_multiple_of(sh * height, multiple_of, min_val=target))
 
 
-def _conv_w(w, cin_pad, cout_pad, dtype=None):
-    """[Cout, Cin, 3, 3] -> [cout_pad, 9*cin_pad] (fp16 unless `dtype`), K ordered (ky, kx, cin)."""
+# ---- the kernels' weight layout: zero-padded [N, K] matrices (fp16, or fp32 for split_weight), (ky, kx, cin) 3x3 filters, fp32
+# bias vectors.  Every engine packs its checkpoint through these three.
+def _mat(m, rows=None, cols=None, dtype=None):
+    """[N, ...] (flattened to [N, K]) -> [rows, cols] fp16 (unless `dtype`), zero padded"""
     import torch
     dtype = dtype or torch.float16
-    co, ci = w.shape[:2]
+    m = m.reshape(m.shape[0], -1)
+    t = torch.zeros(rows or m.shape[0], cols or m.shape[1], dtype=dtype, device=m.device)
+    t[:m.shape[0], :m.shape[1]] = m.to(dtype)
+    return t
+
+
+def _conv_w(w, cin_pad=None, cout_pad=None, dtype=None, groups=1):
+    """[Cout, Cin/groups, 3, 3] -> [cout_pad, 9*cin_pad] fp16 (unless `dtype`), K ordered (ky, kx, cin), zero padded; the groups
+    become diagonal blocks of a dense filter"""
+    import torch
+    dtype = dtype or torch.float16
+    co, cig = w.shape[:2]
+    cin_pad, cout_pad, cog = cin_pad or cig * groups, cout_pad or co, co // groups
     t = torch.zeros(cout_pad, 3, 3, cin_pad, dtype=dtype, device=w.device)
-    t[:co, :, :, :ci] = w.permute(0, 2, 3, 1).to(dtype)
+    wp = w.permute(0, 2, 3, 1).to(dtype)
+    for g in range(groups):
+        t[g * cog:(g + 1) * cog, :, :, g * cig:(g + 1) * cig] = wp[g * cog:(g + 1) * cog]
     return t.reshape(cout_pad, 9 * cin_pad).contiguous()
+
+
+def _vec(b, n=None):
+    """[n] fp32, zero padded"""
+    import torch
+    t = torch.zeros(n or b.numel(), dtype=torch.float32, device=b.device)
+    t[:b.numel()] = b.float().reshape(-1)
+    return t
 
 
 class SplitWeight:
@@ -91,13 +115,6 @@ def split_weight(m, groups=1):
     return SplitWeight(torch.cat([g(hi), g(hi), g(lo)], dim=2).reshape(N, 3 * K).contiguous(), torch.exp2(-e).contiguous())
 
 
-def _pad_vec(b, n):
-    import torch
-    t = torch.zeros(n, dtype=torch.float32, device=b.device)
-    t[:b.numel()] = b.float().reshape(-1)
-    return t
-
-
 class DepthAnythingV2Engine:
     """Depth-Anything-V2 (DINOv2 ViT + DPT head) forward on the sm_90a kernels.
 
@@ -120,6 +137,7 @@ class DepthAnythingV2Engine:
     FINAL_RESIZE_MODE = 0  # bilinear, align_corners=True (src/depthmap_generation.py:558)
     CONFIGS = DAV2_CONFIGS
     SUPPORTS_SPLIT = True
+    NEEDS_READOUT = False       # the features come through the final LayerNorm (emit_feature), not a readout projection
 
     def __init__(self, state_dict, encoder, device, circular=False, split=False):
         import torch
@@ -140,72 +158,66 @@ class DepthAnythingV2Engine:
 
     # ---- weight packing --------------------------------------------------------------------------------------------
     def _pack(self, sd):
+        """sd in Depth-Anything-V2's checkpoint layout, which the MiDaS DPT engines map theirs to (_MidasDptEngine._pack).  Without
+        POS_EMBED there is no 'pretrained.pos_embed', with NEEDS_READOUT no final 'pretrained.norm'."""
         import torch
         dev = self.device
         cfg = self.cfg
         C, Fch, oc = cfg['embed_dim'], cfg['features'], cfg['out_channels']
-        split = self.split
         # GEMM / conv operands: fp16, or (split) built in fp32 and packed by split_weight; `groups` = the taps of a 3x3 filter
-        wdt = torch.float32 if split else torch.float16
-        op = (lambda t, groups=1: split_weight(t, groups)) if split else (lambda t, groups=1: t)
-        gw = lambda t: op(t.detach().to(dev, wdt).contiguous())
-        f32 = lambda t: t.detach().to(dev, torch.float32).contiguous()
+        wdt = torch.float32 if self.split else torch.float16
+        op = (lambda t, groups=1: split_weight(t, groups)) if self.split else (lambda t, groups=1: t)
+        key = lambda k: sd[k].detach().to(dev)
+        mat = lambda k, rows=None, cols=None: op(_mat(key(k), rows, cols, wdt))
+        conv_w = lambda k, ci, co: op(_conv_w(key(k), ci, co, wdt), 9)
+        vec = lambda k, n=None: _vec(key(k), n)
         w = {}
-        pw = sd['pretrained.patch_embed.proj.weight'].detach().to(dev).reshape(C, -1)
-        self.kpad = _ru(pw.shape[1], 64)
-        t = torch.zeros(C, self.kpad, dtype=wdt, device=dev)
-        t[:, :pw.shape[1]] = pw.to(wdt)
-        w['pe_w'], w['pe_b'] = op(t), f32(sd['pretrained.patch_embed.proj.bias'])
-        w['cls'] = f32(sd['pretrained.cls_token']).reshape(C)
-        self._pos_embed = f32(sd['pretrained.pos_embed'])
+        self.kpad = _ru(sd['pretrained.patch_embed.proj.weight'][0].numel(), 64)
+        w['pe_w'], w['pe_b'] = mat('pretrained.patch_embed.proj.weight', cols=self.kpad), vec('pretrained.patch_embed.proj.bias')
+        w['cls'] = vec('pretrained.cls_token')
+        self._pos_embed = vec('pretrained.pos_embed').view_as(sd['pretrained.pos_embed']) if self.POS_EMBED else None
         blocks = []
         for i in range(cfg['depth']):
             p = f'pretrained.blocks.{i}.'
             blocks.append(dict(
-                ln1_w=f32(sd[p + 'norm1.weight']), ln1_b=f32(sd[p + 'norm1.bias']),
-                qkv_w=gw(sd[p + 'attn.qkv.weight']), qkv_b=f32(sd[p + 'attn.qkv.bias']),
-                proj_w=gw(sd[p + 'attn.proj.weight']), proj_b=f32(sd[p + 'attn.proj.bias']), ls1=f32(sd[p + 'ls1.gamma']),
-                ln2_w=f32(sd[p + 'norm2.weight']), ln2_b=f32(sd[p + 'norm2.bias']),
-                fc1_w=gw(sd[p + 'mlp.fc1.weight']), fc1_b=f32(sd[p + 'mlp.fc1.bias']),
-                fc2_w=gw(sd[p + 'mlp.fc2.weight']), fc2_b=f32(sd[p + 'mlp.fc2.bias']), ls2=f32(sd[p + 'ls2.gamma'])))
+                ln1_w=vec(p + 'norm1.weight'), ln1_b=vec(p + 'norm1.bias'),
+                qkv_w=mat(p + 'attn.qkv.weight'), qkv_b=vec(p + 'attn.qkv.bias'),
+                proj_w=mat(p + 'attn.proj.weight'), proj_b=vec(p + 'attn.proj.bias'), ls1=vec(p + 'ls1.gamma'),
+                ln2_w=vec(p + 'norm2.weight'), ln2_b=vec(p + 'norm2.bias'),
+                fc1_w=mat(p + 'mlp.fc1.weight'), fc1_b=vec(p + 'mlp.fc1.bias'),
+                fc2_w=mat(p + 'mlp.fc2.weight'), fc2_b=vec(p + 'mlp.fc2.bias'), ls2=vec(p + 'ls2.gamma')))
         w['blocks'] = blocks
-        w['norm_w'], w['norm_b'] = f32(sd['pretrained.norm.weight']), f32(sd['pretrained.norm.bias'])
+        if not self.NEEDS_READOUT:
+            w['norm_w'], w['norm_b'] = vec('pretrained.norm.weight'), vec('pretrained.norm.bias')
         # ---- DPT head; channel counts padded to multiples of 64 with zero weights (ViT-S/B have 48/96-wide maps) ----
         self.ocp = [_ru(c, 64) for c in oc]
         self.Fp = _ru(Fch, 64)
         self.F2p = _ru(Fch // 2, 64)
         h = 'depth_head.'
-        conv_w = lambda wt, ci, co: op(_conv_w(wt, ci, co, wdt), 9)
         for i in range(4):
-            t = torch.zeros(self.ocp[i], C, dtype=wdt, device=dev)
-            t[:oc[i]] = sd[h + f'projects.{i}.weight'].detach().to(dev).reshape(oc[i], C).to(wdt)
-            w[f'proj{i}_w'], w[f'proj{i}_b'] = op(t), _pad_vec(sd[h + f'projects.{i}.bias'].detach().to(dev), self.ocp[i])
+            w[f'proj{i}_w'], w[f'proj{i}_b'] = mat(h + f'projects.{i}.weight', self.ocp[i]), vec(h + f'projects.{i}.bias', self.ocp[i])
         for i, s in ((0, 4), (1, 2)):  # ConvTranspose2d(k = s): W[(i,j,co), ci] = w[ci, co, i, j]
-            wt = sd[h + f'resize_layers.{i}.weight'].detach().to(dev)  # [ci, co, s, s]
+            wt = key(h + f'resize_layers.{i}.weight')  # [ci, co, s, s]
             t = torch.zeros(s, s, self.ocp[i], self.ocp[i], dtype=wdt, device=dev)
             t[:, :, :oc[i], :oc[i]] = wt.permute(2, 3, 1, 0).to(wdt)
             w[f'up{i}_w'] = op(t.reshape(s * s * self.ocp[i], self.ocp[i]).contiguous())
-            w[f'up{i}_b'] = _pad_vec(sd[h + f'resize_layers.{i}.bias'].detach().to(dev), self.ocp[i]).repeat(s * s).contiguous()
-        w['down3_w'] = conv_w(sd[h + 'resize_layers.3.weight'].detach().to(dev), self.ocp[3], self.ocp[3])
-        w['down3_b'] = _pad_vec(sd[h + 'resize_layers.3.bias'].detach().to(dev), self.ocp[3])
+            w[f'up{i}_b'] = vec(h + f'resize_layers.{i}.bias', self.ocp[i]).repeat(s * s).contiguous()
+        w['down3_w'] = conv_w(h + 'resize_layers.3.weight', self.ocp[3], self.ocp[3])
+        w['down3_b'] = vec(h + 'resize_layers.3.bias', self.ocp[3])
         for i in range(4):
-            w[f'rn{i}_w'] = conv_w(sd[h + f'scratch.layer{i + 1}_rn.weight'].detach().to(dev), self.ocp[i], self.Fp)
+            w[f'rn{i}_w'] = conv_w(h + f'scratch.layer{i + 1}_rn.weight', self.ocp[i], self.Fp)
         for i in range(1, 5):
             r = h + f'scratch.refinenet{i}.'
-            t = torch.zeros(self.Fp, self.Fp, dtype=wdt, device=dev)
-            t[:Fch, :Fch] = sd[r + 'out_conv.weight'].detach().to(dev).reshape(Fch, Fch).to(wdt)
-            w[f'rf{i}_out_w'], w[f'rf{i}_out_b'] = op(t), _pad_vec(sd[r + 'out_conv.bias'].detach().to(dev), self.Fp)
+            w[f'rf{i}_out_w'] = mat(r + 'out_conv.weight', self.Fp, self.Fp)
+            w[f'rf{i}_out_b'] = vec(r + 'out_conv.bias', self.Fp)
             for u in (1, 2):
                 for cv in (1, 2):
                     k = r + f'resConfUnit{u}.conv{cv}.'
                     if k + 'weight' in sd:
-                        w[f'rf{i}_u{u}c{cv}_w'] = conv_w(sd[k + 'weight'].detach().to(dev), self.Fp, self.Fp)
-                        w[f'rf{i}_u{u}c{cv}_b'] = _pad_vec(sd[k + 'bias'].detach().to(dev), self.Fp)
-        w['oc1_w'] = conv_w(sd[h + 'scratch.output_conv1.weight'].detach().to(dev), self.Fp, self.F2p)
-        w['oc1_b'] = _pad_vec(sd[h + 'scratch.output_conv1.bias'].detach().to(dev), self.F2p)
-        w['oc2_w'] = conv_w(sd[h + 'scratch.output_conv2.0.weight'].detach().to(dev), self.F2p, 32)
-        w['oc2_b'] = f32(sd[h + 'scratch.output_conv2.0.bias'])
-        w['oc3_w'] = f32(sd[h + 'scratch.output_conv2.2.weight']).reshape(32)
+                        w[f'rf{i}_u{u}c{cv}_w'], w[f'rf{i}_u{u}c{cv}_b'] = conv_w(k + 'weight', self.Fp, self.Fp), vec(k + 'bias', self.Fp)
+        w['oc1_w'], w['oc1_b'] = conv_w(h + 'scratch.output_conv1.weight', self.Fp, self.F2p), vec(h + 'scratch.output_conv1.bias', self.F2p)
+        w['oc2_w'], w['oc2_b'] = conv_w(h + 'scratch.output_conv2.0.weight', self.F2p, 32), vec(h + 'scratch.output_conv2.0.bias')
+        w['oc3_w'] = vec(h + 'scratch.output_conv2.2.weight')
         self.oc3_b = float(sd[h + 'scratch.output_conv2.2.bias'].detach().float().reshape(-1)[0])
         self.w = w
 
@@ -256,7 +268,7 @@ class DepthAnythingV2Engine:
         b['att'] = h16(B * N, C)
         b['mlp'] = h16(B * N, 4 * C)
         b['feat'] = [h16(B * Np, C) for _ in range(4)]
-        b['cat'] = h16(B * Np, 2 * C) if getattr(self, 'NEEDS_READOUT', False) else None
+        b['cat'] = h16(B * Np, 2 * C) if self.NEEDS_READOUT else None
         sizes = [(gh * 4, gw * 4), (gh * 2, gw * 2), (gh, gw), ((gh - 1) // 2 + 1, (gw - 1) // 2 + 1)]
         b['sizes'] = sizes
         b['p'] = [h16(B * Np, self.ocp[i]) for i in range(4)]
@@ -281,8 +293,12 @@ class DepthAnythingV2Engine:
         # circular padding: the halo copy of a 3x3 convolution's input, sized for the largest one
         convs = [(s, c) for s, c in zip(sizes, self.ocp)] + [(s, Fp) for s in sizes] + [(up[3], Fp), ((nh, nw), self.F2p)]
         b['halo'] = h16(max(B * (h + 2) * (w + 2) * c for (h, w), c in convs)) if self.circular else None
+        self._head_buffers(b, B, nh, nw)
         self._bufs, self._buf_key = b, key
         return b
+
+    def _head_buffers(self, b, B, nh, nw):
+        """hook: a head's own buffers, added to `b` (kept and replaced with the rest)"""
 
     # ---- model-family hooks ------------------------------------------------------------------------------------------
     def net_size(self, W, H, net_w, net_h):
@@ -357,7 +373,7 @@ class DepthAnythingV2Engine:
         else:
             ops.gemm(b['patches'], self.kpad, w['pe_w'], self.kpad, B * Np, C, self.kpad, bias=w['pe_b'], C=b['pe'], ldc=C)
         ops.call("dm_assemble_tokens_f32" if self.split else "dm_assemble_tokens", b['pe'], w['cls'],
-                 self._pos(gh, gw) if self._pos_embed is not None else None, b['x'], B, Np, C)
+                 self._pos(gh, gw) if self.POS_EMBED else None, b['x'], B, Np, C)
         rows = B * N
         fi = 0
         for i, blk in enumerate(w['blocks']):
@@ -412,14 +428,16 @@ class DepthAnythingV2Engine:
             self._gemm(b[f'u{li}'], Fp, w[f'rf{rf}_out_w'], Fp, B * s[0] * s[1], Fp, Fp, bias=w[f'rf{rf}_out_b'], C=b['v'][step + 1], ldc=Fp)
             ops.call(self._resize, b['v'][step + 1], B, s[0], s[1], Fp, b['path'][step + 1], t[0], t[1])
 
-    def run_head(self, b, B, nh, nw):
-        """output_conv (dpt.py:139-150 / dpt_depth.py:150-158) -> the net-size prediction [B, nh, nw] (a pooled buffer, valid until
-        the next forward at this shape)."""
-        ops, w = self.ops, self.w
-        Fp = self.Fp
+    def run_output_conv1(self, b, B, nh, nw):
+        """output_conv's first 3x3 conv (dpt.py:139-150 / dpt_depth.py:150-158) and the resize to the net size -> b['oc1u']"""
         t = b['up_sizes'][3]
-        self._conv(b['path'][3], B, t[0], t[1], Fp, w['oc1_w'], self.F2p, bias=w['oc1_b'], C=b['oc1'], halo=b['halo'])
-        ops.call(self._resize, b['oc1'], B, t[0], t[1], self.F2p, b['oc1u'], nh, nw)
+        self._conv(b['path'][3], B, t[0], t[1], self.Fp, self.w['oc1_w'], self.F2p, bias=self.w['oc1_b'], C=b['oc1'], halo=b['halo'])
+        self.ops.call(self._resize, b['oc1'], B, t[0], t[1], self.F2p, b['oc1u'], nh, nw)
+
+    def run_head(self, b, B, nh, nw):
+        """output_conv -> the net-size prediction [B, nh, nw] (a pooled buffer, valid until the next forward at this shape)."""
+        w = self.w
+        self.run_output_conv1(b, B, nh, nw)
         # conv3x3 -> ReLU -> conv1x1 -> ReLU (+ the outer F.relu, idempotent) fused into one epilogue
         self._conv(b['oc1u'], B, nh, nw, self.F2p, w['oc2_w'], 32, epi=_lib.EPI_HEAD, act=_lib.ACT_RELU, bias=w['oc2_b'], X=b['d'],
                     gamma=w['oc3_w'], head_b2=self.oc3_b, halo=b['halo'])
@@ -467,6 +485,13 @@ def midas_boost_net_size(width, height, msize, multiple_of=32):
     return midas_upper_bound_net_size(width, height, msize, msize, multiple_of)
 
 
+def _check_rects(rects, hi, wi):
+    """BOOST's crops (x0, y0, w, h) must lie inside the wi x hi image"""
+    for x0, y0, w, h in rects:
+        if x0 < 0 or y0 < 0 or w <= 0 or h <= 0 or x0 + w > wi or y0 + h > hi:
+            raise ValueError(f"crop {(x0, y0, w, h)} outside the {wi}x{hi} image")
+
+
 def _midas_crop_groups(planar, rects, msize):
     """estimatemidasBoost's crops (x0, y0, w, h) of one planar fp32 image [3, Hi, Wi] -> (Hi, Wi, {(nh, nw): [crop indices]}): each
     crop at its upper-bound net size for msize.  Crops clipped at the image border are not square, hence the grouping."""
@@ -474,10 +499,9 @@ def _midas_crop_groups(planar, rects, msize):
     hi, wi = int(planar.shape[1]), int(planar.shape[2])
     if planar.dtype != torch.float32 or planar.dim() != 3 or planar.shape[0] != 3 or not planar.is_contiguous():
         raise ValueError("planar must be a contiguous float32 tensor [3, H, W]")
+    _check_rects(rects, hi, wi)
     groups = {}
     for k, (x0, y0, w, h) in enumerate(rects):
-        if x0 < 0 or y0 < 0 or w <= 0 or h <= 0 or x0 + w > wi or y0 + h > hi:
-            raise ValueError(f"crop {(x0, y0, w, h)} outside the {wi}x{hi} image")
         nw, nh = midas_boost_net_size(w, h, msize)
         if nw <= 0 or nh <= 0:
             raise ValueError(f"crop {w}x{h} is too elongated for a net of at most {msize} px")
@@ -485,19 +509,45 @@ def _midas_crop_groups(planar, rects, msize):
     return hi, wi, groups
 
 
-class DptBeitEngine(DepthAnythingV2Engine):
-    """MiDaS 3.1 DPT-BEiT (dpt_beit_large_512 / _384) on the sm_90a kernels.
+class _MidasBoost:
+    """BOOST on a MiDaS network (estimatemidasBoost, src/depthmap_generation.py:1180-1220): forward_batch(None, msize, msize,
+    planar=(img, rect)) -> _forward_crop, and forward_crops(img, rects, msize), on float crops of a planar fp32 image: upper-bound net
+    size (midas_boost_net_size), ImageNet mean / std, the channel order of the crop unchanged (network channel c = plane 2 - c of
+    the RGB image), and a cv2 INTER_CUBIC resize of the prediction back to the crop.  The engine supplies _crops_network."""
 
-    Mirrors the reference's overriding forwards (dmidas/backbones/beit.py:18-129), the reassemble stage
-    (dmidas/backbones/utils.py:28-39,83-124,144-249), DPT / DPTDepthModel (dmidas/dpt_depth.py:110-166) and estimatemidas
-    (src/depthmap_generation.py:455-499).  The relative-position bias, which the reference rebuilds (bilinear table
-    resize + gather) in every block of every forward, is resized once per resolution into a per-head fp32 table per block;
-    the fused attention kernel gathers from it (csrc/attention_wgmma.cu), so no [heads, N, N] tensor exists.
+    BOOST_MEAN = (0.485, 0.456, 0.406)
+    BOOST_STD = (0.229, 0.224, 0.225)
 
-    BOOST (estimatemidasBoost, src/depthmap_generation.py:1180-1220) calls forward_batch(None, msize, msize, planar=(img, rect))
-    and forward_crops(img, rects, msize) on float crops of a planar fp32 image: upper-bound net size (midas_boost_net_size),
-    ImageNet mean / std, the channel order of the crop unchanged (network channel c = plane 2 - c of the RGB image), and a cv2
-    INTER_CUBIC resize of the prediction back to the crop."""
+    def _boost_consts(self):
+        return (ctypes.c_float * 3)(*self.BOOST_MEAN), (ctypes.c_float * 3)(*self.BOOST_STD), (ctypes.c_int * 3)(*self.CHAN_MAP)
+
+    def _forward_crop(self, planar, rect, msize):
+        """estimatemidasBoost's network and resize on one crop -> [1, h, w] (not normalised)"""
+        return self.forward_crops(planar, [rect], msize)[0].unsqueeze(0)
+
+    def forward_crops(self, planar, rects, msize):
+        """B crops (x0, y0, w, h) of one planar fp32 image [3, Hi, Wi] -> [fp32 CUDA [h, w]] in the order of `rects`: each crop at its
+        upper-bound net size for msize, then cv2-cubic back to the crop.  Crops clipped at the image border are not square, so the
+        crops are grouped by net shape, one batched forward per shape."""
+        import torch
+        hi, wi, groups = _midas_crop_groups(planar, rects, msize)
+        out = [None] * len(rects)
+        for (nh, nw), ks in groups.items():
+            r = torch.tensor([[int(v) for v in rects[k]] for k in ks], dtype=torch.int32).to(self.device)
+            d = self._crops_network(planar, hi, wi, r, len(ks), nh, nw)
+            for i, k in enumerate(ks):
+                w, h = int(rects[k][2]), int(rects[k][3])
+                o = torch.empty(h, w, dtype=torch.float32, device=self.device)
+                self.ops.call("dm_boost_resize_cubic", d[i], nw, 0, nh, nw, o, w, 0, h, w, 1)
+                out[k] = o
+        return out
+
+
+class _MidasDptEngine(_MidasBoost, DepthAnythingV2Engine):
+    """What the MiDaS DPT networks (DptBeitEngine, DptVitEngine) share on the Depth-Anything-V2 engine: the checkpoint layout
+    (trunk under 'pretrained.model.', decoder under 'scratch.'), the readout projection of the reassemble stage, DPT /
+    DPTDepthModel (dmidas/dpt_depth.py:31-166), estimatemidas' pre-processing and bicubic resize back (src/depthmap_generation.py:
+    455-499), and BOOST (_MidasBoost)."""
 
     PATCH = 16
     MEAN = (0.5, 0.5, 0.5)
@@ -505,36 +555,27 @@ class DptBeitEngine(DepthAnythingV2Engine):
     SUPPORTS_SPLIT = False
     CHAN_MAP = (2, 1, 0)        # estimatemidas receives the BGR-swapped image of get_raw_prediction (:381) unchanged
     FINAL_RESIZE_MODE = 1       # bicubic, align_corners=False (:487-497)
-    CONFIGS = BEIT_CONFIGS
     NEEDS_READOUT = True
 
     def net_size(self, W, H, net_w, net_h):
         return midas_net_size(W, H, net_w, net_h)
 
+    def _block_keys(self, sd, blk):
+        """hook: the full qkv bias and the LayerScale gammas of the block with checkpoint prefix `blk`, under Depth-Anything-V2's keys"""
+        raise NotImplementedError
+
     def _pack(self, sd):
-        import torch
-        dev = self.device
-        cfg = self.cfg
-        C = cfg['embed_dim']
-        f16 = lambda t: t.detach().to(dev, torch.float16).contiguous()
-        f32 = lambda t: t.detach().to(dev, torch.float32).contiguous()
-        # re-key the MiDaS checkpoint into the layout the shared packer understands
-        m = {}
+        """the MiDaS checkpoint mapped to the layout of DepthAnythingV2Engine._pack, plus the readout projections"""
         p = 'pretrained.model.'
-        m['pretrained.patch_embed.proj.weight'] = sd[p + 'patch_embed.proj.weight']
-        m['pretrained.patch_embed.proj.bias'] = sd[p + 'patch_embed.proj.bias']
-        m['pretrained.cls_token'] = sd[p + 'cls_token']
-        m['pretrained.pos_embed'] = torch.zeros(1, 1, C)
-        for i in range(cfg['depth']):
+        m = {'pretrained.' + k: sd[p + k] for k in ('patch_embed.proj.weight', 'patch_embed.proj.bias', 'cls_token')}
+        if self.POS_EMBED:
+            m['pretrained.pos_embed'] = sd[p + 'pos_embed']
+        for i in range(self.cfg['depth']):
             b, d = p + f'blocks.{i}.', f'pretrained.blocks.{i}.'
             for k in ('norm1.weight', 'norm1.bias', 'attn.qkv.weight', 'attn.proj.weight', 'attn.proj.bias', 'norm2.weight', 'norm2.bias',
                       'mlp.fc1.weight', 'mlp.fc1.bias', 'mlp.fc2.weight', 'mlp.fc2.bias'):
                 m[d + k] = sd[b + k]
-            m[d + 'attn.qkv.bias'] = torch.cat((sd[b + 'attn.q_bias'].float(), torch.zeros(C), sd[b + 'attn.v_bias'].float()))
-            m[d + 'ls1.gamma'] = sd[b + 'gamma_1']
-            m[d + 'ls2.gamma'] = sd[b + 'gamma_2']
-        m['pretrained.norm.weight'] = torch.ones(C)
-        m['pretrained.norm.bias'] = torch.zeros(C)
+            m.update({d + k: v for k, v in self._block_keys(sd, b).items()})
         for j in range(4):
             a = f'pretrained.act_postprocess{j + 1}.'
             m[f'depth_head.projects.{j}.weight'] = sd[a + '3.weight']
@@ -546,17 +587,58 @@ class DptBeitEngine(DepthAnythingV2Engine):
         for k, v in sd.items():
             if k.startswith('scratch.layer') or k.startswith('scratch.refinenet'):
                 m['depth_head.' + k] = v
-        m['depth_head.scratch.output_conv1.weight'] = sd['scratch.output_conv.0.weight']
-        m['depth_head.scratch.output_conv1.bias'] = sd['scratch.output_conv.0.bias']
-        m['depth_head.scratch.output_conv2.0.weight'] = sd['scratch.output_conv.2.weight']
-        m['depth_head.scratch.output_conv2.0.bias'] = sd['scratch.output_conv.2.bias']
-        m['depth_head.scratch.output_conv2.2.weight'] = sd['scratch.output_conv.4.weight']
-        m['depth_head.scratch.output_conv2.2.bias'] = sd['scratch.output_conv.4.bias']
+        for d, k in (('output_conv1', 'output_conv.0'), ('output_conv2.0', 'output_conv.2'), ('output_conv2.2', 'output_conv.4')):
+            m[f'depth_head.scratch.{d}.weight'] = sd[f'scratch.{k}.weight']
+            m[f'depth_head.scratch.{d}.bias'] = sd[f'scratch.{k}.bias']
         super()._pack(m)
-        self._pos_embed = None  # BEiT uses no absolute position embedding (use_abs_pos_emb=False)
-        self.w['readout'] = [(f16(sd[f'pretrained.act_postprocess{j + 1}.0.project.0.weight']),
-                              f32(sd[f'pretrained.act_postprocess{j + 1}.0.project.0.bias'])) for j in range(4)]
-        self._tables = [f32(sd[p + f'blocks.{i}.attn.relative_position_bias_table']) for i in range(cfg['depth'])]
+        key = lambda k: sd[f'pretrained.act_postprocess{k}'].detach().to(self.device)
+        self.w['readout'] = [(_mat(key(f'{j + 1}.0.project.0.weight')), _vec(key(f'{j + 1}.0.project.0.bias'))) for j in range(4)]
+
+    def emit_feature(self, b, fi, B, N, C):
+        """forward hook on the raw block output + ProjectReadout: GELU(Linear(cat(tokens, cls)))."""
+        rw, rb = self.w['readout'][fi]
+        self.ops.call("dm_concat_readout_f16", b['x'], B, N, C, b['cat'])
+        self.ops.gemm(b['cat'], 2 * C, rw, 2 * C, B * (N - 1), C, 2 * C, act=_lib.ACT_GELU, bias=rb, C=b['feat'][fi], ldc=C)
+
+    # ---- BOOST: estimatemidasBoost on float crops ---------------------------------------------------------------------
+    def forward_batch(self, rgb, net_w, net_h=None, out_hw=None, planar=None):
+        """rgb: uint8 CUDA [B,H,W,3] -> float32 CUDA [B,H,W] (estimatemidas).  planar = (fp32 CUDA [3,Hi,Wi] image, (x0, y0, w, h))
+        instead of `rgb`: _forward_crop with msize = net_w."""
+        if planar is not None:
+            return self._forward_crop(*planar, net_w)
+        return super().forward_batch(rgb, net_w, net_h, out_hw)
+
+    def _crops_network(self, planar, hi, wi, r, B, nh, nw):
+        # eager: BOOST alternates crop net sizes, and a new shape drops the graphs (_buffers), so a capture would not replay
+        b = self._buffers(B, nh, nw)
+        self.ops.call("dm_preprocess_patchify_f32_crops", planar, hi, wi, r, B, nh, nw, self.PATCH, *self._boost_consts(), b['patches'],
+                      self.kpad, launches=1 + (self.kpad > 3 * self.PATCH ** 2))
+        return self._network(b, B, nh, nw)
+
+
+class DptBeitEngine(_MidasDptEngine):
+    """MiDaS 3.1 DPT-BEiT (dpt_beit_large_512 / _384) on the sm_90a kernels.
+
+    Mirrors the reference's overriding forwards (dmidas/backbones/beit.py:18-129), the reassemble stage
+    (dmidas/backbones/utils.py:28-39,83-124,144-249), DPT / DPTDepthModel (dmidas/dpt_depth.py:110-166) and estimatemidas
+    (src/depthmap_generation.py:455-499).  No absolute position embedding (use_abs_pos_emb=False).  The relative-position bias,
+    which the reference rebuilds (bilinear table resize + gather) in every block of every forward, is resized once per resolution
+    into a per-head fp32 table per block; the fused attention kernel gathers from it (csrc/attention_wgmma.cu), so no
+    [heads, N, N] tensor exists."""
+
+    CONFIGS = BEIT_CONFIGS
+    POS_EMBED = None
+
+    def _block_keys(self, sd, blk):
+        import torch
+        qkv_b = torch.cat((sd[blk + 'attn.q_bias'].float(), torch.zeros(self.cfg['embed_dim']), sd[blk + 'attn.v_bias'].float()))  # no key bias
+        return {'attn.qkv.bias': qkv_b, 'ls1.gamma': sd[blk + 'gamma_1'], 'ls2.gamma': sd[blk + 'gamma_2']}
+
+    def _pack(self, sd):
+        import torch
+        super()._pack(sd)
+        self._tables = [sd[f'pretrained.model.blocks.{i}.attn.relative_position_bias_table'].detach().to(self.device, torch.float32).contiguous()
+                        for i in range(self.cfg['depth'])]
         self._bias_cache = {}
 
     TABLE_RESOLUTIONS = 4      # resized tables kept resident: BOOST alternates between its whole-image and patch windows
@@ -590,48 +672,8 @@ class DptBeitEngine(DepthAnythingV2Engine):
         tabs, nrd = self.rel_tables(gh, gw)
         self.ops.call("dm_attention_relpos_f16", b['qkv'], B, gh, gw, heads, (C // heads) ** -0.5, tabs[i], nrd, b['att'])
 
-    # ---- BOOST: estimatemidasBoost on float crops ---------------------------------------------------------------------
-    BOOST_MEAN = (0.485, 0.456, 0.406)
-    BOOST_STD = (0.229, 0.224, 0.225)
 
-    def forward_batch(self, rgb, net_w, net_h=None, out_hw=None, planar=None):
-        """rgb: uint8 CUDA [B,H,W,3] -> float32 CUDA [B,H,W] (estimatemidas).  planar = (fp32 CUDA [3,Hi,Wi] image, (x0, y0, w, h))
-        instead of `rgb`: estimatemidasBoost's network and resize on that crop with msize = net_w -> [1, h, w] (not normalised)."""
-        if planar is None:
-            return super().forward_batch(rgb, net_w, net_h, out_hw)
-        img, rect = planar
-        return self.forward_crops(img, [rect], net_w)[0].unsqueeze(0)
-
-    def forward_crops(self, planar, rects, msize):
-        """B crops (x0, y0, w, h) of one planar fp32 image [3, Hi, Wi] -> [fp32 CUDA [h, w]] in the order of `rects`: each crop at its
-        upper-bound net size for msize, then cv2-cubic back to the crop.  Crops clipped at the image border are not square, so the
-        crops are grouped by net shape, one batched forward per shape."""
-        import torch
-        hi, wi, groups = _midas_crop_groups(planar, rects, msize)
-        m, sd, cm = (ctypes.c_float * 3)(*self.BOOST_MEAN), (ctypes.c_float * 3)(*self.BOOST_STD), (ctypes.c_int * 3)(*self.CHAN_MAP)
-        out = [None] * len(rects)
-        for (nh, nw), ks in groups.items():
-            B = len(ks)
-            r = torch.tensor([[int(v) for v in rects[k]] for k in ks], dtype=torch.int32).to(self.device)
-            b = self._buffers(B, nh, nw)
-            self.ops.call("dm_preprocess_patchify_f32_crops", planar, hi, wi, r, B, nh, nw, self.PATCH, m, sd, cm, b['patches'], self.kpad,
-                          launches=1 + (self.kpad > 3 * self.PATCH ** 2))
-            d = self._network(b, B, nh, nw)
-            for i, k in enumerate(ks):
-                w, h = int(rects[k][2]), int(rects[k][3])
-                o = torch.empty(h, w, dtype=torch.float32, device=self.device)
-                self.ops.call("dm_boost_resize_cubic", d[i], nw, 0, nh, nw, o, w, 0, h, w, 1)
-                out[k] = o
-        return out
-
-    def emit_feature(self, b, fi, B, N, C):
-        """forward hook on the raw block output + ProjectReadout: GELU(Linear(cat(tokens, cls)))."""
-        rw, rb = self.w['readout'][fi]
-        self.ops.call("dm_concat_readout_f16", b['x'], B, N, C, b['cat'])
-        self.ops.gemm(b['cat'], 2 * C, rw, 2 * C, B * (N - 1), C, 2 * C, act=_lib.ACT_GELU, bias=rb, C=b['feat'][fi], ldc=C)
-
-
-class DptVitEngine(DptBeitEngine):
+class DptVitEngine(_MidasDptEngine):
     """MiDaS 3.0 dpt_large_384 (model type 3) on the sm_90a kernels, op-level path: timm's vit_large_patch16_384 driven by
     the reference's forward_flex (dmidas/backbones/vit.py:12-79,107-118) — absolute position embedding resized bilinearly to
     the current grid, plain (un-biased) attention, no LayerScale — with the hooks, ProjectReadout, reassemble stage and DPT
@@ -641,27 +683,13 @@ class DptVitEngine(DptBeitEngine):
         'vitl16_384': dict(embed_dim=1024, depth=24, heads=16, features=256, out_channels=[256, 512, 1024, 1024], layers=[5, 11, 17, 23], window=24),
         'vit_tiny': dict(embed_dim=128, depth=4, heads=2, features=64, out_channels=[64, 64, 128, 128], layers=[0, 1, 2, 3], window=4),
     }
-
-    def _pack(self, sd):
-        import torch
-        C = self.cfg['embed_dim']
-        p = 'pretrained.model.'
-        m = dict(sd)
-        for i in range(self.cfg['depth']):      # present the ViT block in the layout the BEiT packer reads
-            b = p + f'blocks.{i}.'
-            qb = sd[b + 'attn.qkv.bias'].float()
-            m[b + 'attn.q_bias'], m[b + 'attn.v_bias'] = qb[:C], qb[2 * C:]
-            m[b + 'gamma_1'] = torch.ones(C)
-            m[b + 'gamma_2'] = torch.ones(C)
-            m[b + 'attn.relative_position_bias_table'] = torch.zeros(1, self.cfg['heads'])
-        super()._pack(m)
-        # the key projection DOES have a bias here: restore the full qkv bias the BEiT packer zeroed
-        for i, blk in enumerate(self.w['blocks']):
-            blk['qkv_b'] = sd[p + f'blocks.{i}.attn.qkv.bias'].detach().to(self.device, torch.float32).contiguous()
-        self._pos_embed = sd[p + 'pos_embed'].detach().to(self.device, torch.float32).contiguous()
-
     POS_EMBED = "dm_vit_pos_embed"      # _resize_pos_embed (vit.py:16-31)
-    attention = DepthAnythingV2Engine.attention     # plain attention, no relative-position bias
+
+    def _block_keys(self, sd, blk):
+        import torch
+        # no LayerScale: gammas of one, as the residual epilogue takes a gamma
+        C = self.cfg['embed_dim']
+        return {'attn.qkv.bias': sd[blk + 'attn.qkv.bias'], 'ls1.gamma': torch.ones(C), 'ls2.gamma': torch.ones(C)}
 
 
 class _ResNeXtEngine:
@@ -702,46 +730,27 @@ class _ResNeXtEngine:
             b = (b - sd[bn + '.running_mean'].detach().float()) * scale + sd[bn + '.bias'].detach().float()
         return w, b
 
-    def _mat(self, w, b, kpad=None, npad=None):
-        import torch
-        co = w.shape[0]
-        m = w.reshape(co, -1)
-        k, n = kpad or m.shape[1], npad or co
-        t = torch.zeros(n, k, dtype=torch.float16)
-        t[:co, :m.shape[1]] = m.to(torch.float16)
-        bb = torch.zeros(n, dtype=torch.float32)
-        bb[:co] = b
-        return t.to(self.device).contiguous(), bb.to(self.device).contiguous()
-
-    def _conv3(self, w, b, groups=1, npad=None):
-        """[Co, Ci/g, 3, 3] -> dense fp16 [Co(pad), 9 * Ci], K ordered (ky, kx, ci); groups become diagonal blocks"""
-        import torch
-        co, cig = w.shape[:2]
-        ci = cig * groups
-        n = npad or co
-        t = torch.zeros(n, 3, 3, ci, dtype=torch.float16)
-        wp = w.permute(0, 2, 3, 1).to(torch.float16)             # [Co, ky, kx, Ci/g]
-        cog = co // groups
-        for g in range(groups):
-            t[g * cog:(g + 1) * cog, :, :, g * cig:(g + 1) * cig] = wp[g * cog:(g + 1) * cog]
-        bb = torch.zeros(n, dtype=torch.float32)
-        bb[:co] = b
-        return t.reshape(n, 9 * ci).to(self.device).contiguous(), bb.to(self.device).contiguous()
+    def _packed(self, sd, conv, bn, groups=1, npad=None):
+        """_fold, then the kernels' layout on the device: a 1x1 conv as an fp16 [Co, Ci] matrix, a 3x3 one as an fp16 (ky, kx, ci)
+        filter with its groups as diagonal blocks (exact: the extra products are zeros) and Co zero padded to npad; fp32 bias"""
+        w, b = self._fold(sd, conv, bn)
+        wt = _mat(w) if w.shape[-1] == 1 else _conv_w(w, cout_pad=npad, groups=groups)
+        return wt.to(self.device), _vec(b, npad).to(self.device)
 
     def _pack_encoder(self, sd, stem_conv, stem_bn, block):
         """folded stem (fp16 [64, 192], K ordered (ky, kx, c)) and bottleneck weights; block(li, bi) is the checkpoint prefix of
         bottleneck bi of stage li"""
         sw, sb = self._fold(sd, stem_conv, stem_bn)               # [64, 3, 7, 7] -> [64, (ky, kx, c)] padded to 192
-        stem = self._mat(sw.permute(0, 2, 3, 1).contiguous(), sb, kpad=192)
+        stem = _mat(sw.permute(0, 2, 3, 1), cols=192).to(self.device), _vec(sb).to(self.device)
         blocks = []
         for li, nb in enumerate(self.LAYERS, start=1):
             for bi in range(nb):
                 p = block(li, bi)
                 blk = dict(stride=2 if (bi == 0 and li > 1) else 1)
-                blk['c1'] = self._mat(*self._fold(sd, p + '.conv1', p + '.bn1'))
-                blk['c2'] = self._conv3(*self._fold(sd, p + '.conv2', p + '.bn2'), groups=self.GROUPS)
-                blk['c3'] = self._mat(*self._fold(sd, p + '.conv3', p + '.bn3'))
-                blk['down'] = self._mat(*self._fold(sd, p + '.downsample.0', p + '.downsample.1')) if bi == 0 else None
+                blk['c1'] = self._packed(sd, p + '.conv1', p + '.bn1')
+                blk['c2'] = self._packed(sd, p + '.conv2', p + '.bn2', groups=self.GROUPS)
+                blk['c3'] = self._packed(sd, p + '.conv3', p + '.bn3')
+                blk['down'] = self._packed(sd, p + '.downsample.0', p + '.downsample.1') if bi == 0 else None
                 blk['width'], blk['cout'] = blk['c1'][0].shape[0], blk['c3'][0].shape[0]
                 blocks.append(blk)
         return stem, blocks
@@ -826,6 +835,24 @@ class _ResNeXtEngine:
             feats.append((x, h, wd, cin))
         return feats
 
+    def _stem_cols(self, B, net_h, net_w):
+        """the im2col of the 7x7 / 2 stem conv, K = (ky, kx, c) padded to 192"""
+        return self._buf('stem_cols', (B * ((net_h + 6 - 7) // 2 + 1) * ((net_w + 6 - 7) // 2 + 1), 192))
+
+    # ---- decoder steps: each output is the pooled buffer `name` -------------------------------------------------------
+    def _conv(self, B, halo, name, xin, hh, ww, ci, wb, co, act=_lib.ACT_NONE, R=None, R2=None, C2=False):
+        """3x3 conv (+ bias, act, residuals R / R2) -> its output, or with C2 the epilogue's relu copy of it"""
+        outp = self._buf(name, (B, hh, ww, co))
+        out2 = self._buf(name + '_r', (B, hh, ww, co)) if C2 else None
+        self.ops.conv3x3(xin, B, hh, ww, ci, wb[0], co, act=act, bias=wb[1], C=outp, C2=out2, R=R, R2=R2, halo=halo)
+        return out2 if C2 else outp
+
+    def _up2(self, B, name, xin, hh, ww, c):
+        """x2 bilinear up-sample, align_corners=True"""
+        outp = self._buf(name, (B, 2 * hh, 2 * ww, c))
+        self.ops.call("dm_resize_bilinear_nhwc_f16", xin, B, hh, ww, c, outp, 2 * hh, 2 * ww)
+        return outp
+
     def to(self, device):
         return self
 
@@ -842,22 +869,20 @@ class LeresEngine(_ResNeXtEngine):
     GRAPH_ENV, NAME = "DEPTHMAP_B200_LERES_GRAPH", "LeReS"
 
     def _pack(self, sd):
-        import torch
         E, D = self.ENC, self.DEC
         w = {}
         w['stem'], w['blocks'] = self._pack_encoder(sd, E + 'conv1', E + 'bn1', lambda li, bi: f"{E}layer{li}.{bi}")
 
         def ftb(p):
-            return dict(c1=self._conv3(*self._fold(sd, p + '.conv1', None)),
-                        b1=self._conv3(*self._fold(sd, p + '.conv_branch.1', p + '.conv_branch.2')),
-                        b4=self._conv3(*self._fold(sd, p + '.conv_branch.4', None)))
+            return dict(c1=self._packed(sd, p + '.conv1', None), b1=self._packed(sd, p + '.conv_branch.1', p + '.conv_branch.2'),
+                        b4=self._packed(sd, p + '.conv_branch.4', None))
         w['conv'] = ftb(D + 'conv')
-        w['conv1'] = self._conv3(*self._fold(sd, D + 'conv1', None))
+        w['conv1'] = self._packed(sd, D + 'conv1', None)
         for k in ('ffm2', 'ffm1', 'ffm0'):
             w[k] = (ftb(D + k + '.ftb1'), ftb(D + k + '.ftb2'))
         a = D + 'outconv.adapt_conv'
-        w['ao0'] = self._conv3(*self._fold(sd, a + '.0', a + '.1'))
-        w['ao3'] = self._conv3(*self._fold(sd, a + '.3', None), npad=32)
+        w['ao0'] = self._packed(sd, a + '.0', a + '.1')
+        w['ao3'] = self._packed(sd, a + '.3', None, npad=32)
         self.w = w
 
     # ---- forward ---------------------------------------------------------------------------------------------------
@@ -877,8 +902,7 @@ class LeresEngine(_ResNeXtEngine):
             raise ValueError("LeReS needs a net size that is a multiple of 32")
         self._trim_pools()
         # stem: pre-processing + im2col of the 7x7 / 2 conv, folded BN + ReLU in the GEMM, max-pool
-        h1, w1 = (net_h + 6 - 7) // 2 + 1, (net_w + 6 - 7) // 2 + 1
-        cols = self._buf('stem_cols', (B * h1 * w1, 192))
+        cols = self._stem_cols(B, net_h, net_w)
         m = (ctypes.c_float * 3)(*self.MEAN)
         s = (ctypes.c_float * 3)(*self.STD)
         if planar is None:
@@ -905,12 +929,9 @@ class LeresEngine(_ResNeXtEngine):
         B = len(rects)
         self._trim_pools()
         hi, wi = int(planar.shape[1]), int(planar.shape[2])
-        for x0, y0, w, h in rects:
-            if x0 < 0 or y0 < 0 or w <= 0 or h <= 0 or x0 + w > wi or y0 + h > hi:
-                raise ValueError(f"crop {(x0, y0, w, h)} outside the {wi}x{hi} image")
+        _check_rects(rects, hi, wi)
         r = torch.tensor([list(map(int, q)) for q in rects], dtype=torch.int32).to(self.device)
-        h1 = (net + 6 - 7) // 2 + 1
-        cols = self._buf('stem_cols', (B * h1 * h1, 192))
+        cols = self._stem_cols(B, net, net)
         m = (ctypes.c_float * 3)(*self.MEAN)
         sdev = (ctypes.c_float * 3)(*self.STD)
         self.ops.call("dm_leres_stem_im2col_f32_batch" + self._cv, planar, hi, wi, r, B, net, net, m, sdev, cols)
@@ -923,22 +944,12 @@ class LeresEngine(_ResNeXtEngine):
         # half the net size)
         halo = self._buf('halo', (B * (net_h // 2 + 2) * (net_w // 2 + 2) * 256,)) if self.circular else None
         feats = self._encoder(B, net_h, net_w, cols, halo)
-
-        def conv(name, xin, hh, ww, ci, wb, co, act=_lib.ACT_NONE, R=None, C2=False):
-            outp = self._buf(name, (B, hh, ww, co))
-            out2 = self._buf(name + '_r', (B, hh, ww, co)) if C2 else None
-            ops.conv3x3(xin, B, hh, ww, ci, wb[0], co, act=act, bias=wb[1], C=outp, C2=out2, R=R, halo=halo)
-            return out2 if C2 else outp
+        conv, up2 = functools.partial(self._conv, B, halo), functools.partial(self._up2, B)
 
         def ftb(name, xin, hh, ww, ci, f, cm):
             x1 = conv(name + '_x1', xin, hh, ww, ci, f['c1'], cm, act=_lib.ACT_RELU)           # the in-place ReLU also rewrites the skip operand
             b1 = conv(name + '_b1', x1, hh, ww, cm, f['b1'], cm, act=_lib.ACT_RELU)
             return conv(name + '_o', b1, hh, ww, cm, f['b4'], cm, R=x1, C2=True)             # relu(x1 + branch)
-
-        def up2(name, xin, hh, ww, c):
-            outp = self._buf(name, (B, 2 * hh, 2 * ww, c))
-            ops.call("dm_resize_bilinear_nhwc_f16", xin, B, hh, ww, c, outp, 2 * hh, 2 * ww)
-            return outp
 
         f3, h3, w3, c3 = feats[3]
         x = ftb('dconv', f3, h3, w3, c3, w['conv'], 512)
@@ -974,7 +985,7 @@ class _RequiredKeys(dict):
         raise ValueError(f"{self.what} checkpoint lacks {key!r}")
 
 
-class MidasV21Engine(_ResNeXtEngine):
+class MidasV21Engine(_MidasBoost, _ResNeXtEngine):
     """MiDaS v2.1 (midas_v21, model type 5) on the sm_90a kernels: estimatemidas (src/depthmap_generation.py:455-499) with the
     'upper_bound' resize and ImageNet statistics, around MidasNet (dmidas/midas_net.py:12-76, dmidas/blocks.py:136-320).
 
@@ -1000,14 +1011,13 @@ class MidasV21Engine(_ResNeXtEngine):
         return f"pretrained.layer1.4.{bi}" if li == 1 else f"pretrained.layer{li}.{bi}"
 
     def _pack(self, sd):
-        import torch
         sd = _RequiredKeys(sd, "MiDaS v2.1")
         w = {}
         w['stem'], w['blocks'] = self._pack_encoder(sd, 'pretrained.layer1.0', 'pretrained.layer1.1', self._block)
         def conv(key, bias=True):
             if bias and key + '.bias' not in sd:       # _fold would take a missing bias for zeros
                 raise ValueError(f"MiDaS v2.1 checkpoint lacks {key + '.bias'!r}")
-            return self._conv3(*self._fold(sd, key, None))
+            return self._packed(sd, key, None)
         w['rn'] = [conv(f'scratch.layer{i}_rn', bias=False) for i in range(1, 5)]
         for i in range(1, 5):
             for u in ((2,) if i == 4 else (1, 2)):
@@ -1015,15 +1025,9 @@ class MidasV21Engine(_ResNeXtEngine):
                     w[f'rf{i}_u{u}c{c}'] = conv(f'scratch.refinenet{i}.resConfUnit{u}.conv{c}')
         w['oc0'] = conv('scratch.output_conv.0')
         w['oc2'] = conv('scratch.output_conv.2')
-        w['oc4_w'] = sd['scratch.output_conv.4.weight'].detach().to(self.device, torch.float32).reshape(32).contiguous()
+        w['oc4_w'] = _vec(sd['scratch.output_conv.4.weight'].detach().to(self.device))
         self.oc4_b = float(sd['scratch.output_conv.4.bias'].detach().float().reshape(-1)[0])
         self.w = w
-
-    def _consts(self):
-        return (ctypes.c_float * 3)(*self.MEAN), (ctypes.c_float * 3)(*self.STD), (ctypes.c_int * 3)(*self.CHAN_MAP)
-
-    def _stem_cols(self, B, nh, nw):
-        return self._buf('stem_cols', (B * ((nh + 6 - 7) // 2 + 1) * ((nw + 6 - 7) // 2 + 1), 192))
 
     # ---- forward ---------------------------------------------------------------------------------------------------
     def net_size(self, W, H, net_w, net_h):
@@ -1034,42 +1038,27 @@ class MidasV21Engine(_ResNeXtEngine):
 
     def forward_batch(self, rgb, net_w, net_h=None, out_hw=None, planar=None):
         """rgb: uint8 CUDA [B,H,W,3] -> float32 CUDA [B,H,W] (what estimatemidas returns; invert = False).  planar = (fp32 CUDA [3,Hi,Wi]
-        image, (x0, y0, w, h)) instead of `rgb`: estimatemidasBoost's network and resize on that crop with msize = net_w -> [1, h, w]
-        (not normalised)."""
+        image, (x0, y0, w, h)) instead of `rgb`: _forward_crop with msize = net_w."""
         import torch
         if planar is not None:
-            img, rect = planar
-            return self.forward_crops(img, [rect], net_w)[0].unsqueeze(0)
+            return self._forward_crop(*planar, net_w)
         B, H, W, _ = rgb.shape
         nw, nh = self.net_size(W, H, net_w, net_h if net_h is not None else net_w)
         self._trim_pools()
         cols = self._stem_cols(B, nh, nw)
-        self.ops.call("dm_midas_stem_im2col" + self._cv, rgb, B, H, W, nh, nw, *self._consts(), cols)
+        m, s, c = (ctypes.c_float * 3)(*self.MEAN), (ctypes.c_float * 3)(*self.STD), (ctypes.c_int * 3)(*self.CHAN_MAP)
+        self.ops.call("dm_midas_stem_im2col" + self._cv, rgb, B, H, W, nh, nw, m, s, c, cols)
         d = self._network(B, nh, nw, cols)
         oh, ow = out_hw if out_hw is not None else (H, W)
         out = torch.empty(B, oh, ow, dtype=torch.float32, device=self.device)
         self.ops.call("dm_resize_f32", d, B, nh, nw, out, oh, ow, 1)     # F.interpolate(bicubic, align_corners=False)
         return out
 
-    def forward_crops(self, planar, rects, msize):
-        """B crops (x0, y0, w, h) of one planar fp32 image [3, Hi, Wi] -> [fp32 CUDA [h, w]] in the order of `rects`: each crop at its
-        upper-bound net size for msize, then cv2-cubic back to the crop; one batched forward per net shape."""
-        import torch
-        hi, wi, groups = _midas_crop_groups(planar, rects, msize)
-        self._trim_pools()
-        out = [None] * len(rects)
-        for (nh, nw), ks in groups.items():
-            B = len(ks)
-            r = torch.tensor([[int(v) for v in rects[k]] for k in ks], dtype=torch.int32).to(self.device)
-            cols = self._stem_cols(B, nh, nw)
-            self.ops.call("dm_midas_stem_im2col_f32_crops" + self._cv, planar, hi, wi, r, B, nh, nw, *self._consts(), cols)
-            d = self._network(B, nh, nw, cols)
-            for i, k in enumerate(ks):
-                w, h = int(rects[k][2]), int(rects[k][3])
-                o = torch.empty(h, w, dtype=torch.float32, device=self.device)
-                self.ops.call("dm_boost_resize_cubic", d[i], nw, 0, nh, nw, o, w, 0, h, w, 1)
-                out[k] = o
-        return out
+    def _crops_network(self, planar, hi, wi, r, B, nh, nw):
+        self._trim_pools()          # each crop group is a forward of its own
+        cols = self._stem_cols(B, nh, nw)
+        self.ops.call("dm_midas_stem_im2col_f32_crops" + self._cv, planar, hi, wi, r, B, nh, nw, *self._boost_consts(), cols)
+        return self._network(B, nh, nw, cols)
 
     def _network_eager(self, B, net_h, net_w, cols):
         """stem GEMM .. head: the depth at the net size, fp32 [B, net_h, net_w] (a pooled buffer)"""
@@ -1079,29 +1068,19 @@ class MidasV21Engine(_ResNeXtEngine):
         # channels at the net size, or its first: 256 at half of it)
         halo = self._buf('halo', (B * max((net_h + 2) * (net_w + 2) * 128, (net_h // 2 + 2) * (net_w // 2 + 2) * F),)) if self.circular else None
         feats = self._encoder(B, net_h, net_w, cols, halo)
-
-        def conv(name, xin, hh, ww, ci, wb, co, act=_lib.ACT_NONE, R=None, R2=None, C2=False):
-            outp = self._buf(name, (B, hh, ww, co))
-            out2 = self._buf(name + '_r', (B, hh, ww, co)) if C2 else None
-            ops.conv3x3(xin, B, hh, ww, ci, wb[0], co, act=act, bias=wb[1], C=outp, C2=out2, R=R, R2=R2, halo=halo)
-            return out2 if C2 else outp
-
-        def up2(name, xin, hh, ww):
-            outp = self._buf(name, (B, 2 * hh, 2 * ww, F))
-            ops.call("dm_resize_bilinear_nhwc_f16", xin, B, hh, ww, F, outp, 2 * hh, 2 * ww)
-            return outp
+        conv, up2 = functools.partial(self._conv, B, halo), functools.partial(self._up2, B)
 
         # layer{i}_rn, followed by the in-place ReLU of the first RCU that reads it
         lr = [conv(f'rn{i}', x, h, wd, c, w['rn'][i], F, act=_lib.ACT_RELU) for i, (x, h, wd, c) in enumerate(feats)]
         _, h, wd, _ = feats[3]
         t = conv('rf4_t', lr[3], h, wd, F, w['rf4_u2c1'], F, act=_lib.ACT_RELU)
-        path = up2('rf4_up', conv('rf4_o', t, h, wd, F, w['rf4_u2c2'], F, R=lr[3]), h, wd)
+        path = up2('rf4_up', conv('rf4_o', t, h, wd, F, w['rf4_u2c2'], F, R=lr[3]), h, wd, F)
         for i in (3, 2, 1):                                   # refinenet{i} reads layer{i}_rn = lr[i - 1]
             _, h, wd, _ = feats[i - 1]
             t = conv(f'rf{i}_t1', lr[i - 1], h, wd, F, w[f'rf{i}_u1c1'], F, act=_lib.ACT_RELU)
             s = conv(f'rf{i}_s', t, h, wd, F, w[f'rf{i}_u1c2'], F, R=lr[i - 1], R2=path, C2=True)     # relu(path + RCU1(l))
             t = conv(f'rf{i}_t2', s, h, wd, F, w[f'rf{i}_u2c1'], F, act=_lib.ACT_RELU)
-            path = up2(f'rf{i}_up', conv(f'rf{i}_o', t, h, wd, F, w[f'rf{i}_u2c2'], F, R=s), h, wd)
+            path = up2(f'rf{i}_up', conv(f'rf{i}_o', t, h, wd, F, w[f'rf{i}_u2c2'], F, R=s), h, wd, F)
         h, wd = 2 * h, 2 * wd
         a = conv('oc0', path, h, wd, F, w['oc0'], 128)
         au = self._buf('oc0_up', (B, net_h, net_w, 128))
@@ -1116,28 +1095,9 @@ class MidasV21Engine(_ResNeXtEngine):
 ZOE_CONFIG = dict(n_bins=64, emb=128, min_temp=0.0212, max_temp=50.0, router_dim=128, router_heads=4, router_layers=4)
 
 
-def _zoe_w(sd, dev, key, rows=None):
-    """1x1 conv / linear weight -> fp16 [rows, cin] (zero padded rows)"""
-    import torch
-    t = sd[key + '.weight'].detach().to(dev).float()
-    t = t.reshape(t.shape[0], -1)
-    o = torch.zeros(rows or t.shape[0], t.shape[1], dtype=torch.float16, device=dev)
-    o[:t.shape[0]] = t.to(torch.float16)
-    return o
-
-
-def _zoe_b(sd, dev, key, n=None):
-    """bias -> fp32 [n] (zero padded)"""
-    import torch
-    t = sd[key + '.bias'].detach().to(dev).float().reshape(-1)
-    o = torch.zeros(n or t.numel(), dtype=torch.float32, device=dev)
-    o[:t.numel()] = t
-    return o
-
-
 def _zoe_lin(sd, dev, key, rows=None):
-    """(weight, bias) of one 1x1 conv / linear layer, output rows zero padded to `rows`"""
-    return _zoe_w(sd, dev, key, rows), _zoe_b(sd, dev, key, rows)
+    """(weight, bias) of one 1x1 conv / linear layer: fp16 [rows, cin], fp32 [rows], output rows zero padded to `rows`"""
+    return _mat(sd[key + '.weight'].detach().to(dev), rows), _vec(sd[key + '.bias'].detach().to(dev), rows)
 
 
 def _zoe_mlp(sd, dev, key):
@@ -1159,21 +1119,15 @@ class _ZoeDepthBase(DptBeitEngine):
         core_sd = {k[len("core.core."):]: v for k, v in state_dict.items() if k.startswith("core.core.")}
         super().__init__(core_sd, core_name, device, circular)
         self._pack_head({k: v for k, v in state_dict.items() if not k.startswith("core.")})
-        # output_conv.2, whose 32-channel ReLU output MidasCore hooks, stored as its own activation
-        self.z['oc2_w'] = _conv_w(self._oc2_weight.to(device), self.F2p, 32)
-        self.z['oc2_b'] = self._oc2_bias.to(device).float().contiguous()
-        self._zbuf_key, self._zbufs = None, {}
 
-    def _pack(self, sd):
-        self._oc2_weight = sd['scratch.output_conv.2.weight'].detach()
-        self._oc2_bias = sd['scratch.output_conv.2.bias'].detach()
-        super()._pack(sd)
+    @property
+    def _zbufs(self):
+        """the head's buffers at the current shape (ZoeDepth tests and tools read them)"""
+        return self._bufs['z']
 
-    def _zbuffers(self, F, nh, nw, b):
+    def _head_buffers(self, b, F, nh, nw):
+        """the head's buffers, b['z']"""
         import torch
-        key = (F, nh, nw)
-        if self._zbuf_key == key:
-            return self._zbufs
         dev = self.device
         h16 = lambda *s: torch.empty(*s, dtype=torch.float16, device=dev)
         f32 = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
@@ -1191,8 +1145,7 @@ class _ZoeDepthBase(DptBeitEngine):
         zb['o32'] = h16(F, nh, nw, 32)
         zb['d'] = f32(F, nh, nw)
         zb.update(self._seed_buffers(F, n0, h16, f32))
-        self._zbufs, self._zbuf_key = zb, key
-        return zb
+        b['z'] = zb
 
     def lin(self, a, lda, wb, M, N, K, out=None, act=_lib.ACT_NONE, f32out=None, resid=None):
         """a [M, K] (row pitch lda) times a (weight, bias) pair -> fp16 `out`, fp32 `f32out`, or added into the fp32 stream `resid`"""
@@ -1217,13 +1170,10 @@ class _ZoeDepthBase(DptBeitEngine):
         b = self._buffers(F, nh, nw)
         ops.call("dm_zoe_preprocess_patchify", rgb, B, H, W, pad_h, pad_w, nh, nw, self.PATCH, b['patches'], self.kpad)
         self.run_network(b, F, nh, nw)
-        zb = self._zbuffers(F, nh, nw, b)
-        Fp = self.Fp
+        zb, Fp = b['z'], self.Fp
         # out_conv activation (MidasCore hooks output_conv[3], the 32-channel ReLU)
-        t = b['up_sizes'][3]
-        ops.conv3x3(b['path'][3], F, t[0], t[1], Fp, self.w['oc1_w'], self.F2p, bias=self.w['oc1_b'], C=b['oc1'], halo=b['halo'])
-        ops.call("dm_resize_bilinear_nhwc_f16", b['oc1'], F, t[0], t[1], self.F2p, b['oc1u'], nh, nw)
-        ops.conv3x3(b['oc1u'], F, nh, nw, self.F2p, z['oc2_w'], 32, act=RELU, bias=z['oc2_b'], C=zb['o32'], halo=b['halo'])
+        self.run_output_conv1(b, F, nh, nw)
+        ops.conv3x3(b['oc1u'], F, nh, nw, self.F2p, self.w['oc2_w'], 32, act=RELU, bias=self.w['oc2_b'], C=zb['o32'], halo=b['halo'])
         n0 = zb['n0']
         # x = conv2(bottleneck); seed bins; seed embedding
         self.lin(b['l'][3], Fp, z['conv2'], F * n0, Fp, Fp, out=zb['x16'])
@@ -1260,14 +1210,15 @@ class ZoeDepthNKEngine(_ZoeDepthBase):
     def _pack_head(self, sd):
         import torch
         dev = self.device
-        W, Bv, lin = (functools.partial(f, sd, dev) for f in (_zoe_w, _zoe_b, _zoe_lin))
+        lin = functools.partial(_zoe_lin, sd, dev)
+        cat = lambda pairs: tuple(torch.cat(t) for t in zip(*pairs))       # layers of both heads stacked
         z = {'conv2': lin('conv2'), 'emb': lin('patch_transformer.embedding_convPxP')}
         layers = []
         for i in range(ZOE_CONFIG['router_layers']):
             q = f'patch_transformer.transformer_encoder.layers.{i}'
-            f32 = lambda k: sd[k].detach().to(dev).float().contiguous()
+            f32 = lambda k: _vec(sd[k].detach().to(dev))
             layers.append(dict(
-                in_w=sd[q + '.self_attn.in_proj_weight'].detach().to(dev, torch.float16).contiguous(), in_b=f32(q + '.self_attn.in_proj_bias'),
+                in_w=_mat(sd[q + '.self_attn.in_proj_weight'].detach().to(dev)), in_b=f32(q + '.self_attn.in_proj_bias'),
                 out=lin(q + '.self_attn.out_proj'), l1=lin(q + '.linear1'), l2=lin(q + '.linear2'),
                 n1=(f32(q + '.norm1.weight'), f32(q + '.norm1.bias')), n2=(f32(q + '.norm2.weight'), f32(q + '.norm2.bias'))))
         z['layers'] = layers
@@ -1277,24 +1228,25 @@ class ZoeDepthNKEngine(_ZoeDepthBase):
         z['zeros128'] = torch.zeros(128, dtype=torch.float32, device=dev)
         names = ('nyu', 'kitti')
         # seed bin regressors of both heads side by side: net.0 stacked, net.2 block-diagonal (nyu -> columns 0..63, kitti 64..127)
-        z['seed0'] = (torch.cat([W(f'seed_bin_regressors.{n}._net.0') for n in names]), torch.cat([Bv(f'seed_bin_regressors.{n}._net.0') for n in names]))
+        z['seed0'] = cat([lin(f'seed_bin_regressors.{n}._net.0') for n in names])
         w2 = torch.zeros(128, 128, dtype=torch.float16, device=dev)
+        b2 = torch.zeros(128, dtype=torch.float32, device=dev)
         for k, n in enumerate(names):
-            w2[64 * k:64 * k + 64, 64 * k:64 * k + 64] = W(f'seed_bin_regressors.{n}._net.2')
-        z['seed2'] = (w2, torch.cat([Bv(f'seed_bin_regressors.{n}._net.2') for n in names]))
+            w2[64 * k:64 * k + 64, 64 * k:64 * k + 64], b2[64 * k:64 * k + 64] = lin(f'seed_bin_regressors.{n}._net.2')
+        z['seed2'] = (w2, b2)
         z['sproj'] = _zoe_mlp(sd, dev, 'seed_projector')
         z['proj'] = [_zoe_mlp(sd, dev, f'projectors.{i}') for i in range(4)]
         att = []
         for i in range(4):
-            a0 = (torch.cat([W(f'attractors.{n}.{i}._net.0') for n in names]), torch.cat([Bv(f'attractors.{n}.{i}._net.0') for n in names]))
+            a0 = cat([lin(f'attractors.{n}.{i}._net.0') for n in names])
             w2 = torch.zeros(64, 256, dtype=torch.float16, device=dev)
             b2 = torch.zeros(64, dtype=torch.float32, device=dev)
             for k, n in enumerate(names):
-                t = W(f'attractors.{n}.{i}._net.2')
+                t, bk = lin(f'attractors.{n}.{i}._net.2')
                 if t.shape[0] != 16:
                     raise NotImplementedError("ZoeDepth-NK attractor layers with other than 16 attractors (the reference always builds 16)")
                 w2[32 * k:32 * k + 16, 128 * k:128 * k + 128] = t
-                b2[32 * k:32 * k + 16] = Bv(f'attractors.{n}.{i}._net.2')
+                b2[32 * k:32 * k + 16] = bk
             att.append((a0, (w2, b2)))
         z['att'] = att
         # conditional log-binomial: mlp.0 split into its out_conv part (32 inputs, evaluated per pixel in clb_final) and its bin
@@ -1390,7 +1342,6 @@ class ZoeDepthEngine(_ZoeDepthBase):
         super().__init__(state_dict, device, core_name, circular)
 
     def _pack_head(self, sd):
-        import torch
         dev = self.device
         lin = functools.partial(_zoe_lin, sd, dev)
         z = {'conv2': lin('conv2'), 'seed': _zoe_mlp(sd, dev, 'seed_bin_regressor'), 'sproj': _zoe_mlp(sd, dev, 'seed_projector'),
@@ -1413,11 +1364,9 @@ class ZoeDepthEngine(_ZoeDepthBase):
         if tuple(m0.shape[:2]) != (80, 161):
             raise ValueError(f"ZoeDepthEngine: conditional_log_binomial.mlp.0 is {tuple(m0.shape)}, expected (80, 161, 1, 1)")
         m0 = m0.reshape(80, 161)
-        we = torch.zeros(128, 128, dtype=torch.float16, device=dev)
-        we[:80] = m0[:, 33:].to(torch.float16)
-        z['clb'] = (we, m0[:, :33].t().contiguous(), _zoe_b(sd, dev, 'conditional_log_binomial.mlp.0'),
+        z['clb'] = (_mat(m0[:, 33:], 128), m0[:, :33].t().contiguous(), _vec(sd['conditional_log_binomial.mlp.0.bias'].detach().to(dev)),
                     sd['conditional_log_binomial.mlp.2.weight'].detach().to(dev).float().reshape(4, 80).contiguous(),
-                    _zoe_b(sd, dev, 'conditional_log_binomial.mlp.2'))
+                    _vec(sd['conditional_log_binomial.mlp.2.bias'].detach().to(dev)))
         self.z = z
 
     def _seed_buffers(self, F, n0, h16, f32):

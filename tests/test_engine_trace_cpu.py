@@ -32,13 +32,18 @@ HOST_ONLY = {"dm_dinov2_pos_embed", "dm_vit_pos_embed", "dm_beit_rel_table", "dm
 
 def kernels(name, args):
     """kernels one call issues (csrc/*.cu): one, except the patchify pre-processing, which first zero-fills the K padding of the
-    patch matrix when kpad exceeds 3 * patch * patch (vit_kernels.cu: patchify_setup)"""
+    patch matrix when kpad exceeds 3 * patch * patch (vit_kernels.cu: patchify_setup), and a circularly padded 3x3 convolution,
+    which first copies its input into the halo buffer"""
     if name in HOST_ONLY:
         return 0
-    if name == "dm_preprocess_patchify":
+    if name in ("dm_preprocess_patchify", "dm_preprocess_patchify_split"):
         return 1 + (args[11] > 3 * args[6] ** 2)
     if name == "dm_preprocess_patchify_f32_crops":
         return 1 + (args[12] > 3 * args[7] ** 2)
+    if name == "dm_conv3x3_circular_ex":
+        return 2
+    if name == "dm_conv3x3_split_ex":
+        return 1 + bool(args[1])
     return 1
 
 
@@ -178,23 +183,34 @@ def _planar(h, w, seed):
     return torch.from_numpy(synth_rgb(h, w, seed).transpose(2, 0, 1).astype(np.float32) / 255.0).contiguous()
 
 
-def test_trace_dav2(fake):
+def _trace_dav2(fake, split=False, circular=False):
     from depthmap_b200.depthmap_generation import DepthAnythingV2Engine
     from oracle import synth_weights
-    eng = DepthAnythingV2Engine(synth_weights.make_dav2_state_dict('vits', seed=0), 'vits', _cpu())
+    eng = DepthAnythingV2Engine(synth_weights.make_dav2_state_dict('vits', seed=0), 'vits', _cpu(), circular=circular, split=split)
     eng.forward_batch(_rgb(2, 60, 80, 1), 70)
-    check_trace("dav2_vits", fake, eng.ops.launches)
+    check_trace("dav2_vits" + "_split" * split + "_circular" * circular, fake, eng.ops.launches)
 
 
-@pytest.mark.parametrize("name", ["beit_tiny", "vit_tiny"])
-def test_trace_dpt(fake, name):
+def test_trace_dav2(fake):
+    _trace_dav2(fake)
+
+
+@pytest.mark.parametrize("split, circular", [(True, False), (False, True), (True, True)])
+def test_trace_dav2_modes(fake, split, circular):
+    """the split (no_half) path and tiling mode"""
+    _trace_dav2(fake, split, circular)
+
+
+@pytest.mark.parametrize("name, circular", [pytest.param(n, c, id=n + "-circular" * c)
+                                            for c in (False, True) for n in ("beit_tiny", "vit_tiny")])
+def test_trace_dpt(fake, name, circular):
     from depthmap_b200.depthmap_generation import DptBeitEngine, DptVitEngine
     from oracle import synth_weights
     cls = DptBeitEngine if name == "beit_tiny" else DptVitEngine
-    eng = cls(synth_weights.make_beit_dpt_state_dict(name, seed=0), name, _cpu())
+    eng = cls(synth_weights.make_beit_dpt_state_dict(name, seed=0), name, _cpu(), circular=circular)
     eng.forward_batch(_rgb(2, 60, 80, 1), 96)
     eng.forward_crops(_planar(100, 120, 2), [(0, 0, 64, 64), (10, 20, 48, 80), (30, 5, 64, 64)], 64)
-    check_trace(f"dpt_{name}", fake, eng.ops.launches)
+    check_trace(f"dpt_{name}" + "_circular" * circular, fake, eng.ops.launches)
 
 
 def _zoe_core(core, seed):
@@ -203,25 +219,33 @@ def _zoe_core(core, seed):
 
 
 def test_trace_zoedepth_nk(fake):
+    _trace_zoedepth_nk(fake)
+
+
+def test_trace_zoedepth_nk_circular(fake):
+    _trace_zoedepth_nk(fake, circular=True)
+
+
+def _trace_zoedepth_nk(fake, circular=False):
     from depthmap_b200.depthmap_generation import ZoeDepthNKEngine
     from oracle import beit_dpt, synth_weights
     sd = _zoe_core('beit_tiny', 0)
     sd.update(synth_weights.make_zoedepth_head_state_dict(feat_ch=beit_dpt.CONFIGS['beit_tiny']['features'], seed=100))
-    eng = ZoeDepthNKEngine(sd, _cpu(), core_name='beit_tiny')
+    eng = ZoeDepthNKEngine(sd, _cpu(), core_name='beit_tiny', circular=circular)
     eng.forward_batch(_rgb(2, 60, 80, 1), 96)
-    check_trace("zoedepth_nk", fake, eng.ops.launches)
+    check_trace("zoedepth_nk" + "_circular" * circular, fake, eng.ops.launches)
 
 
-@pytest.mark.parametrize("variant", ["n", "k"])
-def test_trace_zoedepth_single(fake, variant):
+@pytest.mark.parametrize("variant, circular", [pytest.param(v, c, id=v + "-circular" * c) for c in (False, True) for v in ("n", "k")])
+def test_trace_zoedepth_single(fake, variant, circular):
     from depthmap_b200.depthmap_generation import ZoeDepthEngine
     from oracle import beit_dpt
     from oracle import zoedepth_single as ozs
     sd = _zoe_core('beit_tiny', 0)
     sd.update(ozs.make_zoedepth_single_head_state_dict(variant, feat_ch=beit_dpt.CONFIGS['beit_tiny']['features'], seed=100))
-    eng = ZoeDepthEngine(sd, _cpu(), variant, core_name='beit_tiny')
+    eng = ZoeDepthEngine(sd, _cpu(), variant, core_name='beit_tiny', circular=circular)
     eng.forward_batch(_rgb(2, 60, 80, 1), 96)
-    check_trace(f"zoedepth_{variant}", fake, eng.ops.launches)
+    check_trace(f"zoedepth_{variant}" + "_circular" * circular, fake, eng.ops.launches)
 
 
 @pytest.fixture(scope="module")
@@ -236,13 +260,37 @@ def pix2pix_sd():
     return synth_weights.make_pix2pix_state_dict(seed=0)
 
 
+@pytest.fixture(scope="module")
+def midas_v21_sd():
+    from oracle import midas_v21
+    return midas_v21.make_state_dict(seed=1)
+
+
 def test_trace_leres(fake, leres_sd):
+    _trace_leres(fake, leres_sd)
+
+
+def test_trace_leres_circular(fake, leres_sd):
+    _trace_leres(fake, leres_sd, circular=True)
+
+
+def _trace_leres(fake, leres_sd, circular=False):
     from depthmap_b200.depthmap_generation import LeresEngine
-    eng = LeresEngine(leres_sd, _cpu())
+    eng = LeresEngine(leres_sd, _cpu(), circular=circular)
     eng.forward_batch(_rgb(1, 60, 80, 1), 64)
     eng.forward_batch(_rgb(1, 64, 64, 2), 64)                  # output at net size: a copy, no resize kernel
     eng.forward_crops(_planar(100, 120, 2), [(0, 0, 64, 64), (10, 20, 64, 64)], 64)
-    check_trace("leres", fake, eng.ops.launches)
+    check_trace("leres" + "_circular" * circular, fake, eng.ops.launches)
+
+
+@pytest.mark.parametrize("circular", [False, True])
+def test_trace_midas_v21(fake, midas_v21_sd, circular):
+    from depthmap_b200.depthmap_generation import MidasV21Engine
+    eng = MidasV21Engine(midas_v21_sd, _cpu(), circular=circular)
+    eng.forward_batch(_rgb(2, 100, 150, 1), 384, 384)
+    # 200 x 200 crops at a 384 x 384 net, the 100 x 300 one at 128 x 384: two net shapes
+    eng.forward_crops(_planar(300, 400, 3), [(0, 0, 200, 200), (100, 50, 200, 200), (300, 0, 100, 300)], 384)
+    check_trace("midas_v21" + "_circular" * circular, fake, eng.ops.launches)
 
 
 def test_trace_unet_merge(fake, pix2pix_sd):
@@ -253,13 +301,15 @@ def test_trace_unet_merge(fake, pix2pix_sd):
     check_trace("unet_split", fake, eng.ops.launches)
 
 
-@pytest.mark.parametrize("model_type", [0, 1])
-def test_trace_boost(fake, leres_sd, pix2pix_sd, model_type):
+@pytest.mark.parametrize("model_type", [0, 1, 5])
+def test_trace_boost(fake, leres_sd, pix2pix_sd, midas_v21_sd, model_type):
     from depthmap_b200.boost import BoostPipeline, UnetMergeEngine
-    from depthmap_b200.depthmap_generation import DptBeitEngine, LeresEngine
+    from depthmap_b200.depthmap_generation import DptBeitEngine, LeresEngine, MidasV21Engine
     from oracle import synth_weights
     if model_type == 0:
         depth = LeresEngine(leres_sd, _cpu())
+    elif model_type == 5:
+        depth = MidasV21Engine(midas_v21_sd, _cpu())
     else:
         depth = DptBeitEngine(synth_weights.make_beit_dpt_state_dict('beit_tiny', seed=0), 'beit_tiny', _cpu())
     pipe = BoostPipeline(depth, UnetMergeEngine(pix2pix_sd, _cpu()), _cpu(), model_type)

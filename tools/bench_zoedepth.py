@@ -57,7 +57,7 @@ def head_kernels(eng, model_type):
     from depthmap_b200 import _lib as L
     from depthmap_b200.depthmap_generation import ZOE_CONFIG, ZOE_SINGLE_CONFIG
     lib, zb, st = eng.ops.L, eng._zbufs, L.stream_ptr
-    Fn, nh, nw = eng._zbuf_key
+    Fn, nh, nw = eng._buf_key
     (h2, w2), (h3, w3) = zb['levels'][2], zb['levels'][3]
     bprev, bnew = zb['bnew'][2], zb['bnew'][3]
     if model_type == 9:
