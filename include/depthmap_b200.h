@@ -391,6 +391,10 @@ int dm_leres_stem_im2col_f32_batch(const float *img, int Hi, int Wi, const int *
                                    const float *std, void *out, void *stream);
 int dm_leres_stem_im2col_f32_circular(const float *img, int Hi, int Wi, int x0, int y0, int w, int h, int net_h, int net_w, const float *mean,
                                       const float *std, void *out, void *stream);
+/* singleestimate's ZoeDepth branch (:1062-1064): B crops of the same h x w of the planar image -> uint8 [B,h,w,3] = np.uint8(v * 255) of
+ * the float64 product (truncated toward zero, low 8 bits kept), byte c from plane 2 - c (get_raw_prediction's R/B swap, :381);
+ * rects: DEVICE int32 [B][4] = x0, y0, w, h, inside the image (validated by the caller) */
+int dm_boost_quantise_crops_u8(const float *img /*[3,Hi,Wi]*/, int Hi, int Wi, const int *rects_dev, int B, int h, int w, uint8_t *out, void *stream);
 int dm_leres_stem_im2col_f32_batch_circular(const float *img, int Hi, int Wi, const int *rects_dev, int B, int net_h, int net_w, const float *mean,
                                             const float *std, void *out, void *stream);
 

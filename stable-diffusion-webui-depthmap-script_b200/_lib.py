@@ -73,7 +73,7 @@ EXPORTS = [
     "dm_leres_stem_im2col", "dm_maxpool3x3s2_nhwc_f16", "dm_subsample2_nhwc_f16", "dm_add_f16", "dm_resize_f32_ld",
     "dm_boost_partials", "dm_unet_first_cols", "dm_unet_down_cols", "dm_unet_up_cols", "dm_unet_interleave", "dm_unet_final", "dm_unet_first", "dm_unet_last", "dm_sum_chunks_f32", "dm_boost_minmax",
     "dm_boost_merge_input", "dm_boost_post", "dm_boost_fit_sums", "dm_boost_blend", "dm_boost_resize_cubic", "dm_boost_u8_to_planar",
-    "dm_leres_stem_im2col_f32", "dm_leres_stem_im2col_f32_batch", "dm_boost_minmax_normalise",
+    "dm_leres_stem_im2col_f32", "dm_leres_stem_im2col_f32_batch", "dm_boost_minmax_normalise", "dm_boost_quantise_crops_u8",
     "dm_circular_halo_f16", "dm_conv3x3_circular_ex", "dm_im2col_s2_circular_f16", "dm_leres_stem_im2col_circular",
     "dm_leres_stem_im2col_f32_circular", "dm_leres_stem_im2col_f32_batch_circular",
     "dm_midas_stem_im2col", "dm_midas_stem_im2col_circular", "dm_midas_stem_im2col_f32_crops", "dm_midas_stem_im2col_f32_crops_circular",
@@ -197,6 +197,7 @@ def _bind_optional(L):
         L.dm_boost_blend.argtypes = [vp, i32, vp, vp, i32, vp, i32, i32, i32, i32, i32, vp]
         L.dm_boost_resize_cubic.argtypes = [vp, i32, ll, i32, i32, vp, i32, ll, i32, i32, i32, vp]
         L.dm_boost_u8_to_planar.argtypes = [vp, i32, i32, vp, vp]
+        L.dm_boost_quantise_crops_u8.argtypes = [vp, i32, i32, vp, i32, i32, i32, vp, vp]
         L.dm_leres_stem_im2col_f32.argtypes = [vp, i32, i32, i32, i32, i32, i32, i32, i32, c.POINTER(c.c_float), c.POINTER(c.c_float), vp, vp]
         L.dm_leres_stem_im2col_f32_batch.argtypes = [vp, i32, i32, vp, i32, i32, i32, c.POINTER(c.c_float), c.POINTER(c.c_float), vp, vp]
         L.dm_leres_stem_im2col_f32_circular.argtypes = L.dm_leres_stem_im2col_f32.argtypes

@@ -10,7 +10,9 @@ move: the R_x resolution search and the patch selection look only at the RGB ima
 image) and run through the same cv2 calls.  Every PIXEL of the depth result is produced on the GPU: the float image and its two
 cubic resizes, the base-network forwards on crops (LeReS, model type 0: csrc/boost_kernels.cu leres_stem_im2col_f32; the MiDaS DPT
 models 1-3 and MiDaS v2.1 (5) through estimatemidasBoost, :1180-1220: csrc/vit_kernels.cu preprocess_patchify_f32_crops or
-csrc/midas_kernels.cu midas_stem_im2col_f32_crops, then the per-call min-max normalisation at crop size), the cubic resizes to and from the
+csrc/midas_kernels.cu midas_stem_im2col_f32_crops, then the per-call min-max normalisation at crop size; ZoeDepth-NK (9) through
+estimatezoedepth on np.uint8(crop * 255), :1062-1064: csrc/boost_kernels.cu quantise_crops_u8, then the ZoeDepth forward with its
+pad + flip augmentation, metric depth at crop size), the cubic resizes to and from the
 1024^2 merge resolution, the merge U-Net (split-operand fp32-class GEMMs), min-max normalisations, the degree-1 least-squares fit
 (fp64 sums) and the Gaussian-mask blend; one device->host copy at the end.
 
@@ -322,7 +324,14 @@ class UnetMergeEngine:
 # ---------------------------------------------------------------------------------------------------------------------
 # data plane
 # ---------------------------------------------------------------------------------------------------------------------
-BASE_NETWORKS = (0, 1, 2, 3, 5)   # LeReS res101; DPT-BEiT-L 512, DPT-BEiT-L 384, DPT-Large 384; MiDaS v2.1 (singleestimate, :1053-1066)
+# How singleestimate (:1053-1066) hands each base network's map to doubleestimate:
+#   NET_SIZE    LeReS res101 (0): estimateleres' map, at net size from forward_crops, cubic-resized back to the crop
+#   NORMALISED  DPT-BEiT-L 512 / 384, DPT-Large 384, MiDaS v2.1 (1, 2, 3, 5): estimatemidasBoost's map at crop size, min-max
+#               normalised (a constant map is flagged)
+#   METRIC      ZoeDepth-NK (9): estimatezoedepth's metric depth at crop size, used as is
+NET_SIZE, NORMALISED, METRIC = "net size", "normalised", "metric"
+ESTIMATES = {0: NET_SIZE, 1: NORMALISED, 2: NORMALISED, 3: NORMALISED, 5: NORMALISED, 9: METRIC}
+BASE_NETWORKS = tuple(ESTIMATES)
 
 
 class BoostPipeline:
@@ -331,10 +340,10 @@ class BoostPipeline:
     def __init__(self, depth_engine, merge_engine, device, model_type=0):
         import torch
         if model_type not in BASE_NETWORKS:
-            raise NotImplementedError(f"boost is built for the base networks LeReS res101 (model type 0) and the MiDaS models (1, 2, 3, 5), "
-                                      f"not model type {model_type}")
+            raise NotImplementedError(f"boost is built for the base networks LeReS res101 (model type 0), the MiDaS models (1, 2, 3, 5) "
+                                      f"and ZoeDepth-NK (9), not model type {model_type}")
         self.depth, self.merge, self.device, self.model_type = depth_engine, merge_engine, device, model_type
-        self.midas = model_type != 0      # estimatemidasBoost: crop-size min-max normalisation of every estimate
+        self.estimate = ESTIMATES[model_type]
         self.ops = _lib.Ops()
         self.P = int(self.ops.L.dm_boost_partials())
         self.profile = torch.from_numpy(mask_profile()).to(device)
@@ -381,9 +390,9 @@ class BoostPipeline:
 
     def _estimate_1024(self, planar, rect, msize):
         """singleestimate on a crop (LeReS at msize x msize or the DPT at its upper-bound net size, cubic back to the crop size;
-        min-max normalised for the DPT) followed by the cubic resize to 1024^2"""
+        min-max normalised for the DPT; ZoeDepth's metric map at the crop size as it is) followed by the cubic resize to 1024^2"""
         est = self.depth.forward_batch(None, msize, msize, planar=(planar, rect))[0]
-        if self.midas:
+        if self.estimate == NORMALISED:
             est = self._normalise_estimate(est)
         return self._cubic(est.data_ptr(), rect[2], rect[3], rect[2], PIX2PIX_SIZE, PIX2PIX_SIZE)
 
@@ -409,11 +418,13 @@ class BoostPipeline:
             for k, rect in enumerate(chunk):
                 x, y, w, h = rect
                 ests = []
-                for net, src in ((rf, low[k]), (2 * rf, high[k])):      # cubic back to the crop's size (estimateleres), then to 1024^2 (doubleestimate)
-                    if self.midas:                                     # the DPT engines return the crop-size map; estimatemidasBoost normalises it
+                for net, src in ((rf, low[k]), (2 * rf, high[k])):      # the crop-size map (ESTIMATES), then cubic to 1024^2 (doubleestimate)
+                    if self.estimate == NORMALISED:
                         at_crop = self._normalise_estimate(src)
-                    else:
+                    elif self.estimate == NET_SIZE:
                         at_crop = self._cubic(src.data_ptr(), net, net, net, h, w)
+                    else:
+                        at_crop = src
                     ests.append(self._cubic(at_crop.data_ptr(), w, h, w, PIX2PIX_SIZE, PIX2PIX_SIZE))
                 est = self._post(self._merge(ests[0], ests[1]), True)
                 yield self.fitted_patch(work_img, base, rect, rf, est=est)
@@ -479,6 +490,6 @@ class BoostPipeline:
             for i, rect in enumerate(rects):                                # the blend is order dependent: every rank replays it in order
                 self.blend(updated, all_m[i].view(PIX2PIX_SIZE, PIX2PIX_SIZE), all_s[i], rect)
         out = self._cubic(updated.data_ptr(), ww, wh, ww, H, W)
-        if self.midas and int(self._degenerate.item()):
+        if self.estimate == NORMALISED and int(self._degenerate.item()):
             raise ValueError("boost: the base network returned a constant depth map for a crop (estimatemidasBoost cannot normalise it)")
         return out.cpu().numpy() if to_host else out

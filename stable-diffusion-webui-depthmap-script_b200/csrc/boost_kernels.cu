@@ -15,6 +15,7 @@
 //   leres_stem_im2col_f32: the LeReS stem for a crop of a planar fp32 image (BOOST hands estimateleres float crops)
 //   minmax_normalise     estimatemidasBoost's per-call (x - min) / (max - min) of the crop-size prediction, with a device flag for the
 //                        constant prediction the reference cannot continue from (src/depthmap_generation.py:1212-1220)
+//   quantise_crops_u8    singleestimate's ZoeDepth branch: np.uint8(crop * 255) of B same-shape crops, R and B swapped (:381, :1062-1064)
 #include <cuda_fp16.h>
 #include <math.h>
 
@@ -494,6 +495,26 @@ __global__ void __launch_bounds__(256) leres_stem_im2col_f32_kernel(StemF32Param
     stem_flush_rows_f32(s_rows, p.out, (long long)blockIdx.x * 32, total_pix);
 }
 
+// singleestimate's ZoeDepth branch (src/depthmap_generation.py:1062-1064) hands PIL np.uint8(img * 255) of the float64 crop: the
+// product in double, truncated toward zero, the low 8 bits kept (x86-64: cubic overshoot wraps, 260.1 -> 4, -2.5 -> 254).  img is
+// what get_raw_prediction made of the image (:381), R and B swapped: byte c of a pixel comes from plane 2 - c.  One thread per
+// pixel; consecutive threads read consecutive floats of each plane and write consecutive bytes.
+__global__ void __launch_bounds__(256) boost_quantise_crops_u8_kernel(const float *__restrict__ img, long long plane, int pitch,
+                                                                       const int *__restrict__ rects, int h, int w, long long total,
+                                                                       uint8_t *__restrict__ out) {
+    const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
+    if (i >= total) return;
+    const int x = (int)(i % w);
+    const long long by = i / w;
+    const int y = (int)(by % h), b = (int)(by / h);
+    const float *src = img + (long long)(rects[4 * b + 1] + y) * pitch + rects[4 * b] + x;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        const double v = (double)__ldg(src + (2 - c) * plane) * 255.0;
+        out[3 * i + c] = (uint8_t)(unsigned)__double2int_rz(v);
+    }
+}
+
 }  // namespace dm
 
 #define DM_EXPORT extern "C" __attribute__((visibility("default")))
@@ -630,6 +651,18 @@ DM_EXPORT int dm_boost_u8_to_planar(const uint8_t *rgb, int H, int W, float *out
     if (!rgb || !out) { set_error("dm_boost_u8_to_planar: null argument"); return DM_E_INVALID; }
     boost_u8_to_planar_kernel<<<GRID((long long)H * W), 256, 0, (cudaStream_t)stream_>>>(rgb, (long long)H * W, out);
     DM_LAUNCH_CHECK("boost_u8_to_planar_kernel");
+    return DM_OK;
+}
+
+DM_EXPORT int dm_boost_quantise_crops_u8(const float *img, int Hi, int Wi, const int *rects_dev, int B, int h, int w, uint8_t *out, void *stream_) {
+    using namespace dm;
+    if (!img || !rects_dev || !out || B <= 0 || h <= 0 || w <= 0 || h > Hi || w > Wi) {
+        set_error("dm_boost_quantise_crops_u8: bad arguments");
+        return DM_E_INVALID;
+    }
+    const long long total = (long long)B * h * w;
+    boost_quantise_crops_u8_kernel<<<GRID(total), 256, 0, (cudaStream_t)stream_>>>(img, (long long)Hi * Wi, Wi, rects_dev, h, w, total, out);
+    DM_LAUNCH_CHECK("boost_quantise_crops_u8_kernel");
     return DM_OK;
 }
 

@@ -492,13 +492,18 @@ def _check_rects(rects, hi, wi):
             raise ValueError(f"crop {(x0, y0, w, h)} outside the {wi}x{hi} image")
 
 
+def _check_planar(planar):
+    """BOOST's planar image: a contiguous fp32 [3, Hi, Wi] tensor -> (Hi, Wi)"""
+    import torch
+    if planar.dtype != torch.float32 or planar.dim() != 3 or planar.shape[0] != 3 or not planar.is_contiguous():
+        raise ValueError("planar must be a contiguous float32 tensor [3, H, W]")
+    return int(planar.shape[1]), int(planar.shape[2])
+
+
 def _midas_crop_groups(planar, rects, msize):
     """estimatemidasBoost's crops (x0, y0, w, h) of one planar fp32 image [3, Hi, Wi] -> (Hi, Wi, {(nh, nw): [crop indices]}): each
     crop at its upper-bound net size for msize.  Crops clipped at the image border are not square, hence the grouping."""
-    import torch
-    hi, wi = int(planar.shape[1]), int(planar.shape[2])
-    if planar.dtype != torch.float32 or planar.dim() != 3 or planar.shape[0] != 3 or not planar.is_contiguous():
-        raise ValueError("planar must be a contiguous float32 tensor [3, H, W]")
+    hi, wi = _check_planar(planar)
     _check_rects(rects, hi, wi)
     groups = {}
     for k, (x0, y0, w, h) in enumerate(rects):
@@ -1095,6 +1100,15 @@ class MidasV21Engine(_MidasBoost, _ResNeXtEngine):
 ZOE_CONFIG = dict(n_bins=64, emb=128, min_temp=0.0212, max_temp=50.0, router_dim=128, router_heads=4, router_layers=4)
 
 
+def _nbytes(obj):
+    """device bytes of the tensors in a (nested) buffer dict"""
+    if isinstance(obj, dict):
+        return sum(_nbytes(v) for v in obj.values())
+    if isinstance(obj, (list, tuple)):
+        return sum(_nbytes(v) for v in obj)
+    return obj.numel() * obj.element_size() if hasattr(obj, "element_size") else 0
+
+
 def _zoe_lin(sd, dev, key, rows=None):
     """(weight, bias) of one 1x1 conv / linear layer: fp16 [rows, cin], fp32 [rows], output rows zero padded to `rows`"""
     return _mat(sd[key + '.weight'].detach().to(dev), rows), _vec(sd[key + '.bias'].detach().to(dev), rows)
@@ -1117,8 +1131,29 @@ class _ZoeDepthBase(DptBeitEngine):
 
     def __init__(self, state_dict, device, core_name='beitl16_384', circular=False):
         core_sd = {k[len("core.core."):]: v for k, v in state_dict.items() if k.startswith("core.core.")}
+        self._sets, self._set_bytes, self._set_limit = {}, {}, None
         super().__init__(core_sd, core_name, device, circular)
         self._pack_head({k: v for k, v in state_dict.items() if not k.startswith("core.")})
+
+    def _buffers(self, B, nh, nw):
+        """One buffer set per forward shape, least recently used dropped first once the sets pass half of the device memory.
+        BOOST alternates its crops between two net sizes (and the whole image between two others), so a single set would be
+        rebuilt on every call.  The forward is eager (no CUDA graph reads a dropped set)."""
+        import torch
+        key = (B, nh, nw)
+        b = self._sets.pop(key, None)
+        if b is None:
+            if self._set_limit is None:
+                self._set_limit = torch.cuda.get_device_properties(self.device).total_memory // 2
+            while self._sets and sum(self._set_bytes.values()) > self._set_limit:
+                oldest = next(iter(self._sets))
+                del self._sets[oldest], self._set_bytes[oldest]
+            self._buf_key = None
+            b = super()._buffers(B, nh, nw)
+            self._set_bytes[key] = _nbytes(b)
+        self._sets[key] = b                         # most recently used last
+        self._bufs, self._buf_key = b, key
+        return b
 
     @property
     def _zbufs(self):
@@ -1157,9 +1192,13 @@ class _ZoeDepthBase(DptBeitEngine):
         else:
             self.ops.gemm(a, lda, wt, K, M, N, K, act=act, bias=bias, C=out, ldc=N)
 
-    def forward_batch(self, rgb, net_w, net_h=None, out_hw=None):
-        """rgb: uint8 CUDA [B,H,W,3] -> float32 CUDA [B,H,W] metric depth (what estimatezoedepth returns; invert = True)."""
+    def forward_batch(self, rgb, net_w, net_h=None, out_hw=None, planar=None):
+        """rgb: uint8 CUDA [B,H,W,3] -> float32 CUDA [B,H,W] metric depth (what estimatezoedepth returns; invert = True).
+        planar = (fp32 CUDA [3,Hi,Wi] image, (x0, y0, w, h)) instead of `rgb`: BOOST's estimate of one crop at msize = net_w,
+        [1, h, w] (forward_crops)."""
         import torch
+        if planar is not None:
+            return self.forward_crops(planar[0], [planar[1]], net_w)[0].unsqueeze(0)
         ops, z, P, RELU = self.ops, self.z, self.PROJ, _lib.ACT_RELU
         B, H, W, _ = rgb.shape
         net_h = net_h if net_h is not None else net_w
@@ -1196,6 +1235,28 @@ class _ZoeDepthBase(DptBeitEngine):
         self.log_binomial(zb, bprev, F, nh, nw, hp, wp)
         out = torch.empty(B, H, W, dtype=torch.float32, device=self.device)
         ops.call("dm_zoe_tta_combine", zb['d'], B, nh, nw, pad_h, pad_w, H, W, out)
+        return out
+
+    def forward_crops(self, planar, rects, msize):
+        """BOOST's estimates: singleestimate's ZoeDepth branch (src/depthmap_generation.py:1062-1064, estimatezoedepth :443-452) on
+        crops (x0, y0, w, h) of one planar fp32 image [3, Hi, Wi] -> [fp32 CUDA [h, w]] metric depth at each crop's size (no
+        normalisation), in the order of `rects`.  Each crop is quantised as PIL receives it (np.uint8(crop * 255) of the R/B-swapped
+        image, dm_boost_quantise_crops_u8), then runs infer_pil at msize x msize: the forward above.  Its reflect pad and keep-aspect
+        net size depend on the crop's shape, so the crops are grouped by exact (h, w), one batched forward per shape."""
+        import torch
+        hi, wi = _check_planar(planar)
+        _check_rects(rects, hi, wi)
+        groups = {}
+        for k, (_, _, w, h) in enumerate(rects):
+            groups.setdefault((int(h), int(w)), []).append(k)
+        out = [None] * len(rects)
+        for (h, w), ks in groups.items():
+            r = torch.tensor([[int(v) for v in rects[k]] for k in ks], dtype=torch.int32).to(self.device)
+            u8 = torch.empty(len(ks), h, w, 3, dtype=torch.uint8, device=self.device)
+            self.ops.call("dm_boost_quantise_crops_u8", planar, hi, wi, r, len(ks), h, w, u8)
+            d = self.forward_batch(u8, msize, msize)
+            for i, k in enumerate(ks):
+                out[k] = d[i]
         return out
 
 
@@ -1493,7 +1554,8 @@ class ModelHolder:
         from .boost import BASE_NETWORKS
         if boost and model_type not in BASE_NETWORKS:
             raise NotImplementedError(f"BOOST is implemented in depthmap_b200 for the base networks LeReS res101 (model type 0), "
-                                      f"DPT-BEiT-L 512 / 384 (1, 2), DPT-Large 384 (3) and MiDaS v2.1 (5), not for model type {model_type}")
+                                      f"DPT-BEiT-L 512 / 384 (1, 2), DPT-Large 384 (3), MiDaS v2.1 (5) and ZoeDepth-NK (9), not for "
+                                      f"model type {model_type}")
         # `no_half` is read here, at load time; like the reference, ensure_models does not reload when only the setting changes
         route = no_half_route(model_type, boost, self.precision) if self.no_half else "unchanged"
         if model_type not in CHECKPOINTS:

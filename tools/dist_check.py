@@ -3,7 +3,7 @@ Every rank builds the same model (seeded synthetic weights), takes its contiguou
 depth -> u16 -> stereo -> normal map, all-gathers the finished tensors over NCCL and compares with the whole batch computed
 locally.   python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 tools/dist_check.py [--boost-model-type T]
 --boost-model-type: the BOOST base network, 0 = LeReS res101 (default), 1 = DPT-BEiT-L 512, 2 = DPT-BEiT-L 384, 3 = DPT-Large 384,
-5 = MiDaS v2.1."""
+5 = MiDaS v2.1, 9 = ZoeDepth-NK (on the small 'beit_tiny' core)."""
 import os
 import sys
 
@@ -49,13 +49,16 @@ def main():
     boost_note = ""
     if os.environ.get("DIST_CHECK_BOOST", "1") != "0":
         from depthmap_b200.boost import BoostPipeline, UnetMergeEngine
-        from depthmap_b200.depthmap_generation import DptBeitEngine, DptVitEngine, LeresEngine, MidasV21Engine
+        from depthmap_b200.depthmap_generation import DptBeitEngine, DptVitEngine, LeresEngine, MidasV21Engine, ZoeDepthNKEngine
         from oracle import midas_v21
         t = int(sys.argv[sys.argv.index("--boost-model-type") + 1]) if "--boost-model-type" in sys.argv else 0
         if t == 0:
             base = LeresEngine(synth_weights.make_leres_state_dict(seed=2), dev)
         elif t == 5:
             base = MidasV21Engine(midas_v21.make_state_dict(seed=1), dev)
+        elif t == 9:
+            from test_zoe_gpu import make_zoe_state_dict
+            base = ZoeDepthNKEngine(make_zoe_state_dict('beit_tiny', 1), dev, core_name='beit_tiny')
         else:
             name = {1: 'beitl16_512', 2: 'beitl16_384', 3: 'vitl16_384'}[t]
             base = (DptVitEngine if t == 3 else DptBeitEngine)(synth_weights.make_beit_dpt_state_dict(name, seed=3), name, dev)
