@@ -398,6 +398,47 @@ int dm_boost_quantise_crops_u8(const float *img /*[3,Hi,Wi]*/, int Hi, int Wi, c
 int dm_leres_stem_im2col_f32_batch_circular(const float *img, int Hi, int Wi, const int *rects_dev, int B, int net_h, int net_w, const float *mean,
                                             const float *std, void *out, void *stream);
 
+/* ---------------------------------------------------------------------------------------------------------------
+ * Ragged batches: B images of different pixel sizes that share one network input size run as one forward.  Only the pre- and
+ * post-processing see the image sizes; each ragged entry point computes for image i exactly what its uniform twin computes
+ * for that image alone (B = 1).
+ * An image list is a packed buffer plus one descriptor per image: image i is h x w pixels stored from `offset` on (bytes of a
+ * uint8 HWC [h, w, 3] input, floats of an fp32 [h, w] output).  Every entry point takes the descriptors twice: desc_host (HOST,
+ * validated before any launch: offsets and sizes inside the buffer of `size` bytes / floats, h, w > 0; DM_E_INVALID otherwise)
+ * and desc_dev (DEVICE, the same B records, 16-byte aligned), which the kernels read.
+ * ------------------------------------------------------------------------------------------------------------- */
+typedef struct dm_ragged_image {
+    int64_t offset;
+    int32_t h, w;
+} dm_ragged_image;
+
+/* dm_preprocess_patchify (split = 0) or dm_preprocess_patchify_split (split = 1) per image */
+int dm_preprocess_patchify_ragged(const uint8_t *packed, long long size, const dm_ragged_image *desc_host, const dm_ragged_image *desc_dev,
+                                  int B, int net_h, int net_w, int patch, const float *mean_host, const float *std_host,
+                                  const int *chan_map_host, int split, void *out, int kpad, void *stream);
+/* dm_leres_stem_im2col / dm_midas_stem_im2col and their circular forms per image */
+int dm_leres_stem_im2col_ragged(const uint8_t *packed, long long size, const dm_ragged_image *desc_host, const dm_ragged_image *desc_dev,
+                                int B, int net_h, int net_w, const float *mean_host, const float *std_host, void *out, void *stream);
+int dm_leres_stem_im2col_ragged_circular(const uint8_t *packed, long long size, const dm_ragged_image *desc_host,
+                                         const dm_ragged_image *desc_dev, int B, int net_h, int net_w, const float *mean_host,
+                                         const float *std_host, void *out, void *stream);
+int dm_midas_stem_im2col_ragged(const uint8_t *packed, long long size, const dm_ragged_image *desc_host, const dm_ragged_image *desc_dev,
+                                int B, int net_h, int net_w, const float *mean_host, const float *std_host, const int *chan_map_host,
+                                void *out, void *stream);
+int dm_midas_stem_im2col_ragged_circular(const uint8_t *packed, long long size, const dm_ragged_image *desc_host,
+                                         const dm_ragged_image *desc_dev, int B, int net_h, int net_w, const float *mean_host,
+                                         const float *std_host, const int *chan_map_host, void *out, void *stream);
+/* dm_zoe_preprocess_patchify per image, with image i's reflect pad int(sqrt(h / 2) * 3) x int(sqrt(w / 2) * 3) (float64, as
+ * DepthModel.infer_pil computes it); forwards 2i / 2i+1 are image i and its flip */
+int dm_zoe_preprocess_patchify_ragged(const uint8_t *packed, long long size, const dm_ragged_image *desc_host, const dm_ragged_image *desc_dev,
+                                      int B, int net_h, int net_w, int patch, void *out, int kpad, void *stream);
+/* dm_resize_f32 of in fp32 [B, Hin, Win] to image i's own h x w, written into the packed fp32 output `out` of `size` floats */
+int dm_resize_f32_ragged(const float *in, int B, int Hin, int Win, float *out, long long size, const dm_ragged_image *desc_host,
+                         const dm_ragged_image *desc_dev, int mode, void *stream);
+/* dm_zoe_tta_combine of d fp32 [2B, nh, nw] per image, with image i's pad (as above), into the packed fp32 output `out` */
+int dm_zoe_tta_combine_ragged(const float *d, int B, int nh, int nw, float *out, long long size, const dm_ragged_image *desc_host,
+                              const dm_ragged_image *desc_dev, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -6,6 +6,8 @@ import os
 import sys
 import threading
 
+import numpy as np
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("DEPTHMAP_B200_LIB", os.path.join(_HERE, "_native", "libdepthmap_b200.so"))
 
@@ -80,6 +82,8 @@ EXPORTS = [
     "dm_resize_bilinear_half_nhwc_f16",
     "dm_gemm_split_ex", "dm_conv3x3_split_ex", "dm_attention_split", "dm_preprocess_patchify_split", "dm_assemble_tokens_f32",
     "dm_layernorm_split", "dm_resize_bilinear_nhwc_split",
+    "dm_preprocess_patchify_ragged", "dm_leres_stem_im2col_ragged", "dm_leres_stem_im2col_ragged_circular", "dm_midas_stem_im2col_ragged",
+    "dm_midas_stem_im2col_ragged_circular", "dm_zoe_preprocess_patchify_ragged", "dm_resize_f32_ragged", "dm_zoe_tta_combine_ragged",
 ]
 
 
@@ -215,6 +219,54 @@ def _bind_optional(L):
         L.dm_zoe_seed_bins.argtypes = [vp, i32, c.c_longlong, i32, f32, f32, vp, vp]
         L.dm_zoe_attractor_single.argtypes = [vp, i32, i32, i32, vp, i32, i32, i32, i32, i32, i32, f32, f32, vp, vp]
         L.dm_zoe_clb_single.argtypes = [vp, i32, vp, i32, vp, vp, vp, vp, vp, vp, f32, i32, i32, i32, i32, i32, f32, f32, vp, vp]
+    if hasattr(L, "dm_resize_f32_ragged"):
+        _bind_ragged(L)
+
+
+def _bind_ragged(L):
+    """the ragged-batch twins (include/depthmap_b200.h): packed buffer, its size, host and device descriptors, then the twin's own
+    arguments"""
+    c = ctypes
+    vp, i32, ll, fp, ip = c.c_void_p, c.c_int, c.c_longlong, c.POINTER(c.c_float), c.POINTER(c.c_int)
+    rag = [vp, ll, vp, vp, i32]
+    L.dm_preprocess_patchify_ragged.argtypes = rag + [i32, i32, i32, fp, fp, ip, i32, vp, i32, vp]
+    L.dm_leres_stem_im2col_ragged.argtypes = rag + [i32, i32, fp, fp, vp, vp]
+    L.dm_leres_stem_im2col_ragged_circular.argtypes = L.dm_leres_stem_im2col_ragged.argtypes
+    L.dm_midas_stem_im2col_ragged.argtypes = rag + [i32, i32, fp, fp, ip, vp, vp]
+    L.dm_midas_stem_im2col_ragged_circular.argtypes = L.dm_midas_stem_im2col_ragged.argtypes
+    L.dm_zoe_preprocess_patchify_ragged.argtypes = rag + [i32, i32, i32, vp, i32, vp]
+    L.dm_resize_f32_ragged.argtypes = [vp, i32, i32, i32, vp, ll, vp, vp, i32, vp]
+    L.dm_zoe_tta_combine_ragged.argtypes = [vp, i32, i32, i32, vp, ll, vp, vp, vp]
+
+
+class Ragged:
+    """A ragged image list for the *_ragged entry points: `sizes` [(h, w)] packed back to back from offset 0, `unit` elements per
+    pixel (3 for uint8 RGB, 1 for an fp32 map).  `host` is the dm_ragged_image array (int64 offset, int32 h, int32 w per image),
+    `dev` its copy on `device` (None without a device: a layout only); `size` the packed element count."""
+
+    def __init__(self, sizes, unit, device):
+        import torch
+        self.sizes = [(int(h), int(w)) for h, w in sizes]
+        self.B, self.unit = len(self.sizes), unit
+        rec = np.zeros(self.B, dtype=[("offset", "<i8"), ("h", "<i4"), ("w", "<i4")])
+        off = 0
+        self.offsets = []
+        for i, (h, w) in enumerate(self.sizes):
+            rec[i] = (off, h, w)
+            self.offsets.append(off)
+            off += h * w * unit
+        self.size = off
+        self.host = rec
+        self.dev = torch.from_numpy(rec.view(np.uint8).copy()).to(device) if device is not None else None
+
+    def args(self, packed):
+        """(packed buffer, size, host descriptors, device descriptors, B): the leading arguments of every ragged entry point"""
+        return packed, self.size, self.host.ctypes.data, self.dev, self.B
+
+    def split(self, packed):
+        """views of the B images of a packed tensor of this layout: [h, w] (unit 1) or [h, w, 3] (unit 3)"""
+        shape = () if self.unit == 1 else (self.unit,)
+        return [packed[o:o + h * w * self.unit].view(h, w, *shape) for o, (h, w) in zip(self.offsets, self.sizes)]
 
 
 def check(rc: int, what: str = ""):

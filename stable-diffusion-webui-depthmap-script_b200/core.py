@@ -241,24 +241,66 @@ def max_batch_for(width, height):
     return int(max(1, min(64, (1 << 24) // max(1, int(width) * int(height)))))
 
 
+def _net_request(inp, w, h):
+    """the (net_width, net_height) the funnel asks the model for on a w x h image"""
+    if inp[go.NET_SIZE_MATCH]:
+        return (w + 31) // 32 * 32, (h + 31) // 32 * 32
+    return inp[go.NET_WIDTH], inp[go.NET_HEIGHT]
+
+
+def _group_key(holder, inp, image, custom, boost):
+    """Images with the same key form one device batch.  A depth-model image is keyed by its network input size (and the net size
+    asked for), so images of different pixel sizes that share it run as one ragged forward; custom depth maps and BOOST (per image
+    by design) keep the pixel size."""
+    if custom or boost:
+        return ("pixels", image.width, image.height, custom)
+    req = _net_request(inp, image.width, image.height)
+    return ("net", req, holder.net_size(image.width, image.height, *req))
+
+
 def _process_chunk(holder, inp, dev, images, depthmaps, idxs):
-    """One batch of equally sized images through every requested stage on the device; returns per-image host results."""
+    """One batch of images with one group key through every requested stage on the device; returns per-image host results.  A
+    batch of one pixel size runs as one uniform batch; a mixed one predicts as one ragged batch, then runs the later stages per
+    run of equally sized images."""
+    import torch
+    rgbs = [np.asarray(images[i].convert('RGB') if images[i].mode != 'RGB' else images[i]) for i in idxs]
+    if len({r.shape for r in rgbs}) == 1:
+        return _process_run(holder, inp, dev, images, depthmaps, idxs, rgbs, None)
+    # one host -> device copy: the packed images
+    layout = _lib.Ragged([r.shape[:2] for r in rgbs], 3, None)
+    packed = torch.from_numpy(np.concatenate([r.reshape(-1) for r in rgbs])).to(dev, non_blocking=True)
+    imgs = layout.split(packed)
+    w0, h0 = images[idxs[0]].width, images[idxs[0]].height
+    preds, invert = holder.get_raw_prediction_ragged(imgs, *_net_request(inp, w0, h0))
+    out, j = [], 0
+    while j < len(idxs):
+        k = j + 1
+        while k < len(idxs) and rgbs[k].shape == rgbs[j].shape:
+            k += 1
+        out += _process_run(holder, inp, dev, images, depthmaps, idxs[j:k], rgbs[j:k],
+                            (torch.stack(imgs[j:k]), torch.stack(preds[j:k]), invert))
+        j = k
+    return out
+
+
+def _process_run(holder, inp, dev, images, depthmaps, idxs, rgbs, predicted):
+    """Equally sized images through every requested stage; `predicted` = (rgb batch, prediction batch, invert) when the depth model
+    already ran on them."""
     import torch
     custom = depthmaps[idxs[0]] is not None
-    rgbs = [np.asarray(images[i].convert('RGB') if images[i].mode != 'RGB' else images[i]) for i in idxs]
-    rgb_t = torch.from_numpy(np.stack(rgbs)).to(dev, non_blocking=True)
-    w, h = images[idxs[0]].width, images[idxs[0]].height
     preds = flags = None
     invert = False
+    if predicted is not None:
+        rgb_t, preds, invert = predicted
+    else:
+        rgb_t = torch.from_numpy(np.stack(rgbs)).to(dev, non_blocking=True)
+    w, h = images[idxs[0]].width, images[idxs[0]].height
     if custom:
         outs = [_custom_depth_to_unit(depthmaps[i], images[i]) for i in idxs]
         depth_u16 = convert_to_i16_batch(torch.from_numpy(np.stack(outs)).to(dev))
     else:
-        if inp[go.NET_SIZE_MATCH]:
-            net_width, net_height = (w + 31) // 32 * 32, (h + 31) // 32 * 32
-        else:
-            net_width, net_height = inp[go.NET_WIDTH], inp[go.NET_HEIGHT]
-        preds, invert = holder.get_raw_prediction_batch(rgb_t, net_width, net_height)
+        if preds is None:
+            preds, invert = holder.get_raw_prediction_batch(rgb_t, *_net_request(inp, w, h))
         depth_u16, flags = normalize_prediction_batch(
             preds, invert, inp[go.CLIPDEPTH], inp[go.CLIPDEPTH_MODE], inp[go.CLIPDEPTH_FAR],
             inp[go.CLIPDEPTH_NEAR], return_flags=True)
@@ -313,21 +355,26 @@ def core_generation_funnel(outpath, inputimages, inputdepthmaps, inputnames, inp
             if inputimages[i].mode == 'I':
                 inputimages[i] = inputimages[i].convert('RGB')
 
-        # The reference loop is strictly serial (src/core.py:133).  Here consecutive images of equal size (and equal
-        # "has a custom depth map" state) form one batch of at most max_batch_for(w, h) images; batches are processed and
-        # yielded in input order, so results stream out lazily and host / device memory stay bounded for long clips.
+        # The reference loop is strictly serial (src/core.py:133).  Here consecutive images with one group key (_group_key:
+        # the network input size for the depth model, so mixed pixel sizes can share a forward; the pixel size for custom depth
+        # maps and BOOST) form one batch, bounded by max_batch_for of its largest image; batches are processed and yielded in
+        # input order, so results stream out lazily and host / device memory stay bounded for long clips.
         modes = inp[go.STEREO_MODES]
         n = len(inputimages)
+        boost = bool(inp[go.BOOST])
+        key_of = lambda i: _group_key(holder, inp, inputimages[i], inputdepthmaps[i] is not None, boost)
         count = 0
         while count < n:
-            im0 = inputimages[count]
-            key = (im0.width, im0.height, inputdepthmaps[count] is not None)
-            cap = max_batch_for(im0.width, im0.height)
+            key = key_of(count)
             idxs = [count]
-            while (len(idxs) < cap and idxs[-1] + 1 < n and
-                   (inputimages[idxs[-1] + 1].width, inputimages[idxs[-1] + 1].height,
-                    inputdepthmaps[idxs[-1] + 1] is not None) == key):
+            largest = inputimages[count].width * inputimages[count].height
+            while idxs[-1] + 1 < n:
+                nxt = inputimages[idxs[-1] + 1]
+                grown = max(largest, nxt.width * nxt.height)
+                if len(idxs) + 1 > max_batch_for(grown, 1) or key_of(idxs[-1] + 1) != key:
+                    break
                 idxs.append(idxs[-1] + 1)
+                largest = grown
             results = _process_chunk(holder, inp, dev, inputimages, inputdepthmaps, idxs)
             # yield in the reference's order (src/core.py:194-305)
             for i, (rgb, img_output, pred, stereo, normal) in zip(idxs, results):

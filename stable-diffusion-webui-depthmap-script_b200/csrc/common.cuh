@@ -56,6 +56,32 @@ struct PerDeviceAttr {
     }
 };
 
+// Ragged batches (include/depthmap_b200.h): the host descriptors must lie inside a buffer of `size` units, `unit` units per pixel
+// (3 bytes of a uint8 RGB input, 1 float of an fp32 output), and the device copy must be 16-byte aligned (read as one record).
+// Sets the largest h and w.  Runs before any launch.
+static inline int check_ragged(const char *who, const void *buf, long long size, const dm_ragged_image *host, const dm_ragged_image *dev,
+                               int B, int unit, int *max_h, int *max_w) {
+    if (!buf || !host || !dev || B <= 0 || size < 0) { set_error("%s: bad arguments (null buffer or descriptor, or B <= 0)", who); return DM_E_INVALID; }
+    if (reinterpret_cast<uintptr_t>(dev) % 16) { set_error("%s: the device descriptors must be 16-byte aligned", who); return DM_E_INVALID; }
+    int mh = 0, mw = 0;
+    for (int i = 0; i < B; ++i) {
+        const dm_ragged_image d = host[i];
+        if (d.h <= 0 || d.w <= 0 || d.offset < 0 || d.offset > size || (long long)d.h * d.w * unit > size - d.offset) {
+            set_error("%s: image %d (offset %lld, %d x %d) does not lie inside the buffer of %lld", who, i, (long long)d.offset, d.h, d.w, size);
+            return DM_E_INVALID;
+        }
+        mh = d.h > mh ? d.h : mh;
+        mw = d.w > mw ? d.w : mw;
+    }
+    if (max_h) *max_h = mh;
+    if (max_w) *max_w = mw;
+    return DM_OK;
+}
+
+// DepthModel.infer_pil's reflect pad of an n-pixel side, int(sqrt(n / 2) * 3) in float64 (numpy's arithmetic: both roots are
+// correctly rounded)
+__host__ __device__ __forceinline__ int zoe_pad_of(int n) { return (int)(sqrt((double)n / 2.0) * 3.0); }
+
 // i mod n in [0, n) for any integer i (circular padding, n > 0)
 __host__ __device__ __forceinline__ int wrap_index(int i, int n) {
     const int r = i % n;

@@ -21,6 +21,7 @@ struct StemParams {
     int B, H, W, nh, nw, Ho, Wo;
     float mean[3], inv_std[3];
     __half *out;     // [B*Ho*Wo, 192]
+    const dm_ragged_image *ragged;      // ragged batch: image b is ragged[b] of the packed buffer rgb (H, W unused)
 };
 
 // cv2.resize INTER_LINEAR source coordinates of destination index d: sx, sx+1 (clamped) and the weight of sx+1
@@ -75,6 +76,58 @@ __global__ void __launch_bounds__(256) leres_stem_im2col_kernel(StemParams p) {
                     cv_linear_coord(ix, sx, p.W, x0, x1, fx);
                     const uint8_t *p00 = img + ((long long)y0 * p.W + x0) * 3, *p01 = img + ((long long)y0 * p.W + x1) * 3;
                     const uint8_t *p10 = img + ((long long)y1 * p.W + x0) * 3, *p11 = img + ((long long)y1 * p.W + x1) * 3;
+#pragma unroll
+                    for (int c = 0; c < 3; ++c) {
+                        const float a = ((float)p00[c] * (1.f - fx) + (float)p01[c] * fx) / 255.f, d = ((float)p10[c] * (1.f - fx) + (float)p11[c] * fx) / 255.f;
+                        v[c] = a * (1.f - fy) + d * fy;
+                    }
+                }
+                // the network sees RGB in source order (the holder's channel swap is undone by estimateleres, :408); ImageNet statistics
+#pragma unroll
+                for (int c = 0; c < 3; ++c) v[c] = (v[c] - p.mean[c]) * p.inv_std[c];
+            }
+#pragma unroll
+            for (int c = 0; c < 3; ++c) row[(ky * 7 + kx) * 3 + c] = __float2half_rn(v[c]);
+        }
+    }
+    __syncthreads();
+    stem_flush_rows(s_rows, p.out, (long long)blockIdx.x * 32, total_pix);
+}
+
+// ragged twin of leres_stem_im2col_kernel: image b is p.ragged[b] of the packed buffer p.rgb
+template <bool CIRCULAR>
+__global__ void __launch_bounds__(256) leres_stem_im2col_ragged_kernel(StemParams p) {
+    // one thread per (output pixel, ky): 7 kx taps x 3 channels = 21 values; thread ky == 7 zero-fills the 45 padding columns
+    __shared__ __align__(16) __half s_rows[32 * 192];
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const long long total_pix = (long long)p.B * p.Ho * p.Wo;
+    const int ky = (int)(idx & 7);
+    const long long pix = idx >> 3;
+    const bool live = pix < total_pix;
+    __half *row = s_rows + (threadIdx.x >> 3) * 192;
+    if (live && ky == 7) {
+        for (int k = 147; k < 192; ++k) row[k] = __float2half_rn(0.f);
+    } else if (live) {
+        const int ox = (int)(pix % p.Wo), oy = (int)((pix / p.Wo) % p.Ho), b = (int)(pix / ((long long)p.Wo * p.Ho));
+        const dm_ragged_image d = p.ragged[b];
+        const uint8_t *img = p.rgb + d.offset;
+        const int H = d.h, W = d.w;
+        const bool identity = p.nh == H && p.nw == W;           // cv2.resize to the same size is a copy
+        const float sy = (float)H / (float)p.nh, sx = (float)W / (float)p.nw;
+        const int iy = CIRCULAR ? wrap_index(oy * 2 - 3 + ky, p.nh) : oy * 2 - 3 + ky;
+        for (int kx = 0; kx < 7; ++kx) {
+            const int ix = CIRCULAR ? wrap_index(ox * 2 - 3 + kx, p.nw) : ox * 2 - 3 + kx;
+            float v[3] = {0.f, 0.f, 0.f};
+            if (iy >= 0 && iy < p.nh && ix >= 0 && ix < p.nw) {
+                if (identity) {
+                    const uint8_t *px = img + ((long long)iy * W + ix) * 3;
+                    v[0] = (float)px[0] / 255.f; v[1] = (float)px[1] / 255.f; v[2] = (float)px[2] / 255.f;
+                } else {
+                    int y0, y1, x0, x1; float fy, fx;
+                    cv_linear_coord(iy, sy, H, y0, y1, fy);
+                    cv_linear_coord(ix, sx, W, x0, x1, fx);
+                    const uint8_t *p00 = img + ((long long)y0 * W + x0) * 3, *p01 = img + ((long long)y0 * W + x1) * 3;
+                    const uint8_t *p10 = img + ((long long)y1 * W + x0) * 3, *p11 = img + ((long long)y1 * W + x1) * 3;
 #pragma unroll
                     for (int c = 0; c < 3; ++c) {
                         const float a = ((float)p00[c] * (1.f - fx) + (float)p01[c] * fx) / 255.f, d = ((float)p10[c] * (1.f - fx) + (float)p11[c] * fx) / 255.f;
@@ -171,6 +224,38 @@ DM_EXPORT int dm_leres_stem_im2col(const uint8_t *rgb, int B, int H, int W, int 
 DM_EXPORT int dm_leres_stem_im2col_circular(const uint8_t *rgb, int B, int H, int W, int net_h, int net_w, const float *mean_host,
                                             const float *std_host, void *out, void *stream_) {
     return leres_stem_im2col<true>("dm_leres_stem_im2col_circular", rgb, B, H, W, net_h, net_w, mean_host, std_host, out, stream_);
+}
+
+template <bool CIRCULAR>
+static int leres_stem_im2col_ragged(const char *who, const uint8_t *packed, long long size, const dm_ragged_image *desc_host,
+                                    const dm_ragged_image *desc_dev, int B, int net_h, int net_w, const float *mean_host, const float *std_host,
+                                    void *out, void *stream_) {
+    using namespace dm;
+    const int rc = check_ragged(who, packed, size, desc_host, desc_dev, B, 3, nullptr, nullptr);
+    if (rc) return rc;
+    if (!out || !mean_host || !std_host || net_h <= 0 || net_w <= 0) { set_error("%s: bad arguments", who); return DM_E_INVALID; }
+    StemParams p;
+    p.rgb = packed; p.ragged = desc_dev; p.B = B; p.H = 0; p.W = 0; p.nh = net_h; p.nw = net_w;
+    p.Ho = (net_h + 6 - 7) / 2 + 1; p.Wo = (net_w + 6 - 7) / 2 + 1;
+    for (int c = 0; c < 3; ++c) { p.mean[c] = mean_host[c]; p.inv_std[c] = 1.0f / std_host[c]; }
+    p.out = (__half *)out;
+    const long long total = (long long)B * p.Ho * p.Wo * 8;
+    leres_stem_im2col_ragged_kernel<CIRCULAR><<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream_>>>(p);
+    DM_LAUNCH_CHECK("leres_stem_im2col_ragged_kernel");
+    return DM_OK;
+}
+
+DM_EXPORT int dm_leres_stem_im2col_ragged(const uint8_t *packed, long long size, const dm_ragged_image *desc_host, const dm_ragged_image *desc_dev,
+                                          int B, int net_h, int net_w, const float *mean_host, const float *std_host, void *out, void *stream_) {
+    return leres_stem_im2col_ragged<false>("dm_leres_stem_im2col_ragged", packed, size, desc_host, desc_dev, B, net_h, net_w, mean_host, std_host,
+                                           out, stream_);
+}
+
+DM_EXPORT int dm_leres_stem_im2col_ragged_circular(const uint8_t *packed, long long size, const dm_ragged_image *desc_host,
+                                                   const dm_ragged_image *desc_dev, int B, int net_h, int net_w, const float *mean_host,
+                                                   const float *std_host, void *out, void *stream_) {
+    return leres_stem_im2col_ragged<true>("dm_leres_stem_im2col_ragged_circular", packed, size, desc_host, desc_dev, B, net_h, net_w, mean_host,
+                                          std_host, out, stream_);
 }
 
 DM_EXPORT int dm_maxpool3x3s2_nhwc_f16(const void *in, int B, int H, int W, int C, void *out, void *stream_) {

@@ -22,13 +22,14 @@ struct MidasStemParams {
     float value_scale, mean[3], inv_std[3];
     int chan_map[3];        // network channel c reads source channel chan_map[c]
     __half *out;            // [B*Ho*Wo, 192]
+    const dm_ragged_image *ragged;      // RAGGED (uint8 variant): image b is ragged[b] of the packed buffer rgb (H, W unused)
 };
 
 // One thread per (output pixel, ky): 7 kx taps x 3 channels, each tap a 4x4 cubic sample of the source (L1 / L2 hits: a network
 // pixel is read by ~12 taps).  Thread ky == 7 zero-fills the 45 padding columns.  The 32 rows of a block are assembled in shared
 // memory and leave as 16-byte stores, as in leres_stem_im2col.  CIRCULAR: a tap outside the nh x nw network input wraps around
 // (nn.Conv2d(padding_mode='circular')) before the resize maps it to the source.
-template <bool F32, bool CIRCULAR>
+template <bool F32, bool CIRCULAR, bool RAGGED = false>
 __global__ void __launch_bounds__(256) midas_stem_im2col_kernel(MidasStemParams p) {
     __shared__ __align__(16) __half s_rows[32 * 192];
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -46,6 +47,9 @@ __global__ void __launch_bounds__(256) midas_stem_im2col_kernel(MidasStemParams 
         if (F32) {
             const int4 r = __ldg(reinterpret_cast<const int4 *>(p.rects) + b);
             f32 = F32CropSource{p.img + (long long)r.y * p.W + r.x, p.plane, p.W, r.w, r.z};
+        } else if (RAGGED) {
+            const dm_ragged_image d = p.ragged[b];
+            u8 = U8Source{p.rgb + d.offset, d.h, d.w};
         } else {
             u8.img = p.rgb + (long long)b * p.H * p.W * 3;
         }
@@ -112,7 +116,7 @@ __global__ void __launch_bounds__(256) resize_bilinear_half_nhwc_kernel(const __
 
 #define DM_EXPORT extern "C" __attribute__((visibility("default")))
 
-template <bool F32, bool CIRCULAR>
+template <bool F32, bool CIRCULAR, bool RAGGED = false>
 static int midas_stem_im2col(const char *who, dm::MidasStemParams &p, int net_h, int net_w, const float *mean_host, const float *std_host,
                              const int *chan_map_host, void *out, void *stream_) {
     using namespace dm;
@@ -127,7 +131,7 @@ static int midas_stem_im2col(const char *who, dm::MidasStemParams &p, int net_h,
     p.Ho = (net_h + 6 - 7) / 2 + 1; p.Wo = (net_w + 6 - 7) / 2 + 1;
     p.out = (__half *)out;
     const long long total = (long long)p.B * p.Ho * p.Wo * 8;
-    midas_stem_im2col_kernel<F32, CIRCULAR><<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream_>>>(p);
+    midas_stem_im2col_kernel<F32, CIRCULAR, RAGGED><<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream_>>>(p);
     DM_LAUNCH_CHECK("midas_stem_im2col_kernel");
     return DM_OK;
 }
@@ -172,6 +176,32 @@ DM_EXPORT int dm_midas_stem_im2col_f32_crops_circular(const float *img, int Hi, 
                                                       void *stream_) {
     return midas_stem_crops<true>("dm_midas_stem_im2col_f32_crops_circular", img, Hi, Wi, rects_dev, B, net_h, net_w, mean_host, std_host,
                                   chan_map_host, out, stream_);
+}
+
+template <bool CIRCULAR>
+static int midas_stem_ragged(const char *who, const uint8_t *packed, long long size, const dm_ragged_image *desc_host,
+                             const dm_ragged_image *desc_dev, int B, int net_h, int net_w, const float *mean_host, const float *std_host,
+                             const int *chan_map_host, void *out, void *stream_) {
+    int mh = 0, mw = 0;
+    const int rc = dm::check_ragged(who, packed, size, desc_host, desc_dev, B, 3, &mh, &mw);
+    if (rc) return rc;
+    dm::MidasStemParams p{};
+    p.rgb = packed; p.ragged = desc_dev; p.B = B; p.H = mh; p.W = mw; p.value_scale = 1.0f / 255.0f;    // H, W: only checked > 0
+    return midas_stem_im2col<false, CIRCULAR, true>(who, p, net_h, net_w, mean_host, std_host, chan_map_host, out, stream_);
+}
+
+DM_EXPORT int dm_midas_stem_im2col_ragged(const uint8_t *packed, long long size, const dm_ragged_image *desc_host, const dm_ragged_image *desc_dev,
+                                          int B, int net_h, int net_w, const float *mean_host, const float *std_host, const int *chan_map_host,
+                                          void *out, void *stream_) {
+    return midas_stem_ragged<false>("dm_midas_stem_im2col_ragged", packed, size, desc_host, desc_dev, B, net_h, net_w, mean_host, std_host,
+                                    chan_map_host, out, stream_);
+}
+
+DM_EXPORT int dm_midas_stem_im2col_ragged_circular(const uint8_t *packed, long long size, const dm_ragged_image *desc_host,
+                                                   const dm_ragged_image *desc_dev, int B, int net_h, int net_w, const float *mean_host,
+                                                   const float *std_host, const int *chan_map_host, void *out, void *stream_) {
+    return midas_stem_ragged<true>("dm_midas_stem_im2col_ragged_circular", packed, size, desc_host, desc_dev, B, net_h, net_w, mean_host,
+                                   std_host, chan_map_host, out, stream_);
 }
 
 DM_EXPORT int dm_resize_bilinear_half_nhwc_f16(const void *in, int B, int Hin, int Win, int C, void *out, int Hout, int Wout, void *stream_) {

@@ -68,6 +68,22 @@ __global__ void __launch_bounds__(256) preprocess_patchify_kernel(PreParams p) {
     store_patch_pixel<SPLIT>(p, b, y, x, v, 1.0f / 255.0f);
 }
 
+// ragged batch: image b is desc[b] of the packed buffer p.rgb (p.H, p.W unused)
+template <bool SPLIT>
+__global__ void __launch_bounds__(256) preprocess_patchify_ragged_kernel(PreParams p, const dm_ragged_image *__restrict__ desc) {
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const long long total = (long long)p.B * p.nh * p.nw;
+    if (idx >= total) return;
+    const int x = (int)(idx % p.nw);
+    const int y = (int)((idx / p.nw) % p.nh);
+    const int b = (int)(idx / ((long long)p.nw * p.nh));
+    const dm_ragged_image d = desc[b];
+    const U8Source src{p.rgb + d.offset, d.h, d.w};
+    float v[3];
+    cubic_sample(src, p.nh, p.nw, y, x, v);
+    store_patch_pixel<SPLIT>(p, b, y, x, v, 1.0f / 255.0f);
+}
+
 // BOOST crops: p.rgb unused; image b is the crop rects[b] = (x0, y0, w, h) of the planar fp32 image, values used as they are
 __global__ void __launch_bounds__(256) preprocess_patchify_f32_crops_kernel(PreParams p, const float *__restrict__ img, int Hi, int Wi,
                                                                             const int *__restrict__ rects) {
@@ -298,6 +314,48 @@ __global__ void __launch_bounds__(256) resize_f32_kernel(const float *__restrict
     }
 }
 
+// resize_f32_kernel (ld = 1) to a ragged output: image b at its own desc[b] size and place; grid (max h * max w, B)
+__global__ void __launch_bounds__(256) resize_f32_ragged_kernel(const float *__restrict__ in, int Hin, int Win, float *__restrict__ out,
+                                                                const dm_ragged_image *__restrict__ desc, int mode) {
+    const int b = blockIdx.y;
+    const dm_ragged_image d = desc[b];
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= (long long)d.h * d.w) return;
+    const int x = (int)(idx % d.w), y = (int)(idx / d.w);
+    const int Hout = d.h, Wout = d.w;
+    const float *img = in + (long long)b * Hin * Win;
+    float r;
+    if (mode == 0) {
+        const float sy = Hout > 1 ? (float)(Hin - 1) / (float)(Hout - 1) : 0.f;
+        const float sx = Wout > 1 ? (float)(Win - 1) / (float)(Wout - 1) : 0.f;
+        const float fy = sy * (float)y, fx = sx * (float)x;
+        const int y0 = min((int)fy, Hin - 1), x0 = min((int)fx, Win - 1);
+        const int y1 = min(y0 + 1, Hin - 1), x1 = min(x0 + 1, Win - 1);
+        const float ly = fy - (float)y0, lx = fx - (float)x0, hy = 1.f - ly, hx = 1.f - lx;
+        r = hy * (hx * img[(long long)y0 * Win + x0] + lx * img[(long long)y0 * Win + x1]) +
+            ly * (hx * img[(long long)y1 * Win + x0] + lx * img[(long long)y1 * Win + x1]);
+    } else {
+        const float sy = (float)Hin / (float)Hout, sx = (float)Win / (float)Wout;
+        float fy = sy * ((float)y + 0.5f) - 0.5f, fx = sx * ((float)x + 0.5f) - 0.5f;
+        const int iy = (int)floorf(fy), ix = (int)floorf(fx);
+        fy -= (float)iy; fx -= (float)ix;
+        float cx[4], cy[4];
+        cubic_coeffs(fx, cx);
+        cubic_coeffs(fy, cy);
+        float acc = 0.f;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int yy = min(max(iy - 1 + j, 0), Hin - 1);
+            float s = 0.f;
+#pragma unroll
+            for (int i = 0; i < 4; ++i) s += cx[i] * img[(long long)yy * Win + min(max(ix - 1 + i, 0), Win - 1)];
+            acc += cy[j] * s;
+        }
+        r = acc;
+    }
+    out[d.offset + idx] = r;
+}
+
 // im2col for a 3x3 stride-2 pad-1 convolution on NHWC fp16: out [B*Ho*Wo, 9*C] ordered (ky, kx, c).  CIRCULAR: the padding
 // wraps around (nn.Conv2d(padding_mode='circular')) instead of being zeros
 template <bool CIRCULAR>
@@ -387,6 +445,30 @@ DM_EXPORT int dm_preprocess_patchify_split(const uint8_t *rgb, int B, int H, int
     const long long total = (long long)B * net_h * net_w;
     preprocess_patchify_kernel<true><<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(p);
     DM_LAUNCH_CHECK("preprocess_patchify_kernel");
+    return DM_OK;
+}
+
+DM_EXPORT int dm_preprocess_patchify_ragged(const uint8_t *packed, long long size, const dm_ragged_image *desc_host, const dm_ragged_image *desc_dev,
+                                            int B, int net_h, int net_w, int patch, const float *mean_host, const float *std_host,
+                                            const int *chan_map_host, int split, void *out, int kpad, void *stream_) {
+    using namespace dm;
+    const char *who = "dm_preprocess_patchify_ragged";
+    int rc = check_ragged(who, packed, size, desc_host, desc_dev, B, 3, nullptr, nullptr);
+    if (rc) return rc;
+    if (!out || patch <= 0 || net_h <= 0 || net_w <= 0 || net_h % patch || net_w % patch || kpad < 3 * patch * patch || (split != 0 && split != 1)) {
+        set_error("%s: bad arguments", who); return DM_E_INVALID;
+    }
+    cudaStream_t stream = (cudaStream_t)stream_;
+    PreParams p;
+    p.rgb = packed; p.H = 0; p.W = 0;
+    // split: the zero fill treats each row of 3*kpad as three rows of kpad, as dm_preprocess_patchify_split
+    rc = patchify_setup(p, split ? 3 * B : B, net_h, net_w, patch, mean_host, std_host, chan_map_host, out, kpad, stream);
+    if (rc) return rc;
+    p.B = B;
+    const long long total = (long long)B * net_h * net_w;
+    if (split) preprocess_patchify_ragged_kernel<true><<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(p, desc_dev);
+    else preprocess_patchify_ragged_kernel<false><<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(p, desc_dev);
+    DM_LAUNCH_CHECK("preprocess_patchify_ragged_kernel");
     return DM_OK;
 }
 
@@ -492,6 +574,19 @@ DM_EXPORT int dm_resize_f32(const float *in, int B, int Hin, int Win, float *out
     const long long total = (long long)B * Hout * Wout;
     resize_f32_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream_>>>(in, B, Hin, Win, out, Hout, Wout, mode, 1);
     DM_LAUNCH_CHECK("resize_f32_kernel");
+    return DM_OK;
+}
+
+DM_EXPORT int dm_resize_f32_ragged(const float *in, int B, int Hin, int Win, float *out, long long size, const dm_ragged_image *desc_host,
+                                   const dm_ragged_image *desc_dev, int mode, void *stream_) {
+    using namespace dm;
+    int mh = 0, mw = 0;
+    const int rc = check_ragged("dm_resize_f32_ragged", out, size, desc_host, desc_dev, B, 1, &mh, &mw);
+    if (rc) return rc;
+    if (!in || Hin <= 0 || Win <= 0 || (mode != 0 && mode != 1) || B > 65535) { set_error("dm_resize_f32_ragged: bad arguments"); return DM_E_INVALID; }
+    const dim3 grid((unsigned)(((long long)mh * mw + 255) / 256), (unsigned)B);
+    resize_f32_ragged_kernel<<<grid, 256, 0, (cudaStream_t)stream_>>>(in, Hin, Win, out, desc_dev, mode);
+    DM_LAUNCH_CHECK("resize_f32_ragged_kernel");
     return DM_OK;
 }
 

@@ -39,6 +39,7 @@ struct ZoePre {
     const uint8_t *rgb;
     int B, H, W, pad_h, pad_w, nh, nw, patch, gh, gw, kpad;
     __half *out;
+    const dm_ragged_image *ragged;      // ragged batch: image b is ragged[b] of the packed buffer rgb (H, W, pads unused)
 };
 
 __global__ void __launch_bounds__(256) zoe_preprocess_patchify_kernel(ZoePre p) {
@@ -64,6 +65,45 @@ __global__ void __launch_bounds__(256) zoe_preprocess_patchify_kernel(ZoePre p) 
         sy_ = sy_ < 0 ? -sy_ : (sy_ >= p.H ? 2 * (p.H - 1) - sy_ : sy_);
         sx_ = sx_ < 0 ? -sx_ : (sx_ >= p.W ? 2 * (p.W - 1) - sx_ : sx_);
         const uint8_t *px = img + ((long long)sy_ * p.W + sx_) * 3;
+        v[0] = (float)px[0] / 255.0f; v[1] = (float)px[1] / 255.0f; v[2] = (float)px[2] / 255.0f;   // transforms.ToTensor
+    };
+    float v00[3], v01[3], v10[3], v11[3];
+    src(y0, x0, v00); src(y0, x1, v01); src(y1, x0, v10); src(y1, x1, v11);
+    const int py = y / p.patch, ky = y % p.patch, pxi = x / p.patch, kx = x % p.patch;
+    __half *row = p.out + ((long long)(f * p.gh + py) * p.gw + pxi) * p.kpad;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        const float r = hy * (hx * v00[c] + lx * v01[c]) + ly * (hx * v10[c] + lx * v11[c]);
+        row[(c * p.patch + ky) * p.patch + kx] = __float2half_rn((r - 0.5f) / 0.5f);
+    }
+}
+
+// ragged twin of zoe_preprocess_patchify_kernel: image b is p.ragged[b] of the packed buffer p.rgb, padded by zoe_pad_of
+__global__ void __launch_bounds__(256) zoe_preprocess_patchify_ragged_kernel(ZoePre p) {
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const long long total = (long long)2 * p.B * p.nh * p.nw;
+    if (idx >= total) return;
+    const int x = (int)(idx % p.nw);
+    const int y = (int)((idx / p.nw) % p.nh);
+    const int f = (int)(idx / ((long long)p.nw * p.nh));
+    const int b = f >> 1, flip = f & 1;
+    const dm_ragged_image d = p.ragged[b];
+    const uint8_t *img = p.rgb + d.offset;
+    const int H = d.h, W = d.w, pad_h = zoe_pad_of(H), pad_w = zoe_pad_of(W);
+    const int Hp = H + 2 * pad_h, Wp = W + 2 * pad_w;
+    // F.interpolate(bilinear, align_corners=True) over the padded (and flipped) image
+    const float sy = p.nh > 1 ? (float)(Hp - 1) / (float)(p.nh - 1) : 0.f;
+    const float sx = p.nw > 1 ? (float)(Wp - 1) / (float)(p.nw - 1) : 0.f;
+    const float fy = sy * (float)y, fx = sx * (float)x;
+    const int y0 = min((int)fy, Hp - 1), x0 = min((int)fx, Wp - 1);
+    const int y1 = min(y0 + 1, Hp - 1), x1 = min(x0 + 1, Wp - 1);
+    const float ly = fy - (float)y0, lx = fx - (float)x0, hy = 1.f - ly, hx = 1.f - lx;
+    auto src = [&](int yy, int xx, float *v) {
+        if (flip) xx = Wp - 1 - xx;
+        int sy_ = yy - pad_h, sx_ = xx - pad_w;           // F.pad(mode="reflect"): edge not repeated
+        sy_ = sy_ < 0 ? -sy_ : (sy_ >= H ? 2 * (H - 1) - sy_ : sy_);
+        sx_ = sx_ < 0 ? -sx_ : (sx_ >= W ? 2 * (W - 1) - sx_ : sx_);
+        const uint8_t *px = img + ((long long)sy_ * W + sx_) * 3;
         v[0] = (float)px[0] / 255.0f; v[1] = (float)px[1] / 255.0f; v[2] = (float)px[2] / 255.0f;   // transforms.ToTensor
     };
     float v00[3], v01[3], v10[3], v11[3];
@@ -392,14 +432,8 @@ __global__ void __launch_bounds__(128) clb_final_kernel(ClbParams p) {
 
 // out[b, y, x] = 0.5 * (up(d[2b])[y + pad_h, x + pad_w] + up(d[2b+1])[y + pad_h, Wp - 1 - (x + pad_w)]), up = bicubic
 // align_corners=False from (nh, nw) to the padded size (Hp, Wp); identity when the sizes agree (depth_model.py:88-89)
-__global__ void __launch_bounds__(256) tta_combine_kernel(const float *__restrict__ d, int B, int nh, int nw, int Hp, int Wp, int pad_h, int pad_w,
-                                                          int H, int W, float *__restrict__ out) {
-    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const long long total = (long long)B * H * W;
-    if (idx >= total) return;
-    const int x = (int)(idx % W);
-    const int y = (int)((idx / W) % H);
-    const int b = (int)(idx / ((long long)W * H));
+__device__ __forceinline__ float tta_combine_pixel(const float *__restrict__ d, int b, int nh, int nw, int Hp, int Wp, int pad_h, int pad_w,
+                                                   int y, int x) {
     const bool same = (nh == Hp && nw == Wp);
     const float sy = (float)nh / (float)Hp, sx = (float)nw / (float)Wp;
     auto sample = [&](const float *img, int yy, int xx) {
@@ -423,7 +457,29 @@ __global__ void __launch_bounds__(256) tta_combine_kernel(const float *__restric
     };
     const float a = sample(d + (long long)(2 * b) * nh * nw, y + pad_h, x + pad_w);
     const float c = sample(d + (long long)(2 * b + 1) * nh * nw, y + pad_h, Wp - 1 - (x + pad_w));
-    out[idx] = (a + c) / 2.f;
+    return (a + c) / 2.f;
+}
+
+__global__ void __launch_bounds__(256) tta_combine_kernel(const float *__restrict__ d, int B, int nh, int nw, int Hp, int Wp, int pad_h, int pad_w,
+                                                          int H, int W, float *__restrict__ out) {
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const long long total = (long long)B * H * W;
+    if (idx >= total) return;
+    const int x = (int)(idx % W);
+    const int y = (int)((idx / W) % H);
+    const int b = (int)(idx / ((long long)W * H));
+    out[idx] = tta_combine_pixel(d, b, nh, nw, Hp, Wp, pad_h, pad_w, y, x);
+}
+
+// ragged twin: image b at its own desc[b] size, padding and place; grid (max h * max w, B)
+__global__ void __launch_bounds__(256) tta_combine_ragged_kernel(const float *__restrict__ d, int nh, int nw, float *__restrict__ out,
+                                                                 const dm_ragged_image *__restrict__ desc) {
+    const int b = blockIdx.y;
+    const dm_ragged_image r = desc[b];
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= (long long)r.h * r.w) return;
+    const int pad_h = zoe_pad_of(r.h), pad_w = zoe_pad_of(r.w);
+    out[r.offset + idx] = tta_combine_pixel(d, b, nh, nw, r.h + 2 * pad_h, r.w + 2 * pad_w, pad_h, pad_w, (int)(idx / r.w), (int)(idx % r.w));
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -646,6 +702,30 @@ DM_EXPORT int dm_zoe_preprocess_patchify(const uint8_t *rgb, int B, int H, int W
     return DM_OK;
 }
 
+DM_EXPORT int dm_zoe_preprocess_patchify_ragged(const uint8_t *packed, long long size, const dm_ragged_image *desc_host,
+                                                const dm_ragged_image *desc_dev, int B, int net_h, int net_w, int patch, void *out, int kpad,
+                                                void *stream_) {
+    using namespace dm;
+    const char *who = "dm_zoe_preprocess_patchify_ragged";
+    const int rc = check_ragged(who, packed, size, desc_host, desc_dev, B, 3, nullptr, nullptr);
+    if (rc) return rc;
+    if (!out || patch <= 0 || net_h <= 0 || net_w <= 0 || net_h % patch || net_w % patch || kpad != 3 * patch * patch) {
+        set_error("%s: bad arguments (kpad = 3*patch^2)", who); return DM_E_INVALID;
+    }
+    for (int i = 0; i < B; ++i) {
+        if (zoe_pad_of(desc_host[i].h) >= desc_host[i].h || zoe_pad_of(desc_host[i].w) >= desc_host[i].w) {
+            set_error("%s: image %d (%d x %d) is smaller than its reflect padding", who, i, desc_host[i].h, desc_host[i].w); return DM_E_INVALID;
+        }
+    }
+    ZoePre p;
+    p.rgb = packed; p.ragged = desc_dev; p.B = B; p.H = p.W = p.pad_h = p.pad_w = 0; p.nh = net_h; p.nw = net_w; p.patch = patch;
+    p.gh = net_h / patch; p.gw = net_w / patch; p.kpad = kpad; p.out = (__half *)out;
+    const long long total = (long long)2 * B * net_h * net_w;
+    zoe_preprocess_patchify_ragged_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream_>>>(p);
+    DM_LAUNCH_CHECK("zoe_preprocess_patchify_ragged_kernel");
+    return DM_OK;
+}
+
 DM_EXPORT int dm_layernorm_post_f16(float *x, long long rows, int C, const float *gamma, const float *beta, float eps, void *out, void *stream_) {
     using namespace dm;
     if (C != 128) { set_error("dm_layernorm_post_f16: width must be 128 (router embedding)"); return DM_E_UNSUPPORTED; }
@@ -727,6 +807,19 @@ DM_EXPORT int dm_zoe_tta_combine(const float *d, int B, int nh, int nw, int pad_
     const long long total = (long long)B * H * W;
     tta_combine_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream_>>>(d, B, nh, nw, H + 2 * pad_h, W + 2 * pad_w, pad_h, pad_w, H, W, out);
     DM_LAUNCH_CHECK("tta_combine_kernel");
+    return DM_OK;
+}
+
+DM_EXPORT int dm_zoe_tta_combine_ragged(const float *d, int B, int nh, int nw, float *out, long long size, const dm_ragged_image *desc_host,
+                                        const dm_ragged_image *desc_dev, void *stream_) {
+    using namespace dm;
+    int mh = 0, mw = 0;
+    const int rc = check_ragged("dm_zoe_tta_combine_ragged", out, size, desc_host, desc_dev, B, 1, &mh, &mw);
+    if (rc) return rc;
+    if (!d || nh <= 0 || nw <= 0 || B > 65535) { set_error("dm_zoe_tta_combine_ragged: bad arguments"); return DM_E_INVALID; }
+    const dim3 grid((unsigned)(((long long)mh * mw + 255) / 256), (unsigned)B);
+    tta_combine_ragged_kernel<<<grid, 256, 0, (cudaStream_t)stream_>>>(d, nh, nw, out, desc_dev);
+    DM_LAUNCH_CHECK("tta_combine_ragged_kernel");
     return DM_OK;
 }
 

@@ -91,6 +91,24 @@ def _vec(b, n=None):
     return t
 
 
+def _ragged_net_size(engine, desc, net_w, net_h):
+    """the one network input size of a ragged batch (desc: _lib.Ragged of its images); ValueError if the images do not share one"""
+    net_h = net_h if net_h is not None else net_w
+    nets = {engine.net_size(w, h, net_w, net_h) for h, w in desc.sizes}
+    if len(nets) != 1:
+        raise ValueError(f"a ragged batch must share one network input size; these images map to {sorted(nets)}")
+    return nets.pop()
+
+
+def _resize_ragged(engine, d, B, nh, nw, desc, mode):
+    """the final resize of a ragged batch: d fp32 [B, nh, nw] -> packed fp32, image i at desc.sizes[i] (layout _lib.Ragged(sizes, 1))"""
+    import torch
+    out_desc = _lib.Ragged(desc.sizes, 1, engine.device)
+    out = torch.empty(out_desc.size, dtype=torch.float32, device=engine.device)
+    engine.ops.call("dm_resize_f32_ragged", d, B, nh, nw, out, out_desc.size, out_desc.host.ctypes.data, out_desc.dev, mode)
+    return out
+
+
 class SplitWeight:
     """A GEMM / conv operand of the split (fp32-class) path: `t` fp16 [N, 3K], `scale` fp32 [N] (see split_weight)."""
 
@@ -353,6 +371,19 @@ class DepthAnythingV2Engine:
         out = torch.empty(B, oh, ow, dtype=torch.float32, device=self.device)
         self.ops.call("dm_resize_f32", d, B, nh, nw, out, oh, ow, self.FINAL_RESIZE_MODE)
         return out
+
+    def forward_ragged(self, packed, desc, net_w, net_h=None):
+        """Ragged batch: uint8 CUDA images packed back to back (desc: their _lib.Ragged, unit 3) that share one net size -> fp32 CUDA
+        predictions packed the same way (_lib.Ragged(desc.sizes, 1)).  Image i's prediction equals forward_batch of that image alone:
+        only the pre-processing and the final resize see the image sizes, and the network runs under the uniform batch's graph key."""
+        nw, nh = _ragged_net_size(self, desc, net_w, net_h)
+        B, P_ = desc.B, self.PATCH
+        b = self._buffers(B, nh, nw)
+        self.ops.call("dm_preprocess_patchify_ragged", *desc.args(packed), nh, nw, P_, (ctypes.c_float * 3)(*self.MEAN),
+                      (ctypes.c_float * 3)(*self.STD), (ctypes.c_int * 3)(*self.CHAN_MAP), int(self.split), b['patches'], self.kpad,
+                      launches=1 + (self.kpad > 3 * P_ * P_))
+        d = self._graphs.run((B, nh, nw), lambda: self._network(b, B, nh, nw))
+        return _resize_ragged(self, d, B, nh, nw, desc, self.FINAL_RESIZE_MODE)
 
     def _network(self, b, B, nh, nw):
         """patch matrix in b['patches'] -> the net-size prediction b['d']"""
@@ -924,6 +955,23 @@ class LeresEngine(_ResNeXtEngine):
             self.ops.call("dm_resize_f32", dn, B, 2 * hh, 2 * ww, out, oh, ow, 1)   # cv2.INTER_CUBIC (A = -0.75, replicated borders)
         return out
 
+    def net_size(self, W, H, net_w, net_h):
+        return net_w, net_h           # estimateleres resizes every image to the net size
+
+    def forward_ragged(self, packed, desc, net_w, net_h=None):
+        """Ragged batch (DepthAnythingV2Engine.forward_ragged): every image at (net_w, net_h), cv2.INTER_CUBIC back to its own size"""
+        net_w, net_h = _ragged_net_size(self, desc, net_w, net_h)
+        if net_w % 32 or net_h % 32:
+            raise ValueError("LeReS needs a net size that is a multiple of 32")
+        self._trim_pools()
+        B = desc.B
+        cols = self._stem_cols(B, net_h, net_w)
+        self.ops.call("dm_leres_stem_im2col_ragged" + self._cv, *desc.args(packed), net_h, net_w, (ctypes.c_float * 3)(*self.MEAN),
+                      (ctypes.c_float * 3)(*self.STD), cols)
+        dn = self._network(B, net_h, net_w, cols)
+        # the uniform path copies a prediction already at the image size; the bicubic resize at scale 1 reproduces it exactly
+        return _resize_ragged(self, dn, B, net_h, net_w, desc, 1)
+
     def forward_crops(self, planar, rects, net):
         """BOOST's patch batch: estimateleres' network on B crops of one planar fp32 image ([3, Hi, Wi], rects = [(x0, y0, w, h)]), all at the
         same square net size -> fp32 [B, net, net] (a pooled buffer, valid until the next call at this (B, net)); the caller does the
@@ -1059,6 +1107,17 @@ class MidasV21Engine(_MidasBoost, _ResNeXtEngine):
         self.ops.call("dm_resize_f32", d, B, nh, nw, out, oh, ow, 1)     # F.interpolate(bicubic, align_corners=False)
         return out
 
+    def forward_ragged(self, packed, desc, net_w, net_h=None):
+        """Ragged batch (DepthAnythingV2Engine.forward_ragged)"""
+        nw, nh = _ragged_net_size(self, desc, net_w, net_h)
+        self._trim_pools()
+        B = desc.B
+        cols = self._stem_cols(B, nh, nw)
+        m, s, c = (ctypes.c_float * 3)(*self.MEAN), (ctypes.c_float * 3)(*self.STD), (ctypes.c_int * 3)(*self.CHAN_MAP)
+        self.ops.call("dm_midas_stem_im2col_ragged" + self._cv, *desc.args(packed), nh, nw, m, s, c, cols)
+        d = self._network(B, nh, nw, cols)
+        return _resize_ragged(self, d, B, nh, nw, desc, 1)
+
     def _crops_network(self, planar, hi, wi, r, B, nh, nw):
         self._trim_pools()          # each crop group is a forward of its own
         cols = self._stem_cols(B, nh, nw)
@@ -1107,6 +1166,11 @@ def _nbytes(obj):
     if isinstance(obj, (list, tuple)):
         return sum(_nbytes(v) for v in obj)
     return obj.numel() * obj.element_size() if hasattr(obj, "element_size") else 0
+
+
+def _zoe_pads(H, W):
+    """DepthModel.infer_pil's reflect pad of an H x W image (depth_model.py:80-82, fh = fw = 3)"""
+    return int(np.sqrt(H / 2) * 3.0), int(np.sqrt(W / 2) * 3.0)
 
 
 def _zoe_lin(sd, dev, key, rows=None):
@@ -1199,15 +1263,41 @@ class _ZoeDepthBase(DptBeitEngine):
         import torch
         if planar is not None:
             return self.forward_crops(planar[0], [planar[1]], net_w)[0].unsqueeze(0)
-        ops, z, P, RELU = self.ops, self.z, self.PROJ, _lib.ACT_RELU
+        ops = self.ops
         B, H, W, _ = rgb.shape
         net_h = net_h if net_h is not None else net_w
-        pad_h, pad_w = int(np.sqrt(H / 2) * 3.0), int(np.sqrt(W / 2) * 3.0)       # depth_model.py:80-82 (fh = fw = 3)
-        Hp, Wp = H + 2 * pad_h, W + 2 * pad_w
-        nw, nh = midas_net_size(Wp, Hp, net_w, net_h)                               # PrepForMidas: keep aspect, x32, "minimal"
+        pad_h, pad_w = _zoe_pads(H, W)
+        nw, nh = self.net_size(W, H, net_w, net_h)
         F = 2 * B
         b = self._buffers(F, nh, nw)
         ops.call("dm_zoe_preprocess_patchify", rgb, B, H, W, pad_h, pad_w, nh, nw, self.PATCH, b['patches'], self.kpad)
+        zb = self._zoe_network(b, F, nh, nw)
+        out = torch.empty(B, H, W, dtype=torch.float32, device=self.device)
+        ops.call("dm_zoe_tta_combine", zb['d'], B, nh, nw, pad_h, pad_w, H, W, out)
+        return out
+
+    def net_size(self, W, H, net_w, net_h):
+        """PrepForMidas (keep aspect, x32, "minimal") of the reflect-padded image"""
+        pad_h, pad_w = _zoe_pads(H, W)
+        return midas_net_size(W + 2 * pad_w, H + 2 * pad_h, net_w, net_h)
+
+    def forward_ragged(self, packed, desc, net_w, net_h=None):
+        """Ragged batch (DepthAnythingV2Engine.forward_ragged): each image with its own reflect pad and flip, one forward of 2B"""
+        import torch
+        nw, nh = _ragged_net_size(self, desc, net_w, net_h)
+        B = desc.B
+        F = 2 * B
+        b = self._buffers(F, nh, nw)
+        self.ops.call("dm_zoe_preprocess_patchify_ragged", *desc.args(packed), nh, nw, self.PATCH, b['patches'], self.kpad)
+        zb = self._zoe_network(b, F, nh, nw)
+        out_desc = _lib.Ragged(desc.sizes, 1, self.device)
+        out = torch.empty(out_desc.size, dtype=torch.float32, device=self.device)
+        self.ops.call("dm_zoe_tta_combine_ragged", zb['d'], B, nh, nw, out, out_desc.size, out_desc.host.ctypes.data, out_desc.dev)
+        return out
+
+    def _zoe_network(self, b, F, nh, nw):
+        """patch matrix of the F = 2B forwards in b['patches'] -> the head's buffers, the net-size metric depth in zb['d']"""
+        ops, z, P, RELU = self.ops, self.z, self.PROJ, _lib.ACT_RELU
         self.run_network(b, F, nh, nw)
         zb, Fp = b['z'], self.Fp
         # out_conv activation (MidasCore hooks output_conv[3], the 32-channel ReLU)
@@ -1233,9 +1323,7 @@ class _ZoeDepthBase(DptBeitEngine):
         # conditional log-binomial + expectation, then un-pad / un-flip / average (depth_model.py:88-129)
         ops.gemm(zb['bemb'][3], 128, z['clb'][0], 128, F * hp * wp, 128, 128, epi=_lib.EPI_STORE_F32, X=zb['ze'], ldx=128)
         self.log_binomial(zb, bprev, F, nh, nw, hp, wp)
-        out = torch.empty(B, H, W, dtype=torch.float32, device=self.device)
-        ops.call("dm_zoe_tta_combine", zb['d'], B, nh, nw, pad_h, pad_w, H, W, out)
-        return out
+        return zb
 
     def forward_crops(self, planar, rects, msize):
         """BOOST's estimates: singleestimate's ZoeDepth branch (src/depthmap_generation.py:1062-1064, estimatezoedepth :443-452) on
@@ -1639,6 +1727,39 @@ class ModelHolder:
         else:
             raise NotImplementedError(f"model_type {self.depth_model_type}")
         return pred, self.depth_model_type in [0, 7, 8, 9, 10]
+
+    def net_size(self, w, h, net_w, net_h):
+        """the network input size (width, height) the loaded depth model gives a w x h image for the requested net size: images
+        that share it can run as one ragged batch (get_raw_prediction_ragged)"""
+        if self.depth_model is None:
+            raise RuntimeError("no depth model loaded; call ensure_models first")
+        return tuple(self.depth_model.net_size(int(w), int(h), net_w, net_h))
+
+    def get_raw_prediction_ragged(self, images, net_width, net_height):
+        """list of uint8 CUDA [Hi, Wi, 3] images of any sizes -> (list of float32 CUDA [Hi, Wi] in input order, invert flag).  The images
+        are grouped by network input size, one forward per group; each result equals get_raw_prediction_batch of that image alone.
+        With BOOST loaded each image runs through the BOOST pipeline on its own, as in get_raw_prediction_batch."""
+        import torch
+        if self.depth_model is None:
+            raise RuntimeError("no depth model loaded; call ensure_models first")
+        for t in images:
+            if not torch.is_tensor(t) or t.dtype != torch.uint8 or t.dim() != 3 or t.shape[-1] != 3 or t.shape[0] < 1 or t.shape[1] < 1:
+                raise ValueError("every image must be a uint8 tensor [H,W,3]")      # the kernels read the tensors' memory as such
+        invert = self.depth_model_type in [0, 7, 8, 9, 10]
+        if self.pix2pix_model is not None:
+            return [self.pix2pix_model.run(t.cpu().numpy(), self.boost_rmax, to_host=False) for t in images], invert
+        dev = self.depth_model.device
+        groups = {}
+        for i, t in enumerate(images):
+            groups.setdefault(self.net_size(t.shape[1], t.shape[0], net_width, net_height), []).append(i)
+        out = [None] * len(images)
+        for idx in groups.values():
+            desc = _lib.Ragged([tuple(images[i].shape[:2]) for i in idx], 3, dev)
+            packed = torch.cat([images[i].to(dev).reshape(-1) for i in idx])
+            pred = self.depth_model.forward_ragged(packed, desc, net_width, net_height)
+            for i, p in zip(idx, _lib.Ragged(desc.sizes, 1, None).split(pred)):
+                out[i] = p
+        return out, invert
 
     def get_raw_prediction(self, input, net_width, net_height):
         """Get prediction from the model currently loaded by the ModelHolder object (reference :375-403)."""
