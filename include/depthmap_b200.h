@@ -439,6 +439,29 @@ int dm_resize_f32_ragged(const float *in, int B, int Hin, int Win, float *out, l
 int dm_zoe_tta_combine_ragged(const float *d, int B, int nh, int nw, float *out, long long size, const dm_ragged_image *desc_host,
                               const dm_ragged_image *desc_dev, void *stream);
 
+/* ---------------------------------------------------------------------------------------------------------------
+ * P1 — PNG encoding: B images on the device -> B finished PNG files, packed back to back in `out`; file i is
+ * out[offsets[i] .. offsets[i + 1]) (offsets: DEVICE int64 [B + 1], written by the call).
+ *   replaces  PIL's Image.save(format='png') of the funnel's outputs (src/backbone.py:91-101) and its host-side formatting
+ * img: uint16 [B][H][W] (C = 1, bit_depth = 16: 16-bit greyscale, samples stored big-endian in the file) or uint8 [B][H][W][3]
+ * (C = 3, bit_depth = 8: RGB).  flags: DM_PNG_INVERT XORs every 16-bit sample with 0xFFFF (OUTPUT_DEPTH_INVERT's np.bitwise_not).
+ * Each row gets one PNG filter (0-4, minimum sum of absolute signed bytes).  The filtered stream is cut into 32 KiB segments,
+ * each deflated by one CTA with its own dynamic Huffman code, the fixed code or a stored block, whichever is smallest; every
+ * segment but the last ends with an empty stored block (00 00 FF FF), and each segment is one IDAT chunk.  A file depends on its
+ * image alone, not on the batch, the call or the device.
+ * dm_png_encode_bound: the largest file of one H x W image (0 for an unsupported format); out_capacity must be at least
+ * B * bound and workspace_bytes at least dm_png_encode_workspace_bytes, else DM_E_WORKSPACE with nothing written.
+ * ------------------------------------------------------------------------------------------------------------- */
+enum { DM_PNG_INVERT = 1 };
+size_t dm_png_encode_bound(int H, int W, int C, int bit_depth);
+size_t dm_png_encode_workspace_bytes(int B, int H, int W, int C, int bit_depth);
+int dm_png_encode(const void *img, int B, int H, int W, int C, int bit_depth, int flags, uint8_t *out, size_t out_capacity,
+                  int64_t *offsets, void *workspace, size_t workspace_bytes, void *stream);
+/* OUTPUT_DEPTH_COMBINE (src/core.py:52-58, :289-293): rgb uint8 [B][H][W][3] and depth uint16 [B][H][W] (XOR 0xFFFF when
+ * invert) -> uint8 RGB [B][H][2W][3] (horizontal = 1) or [B][2H][W][3]: the image, then depth >> 8 on all three channels */
+int dm_depth_combine_rgb(const uint8_t *rgb, const uint16_t *depth, int B, int H, int W, int horizontal, int invert, uint8_t *out,
+                         void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -16,6 +16,7 @@ DM_DEPTH_U16, DM_DEPTH_ND64 = 0, 1
 DM_FILL = {"none": 0, "naive": 1, "naive_interpolating": 2, "polylines_soft": 3, "polylines_sharp": 4}
 DM_EYE_WARP, DM_EYE_IDENTITY, DM_EYE_SKIP = 0, 1, 2
 DM_PACK_STRIDED, DM_PACK_ANAGLYPH = 0, 1
+DM_PNG_INVERT = 1
 
 
 class StereoParams(ctypes.Structure):
@@ -84,6 +85,7 @@ EXPORTS = [
     "dm_layernorm_split", "dm_resize_bilinear_nhwc_split",
     "dm_preprocess_patchify_ragged", "dm_leres_stem_im2col_ragged", "dm_leres_stem_im2col_ragged_circular", "dm_midas_stem_im2col_ragged",
     "dm_midas_stem_im2col_ragged_circular", "dm_zoe_preprocess_patchify_ragged", "dm_resize_f32_ragged", "dm_zoe_tta_combine_ragged",
+    "dm_png_encode_bound", "dm_png_encode_workspace_bytes", "dm_png_encode", "dm_depth_combine_rgb",
 ]
 
 
@@ -221,6 +223,13 @@ def _bind_optional(L):
         L.dm_zoe_clb_single.argtypes = [vp, i32, vp, i32, vp, vp, vp, vp, vp, vp, f32, i32, i32, i32, i32, i32, f32, f32, vp, vp]
     if hasattr(L, "dm_resize_f32_ragged"):
         _bind_ragged(L)
+    if hasattr(L, "dm_png_encode"):
+        L.dm_png_encode_bound.argtypes = [i32, i32, i32, i32]
+        L.dm_png_encode_bound.restype = sz
+        L.dm_png_encode_workspace_bytes.argtypes = [i32, i32, i32, i32, i32]
+        L.dm_png_encode_workspace_bytes.restype = sz
+        L.dm_png_encode.argtypes = [vp, i32, i32, i32, i32, i32, i32, vp, sz, vp, vp, sz, vp]
+        L.dm_depth_combine_rgb.argtypes = [vp, vp, i32, i32, i32, i32, i32, vp, vp]
 
 
 def _bind_ragged(L):

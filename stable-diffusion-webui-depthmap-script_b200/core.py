@@ -258,14 +258,14 @@ def _group_key(holder, inp, image, custom, boost):
     return ("net", req, holder.net_size(image.width, image.height, *req))
 
 
-def _process_chunk(holder, inp, dev, images, depthmaps, idxs):
-    """One batch of images with one group key through every requested stage on the device; returns per-image host results.  A
-    batch of one pixel size runs as one uniform batch; a mixed one predicts as one ragged batch, then runs the later stages per
+def _process_chunk(holder, inp, dev, images, depthmaps, idxs, finish):
+    """One batch of images with one group key through every requested stage on the device; returns `finish`'s per-image results.
+    A batch of one pixel size runs as one uniform batch; a mixed one predicts as one ragged batch, then runs the later stages per
     run of equally sized images."""
     import torch
     rgbs = [np.asarray(images[i].convert('RGB') if images[i].mode != 'RGB' else images[i]) for i in idxs]
     if len({r.shape for r in rgbs}) == 1:
-        return _process_run(holder, inp, dev, images, depthmaps, idxs, rgbs, None)
+        return _process_run(holder, inp, dev, images, depthmaps, idxs, rgbs, None, finish)
     # one host -> device copy: the packed images
     layout = _lib.Ragged([r.shape[:2] for r in rgbs], 3, None)
     packed = torch.from_numpy(np.concatenate([r.reshape(-1) for r in rgbs])).to(dev, non_blocking=True)
@@ -278,14 +278,14 @@ def _process_chunk(holder, inp, dev, images, depthmaps, idxs):
         while k < len(idxs) and rgbs[k].shape == rgbs[j].shape:
             k += 1
         out += _process_run(holder, inp, dev, images, depthmaps, idxs[j:k], rgbs[j:k],
-                            (torch.stack(imgs[j:k]), torch.stack(preds[j:k]), invert))
+                            (torch.stack(imgs[j:k]), torch.stack(preds[j:k]), invert), finish)
         j = k
     return out
 
 
-def _process_run(holder, inp, dev, images, depthmaps, idxs, rgbs, predicted):
+def _process_run(holder, inp, dev, images, depthmaps, idxs, rgbs, predicted, finish):
     """Equally sized images through every requested stage; `predicted` = (rgb batch, prediction batch, invert) when the depth model
-    already ran on them."""
+    already ran on them.  `finish` turns the device results into per-image results (_HostImages or _PngFiles)."""
     import torch
     custom = depthmaps[idxs[0]] is not None
     preds = flags = None
@@ -317,21 +317,81 @@ def _process_run(holder, inp, dev, images, depthmaps, idxs, rgbs, predicted):
             inp[go.NORMALMAP_SOBEL_KERNEL] if inp[go.NORMALMAP_SOBEL] else None,
             inp[go.NORMALMAP_POST_BLUR_KERNEL] if inp[go.NORMALMAP_POST_BLUR] else None,
             inp[go.NORMALMAP_INVERT])
-    # one device -> host transfer per tensor per batch
-    depth_h = depth_u16.cpu().numpy()
-    preds_h = preds.cpu().numpy() if preds is not None else None
-    flags_h = flags.cpu().numpy() if flags is not None else None
-    stereo_h = [s.cpu().numpy() for s in stereo] if stereo is not None else None
-    normal_h = normal.cpu().numpy() if normal is not None else None
-    out = []
-    for j in range(len(idxs)):
-        out.append((rgbs[j], depth_h[j], None if preds_h is None else (preds_h[j], invert, int(flags_h[j])),
-                    None if stereo_h is None else [s[j] for s in stereo_h],
-                    None if normal_h is None else normal_h[j]))
-    return out
+    # the prediction crosses to the host only when it is yielded
+    want_pred = preds is not None and inp[go.DO_OUTPUT_DEPTH_PREDICTION]
+    preds_h = preds.cpu().numpy() if want_pred else None
+    flags_h = flags.cpu().numpy() if want_pred else None
+    pred_of = lambda j: None if preds_h is None else (preds_h[j], invert, int(flags_h[j]))
+    return finish.run(inp, rgbs, rgb_t, depth_u16, pred_of, stereo, normal)
+
+
+class _HostImages:
+    """core_generation_funnel's results: one device -> host transfer per tensor per batch, PIL images made as they are yielded"""
+
+    @staticmethod
+    def run(inp, rgbs, rgb_t, depth_u16, pred_of, stereo, normal):
+        depth_h = depth_u16.cpu().numpy()
+        stereo_h = [s.cpu().numpy() for s in stereo] if stereo is not None else None
+        normal_h = normal.cpu().numpy() if normal is not None else None
+        return [(rgbs[j], depth_h[j], pred_of(j), None if stereo_h is None else [s[j] for s in stereo_h],
+                 None if normal_h is None else normal_h[j]) for j in range(len(rgbs))]
+
+    @staticmethod
+    def depth(inp, rgb, img_output):
+        img_depth = np.bitwise_not(img_output) if inp[go.OUTPUT_DEPTH_INVERT] else img_output
+        if inp[go.OUTPUT_DEPTH_COMBINE]:
+            axis = 1 if inp[go.OUTPUT_DEPTH_COMBINE_AXIS] == 'Horizontal' else 0
+            return Image.fromarray(np.concatenate((rgb, convert_i16_to_rgb(img_depth, rgb)), axis=axis))
+        return Image.fromarray(img_depth)
+
+    @staticmethod
+    def image(x):
+        return Image.fromarray(x)
+
+
+class _PngFiles:
+    """core_generation_funnel_png's results: every image kind encoded to PNG on the device (invert and combine folded in), so only
+    the compressed files cross to the host"""
+
+    @staticmethod
+    def run(inp, rgbs, rgb_t, depth_u16, pred_of, stereo, normal):
+        from .png import combine_depth_rgb, encode_png_batch
+        n = len(rgbs)
+        depth = [None] * n
+        if inp[go.DO_OUTPUT_DEPTH]:
+            invert = bool(inp[go.OUTPUT_DEPTH_INVERT])
+            if inp[go.OUTPUT_DEPTH_COMBINE]:
+                horizontal = inp[go.OUTPUT_DEPTH_COMBINE_AXIS] == 'Horizontal'
+                depth = encode_png_batch(combine_depth_rgb(rgb_t, depth_u16, horizontal, invert))
+            else:
+                depth = encode_png_batch(depth_u16, invert=invert)
+        stereo_png = [encode_png_batch(s) for s in stereo] if stereo is not None else None
+        normal_png = encode_png_batch(normal) if normal is not None else None
+        return [(rgbs[j], depth[j], pred_of(j), None if stereo_png is None else [s[j] for s in stereo_png],
+                 None if normal_png is None else normal_png[j]) for j in range(n)]
+
+    @staticmethod
+    def depth(inp, rgb, png):
+        return png
+
+    @staticmethod
+    def image(png):
+        return png
 
 
 def core_generation_funnel(outpath, inputimages, inputdepthmaps, inputnames, inp, ops=None):
+    return _funnel(outpath, inputimages, inputdepthmaps, inputnames, inp, ops, _HostImages)
+
+
+def core_generation_funnel_png(outpath, inputimages, inputdepthmaps, inputnames, inp, ops=None):
+    """core_generation_funnel with every image result as the bytes of a PNG file, encoded on the device (png.encode_png_batch):
+    the same batching, options and (input_index, kind) sequence; `depth` (16-bit greyscale), `concat_depth`, every stereo mode and
+    `normalmap` (8-bit RGB) are PNG bytes whose pixels equal the PIL image core_generation_funnel yields; `depth_prediction` is the
+    same float array."""
+    return _funnel(outpath, inputimages, inputdepthmaps, inputnames, inp, ops, _PngFiles)
+
+
+def _funnel(outpath, inputimages, inputdepthmaps, inputnames, inp, ops, out_kind):
     if len(inputimages) == 0 or inputimages[0] is None:
         return
     if inputdepthmaps is None or len(inputdepthmaps) == 0:
@@ -375,7 +435,7 @@ def core_generation_funnel(outpath, inputimages, inputdepthmaps, inputnames, inp
                     break
                 idxs.append(idxs[-1] + 1)
                 largest = grown
-            results = _process_chunk(holder, inp, dev, inputimages, inputdepthmaps, idxs)
+            results = _process_chunk(holder, inp, dev, inputimages, inputdepthmaps, idxs, out_kind)
             # yield in the reference's order (src/core.py:194-305)
             for i, (rgb, img_output, pred, stereo, normal) in zip(idxs, results):
                 if pred is not None and inp[go.DO_OUTPUT_DEPTH_PREDICTION] and not pred[2]:
@@ -384,18 +444,12 @@ def core_generation_funnel(outpath, inputimages, inputdepthmaps, inputnames, inp
                         p *= -1
                     yield i, 'depth_prediction', p
                 if inp[go.DO_OUTPUT_DEPTH]:
-                    img_depth = np.bitwise_not(img_output) if inp[go.OUTPUT_DEPTH_INVERT] else img_output
-                    if inp[go.OUTPUT_DEPTH_COMBINE]:
-                        axis = 1 if inp[go.OUTPUT_DEPTH_COMBINE_AXIS] == 'Horizontal' else 0
-                        yield i, 'concat_depth', Image.fromarray(
-                            np.concatenate((rgb, convert_i16_to_rgb(img_depth, rgb)), axis=axis))
-                    else:
-                        yield i, 'depth', Image.fromarray(img_depth)
+                    yield i, 'concat_depth' if inp[go.OUTPUT_DEPTH_COMBINE] else 'depth', out_kind.depth(inp, rgb, img_output)
                 if stereo is not None:
                     for c in range(len(stereo)):
-                        yield i, modes[c], Image.fromarray(stereo[c])
+                        yield i, modes[c], out_kind.image(stereo[c])
                 if normal is not None:
-                    yield i, 'normalmap', Image.fromarray(normal)
+                    yield i, 'normalmap', out_kind.image(normal)
             count = idxs[-1] + 1
     except Exception as e:
         if 'out of memory' in str(e).lower():

@@ -27,7 +27,7 @@ UNITS = [
     ("normalmap.cu", ["-fmad=false"]),
     ("stereo.cu", ["-fmad=false"]),
 ]
-for _extra in ("vit_kernels.cu", "gemm_wgmma.cu", "attention_wgmma.cu", "zoe_kernels.cu", "leres_kernels.cu", "midas_kernels.cu", "boost_kernels.cu", "pos_tables.cu"):
+for _extra in ("vit_kernels.cu", "gemm_wgmma.cu", "attention_wgmma.cu", "zoe_kernels.cu", "leres_kernels.cu", "midas_kernels.cu", "boost_kernels.cu", "pos_tables.cu", "png_encode.cu"):
     if os.path.exists(os.path.join(HERE, _extra)):
         UNITS.append((_extra, []))
 
